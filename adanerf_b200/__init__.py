@@ -1,4 +1,4 @@
-"""adanerf_b200 -- B200-native (sm_100a) AdaNeRF inference renderer: hand-written CUDA kernels behind a
+"""adanerf_b200 -- H100-native (sm_90a) AdaNeRF inference renderer: hand-written CUDA kernels behind a
 C ABI (include/adanerf_b200.h), driven from Python through ctypes.  No CPU fallback."""
 from ._lib import AdnError, LIB_PATH, load_library  # noqa: F401
 from .renderer import Renderer, make_scene, render  # noqa: F401

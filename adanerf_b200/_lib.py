@@ -6,7 +6,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("ADN_LIB_PATH") or os.path.join(_HERE, "libadanerf_b200.so")   # override: A/B builds
 
-STATUS_TEXT = {0: "ok", 1: "invalid argument", 2: "CUDA error", 3: "no usable sm_100 device",
+STATUS_TEXT = {0: "ok", 1: "invalid argument", 2: "CUDA error", 3: "no usable sm_90 device",
                4: "weights not set", 5: "I/O error", 6: "device watchdog tripped"}
 
 

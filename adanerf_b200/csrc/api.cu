@@ -1,4 +1,4 @@
-// C ABI + host-side context of the B200 AdaNeRF renderer (see include/adanerf_b200.h).
+// C ABI + host-side context of the H100 AdaNeRF renderer (see include/adanerf_b200.h).
 #include <cuda_runtime.h>
 
 #include <cmath>
@@ -11,7 +11,7 @@
 
 #include "../../include/adanerf_b200.h"
 #include "export_loader.h"
-#include "mlp_umma.cuh"
+#include "mlp.cuh"
 #include "ptx.cuh"
 #include "stages.cuh"
 
@@ -26,8 +26,7 @@ struct HostTensor {
 
 struct Net {
   bool ready = false;
-  bool sh = false;   // shading net packed for mlp_sh_kernel (N half outermost weights, fixed side layout)
-  int nsplit = 1, ng = 1;
+  int nsplit = 1;
   int n_in = 0, n_out = 0;
   MlpProgram prog{};
   InputLayout lay{};
@@ -44,7 +43,7 @@ struct Buf {
 
 struct adn_ctx {
   int device = 0;
-  int num_sms = 148;
+  int num_sms = 132;
   adn_scene scene{};
   SceneDev sc{};
   float* d_zlut = nullptr;        // [128] world depth of the cell centres (log warp)
@@ -53,19 +52,15 @@ struct adn_ctx {
   Net net[2];
   int mlp0_terms = 3;
   int n_feat0 = 90;               // sampling-net input features: 6 + 6 (n_freq_pos0 + n_freq_dir0)
-  bool fuse_encoder = false;      // stage 3 inside the shading kernel (encoder warp): saves the 1.3 GB tile buffer, measured 5 % slower
-  bool sh_kernel = true;          // shading net on mlp_sh_kernel (needs CTA pairs, no fused encoder); false: mlp_umma_kernel<1,2,.>
-  int cta_group = 2;              // MLP kernels: 2 = CTA pairs (cta_group::2 MMAs), 1 = single CTA
+  bool fuse_encoder = false;      // stage 3 inside the shading kernel: saves the [M, 90]-sized tile buffer
   int64_t chunk_rays = 0;
   bool profile = false;
   int weight_copies = 1;   // replicas of each packed weight blob (MlpProgram::w_copies)
   // scratch
-  Buf tiles0, raw0, x0, ray_o, ray_d, dirs, count, offset, rayidx, zbuf, zpbuf, tiles1, raw1, s2scratch, rgb, rgba, x1, metric, enc_scratch;
+  Buf tiles0, raw0, x0, ray_o, ray_d, dirs, count, offset, rayidx, zbuf, zpbuf, tiles1, raw1, s2scratch, rgb, rgba, x1, metric;
   long long* d_total = nullptr;
   int* d_err = nullptr;           // device view of h_err
   int* h_err = nullptr;           // watchdog flag in mapped pinned host memory: still readable after a device trap
-  long long* d_trace = nullptr;   // debug timeline of the MLP kernels (option "trace")
-  int trace_net = -1;
   // pinned staging for the *_host entry points
   Stage2Sync s2sync;              // epoch / ticket base of s2scratch (no per-launch memset)
   Buf h_in, h_out, h_ns;
@@ -81,7 +76,7 @@ struct adn_ctx {
 
 namespace {
 
-const char* kStatusText[] = {"ok", "invalid argument", "CUDA error", "no usable sm_100 device", "weights not set",
+const char* kStatusText[] = {"ok", "invalid argument", "CUDA error", "no usable sm_90 device", "weights not set",
                              "I/O error", "device watchdog tripped"};
 
 adn_status fail(adn_ctx* ctx, adn_status s, const std::string& msg) {
@@ -150,19 +145,13 @@ struct Seg {
   int col0, valid;
 };
 
-// Packs one layer's weights W [n_out, k_in] into the ring-stage stream: for each K block (Seg), for each
-// 128-row N half: a [128 x 64] K-major SWIZZLE_128B bf16 tile (hi), followed by the lo tile when nsplit == 2.
-void pack_layer(const float* W, int n_out, int k_in, const std::vector<Seg>& segs, int nsplit, std::vector<uint8_t>& blob,
-                bool nh_outer_bf16 = false) {
+// Packs one layer's weights W [n_out, k_in] into the ring-stage stream, in the order the MLP kernel consumes it: for each
+// 128-row N half, for each K block (Seg): a [128 x 64] K-major SWIZZLE_128B bf16 tile (hi), followed by the lo tile when
+// nsplit == 2.
+void pack_layer(const float* W, int n_out, int k_in, const std::vector<Seg>& segs, int nsplit, std::vector<uint8_t>& blob) {
   const int n_half = (n_out + 127) / 128;
-  // stage order = consumption order: the half-pipelined kernels (split-precision sampling net, mlp_sh_kernel) walk N half
-  // outermost (half 0's accumulator completes first), mlp_umma_kernel K block outermost (both halves of a K block form one stage)
-  const bool nh_outer = (nsplit == 2) || nh_outer_bf16;
-  const int n_seg = int(segs.size());
-  for (int o = 0; o < (nh_outer ? n_half : n_seg); ++o) {
-    for (int i = 0; i < (nh_outer ? n_seg : n_half); ++i) {
-      const int nh = nh_outer ? o : i;
-      const Seg& sg = segs[nh_outer ? i : o];
+  for (int nh = 0; nh < n_half; ++nh) {
+    for (const Seg& sg : segs) {
       const size_t base = blob.size();
       blob.resize(base + size_t(nsplit) * kBlkBytes, 0);
       for (int n = 0; n < 128; ++n) {
@@ -189,19 +178,6 @@ size_t push_floats(std::vector<float>& f, const float* src, size_t n) {
   f.insert(f.end(), src, src + n);
   while (f.size() % 4) f.push_back(0.0f);
   return off;
-}
-
-// Bias vector of a layer: fp32, or -- hidden layers of plain-bf16 nets -- bf16 pairs (element 2i in the low half of word i),
-// which the epilogue unpacks with a shift / mask (see epilogue_chunk).  Returns the word offset in `f`.
-size_t push_bias(std::vector<float>& f, const float* b, size_t n, bool packed_bf16) {
-  if (!packed_bf16) return push_floats(f, b, n);
-  std::vector<float> words((n + 1) / 2);
-  for (size_t i = 0; i < words.size(); ++i) {
-    const uint32_t lo = f2bf(b[2 * i]), hi = (2 * i + 1 < n) ? f2bf(b[2 * i + 1]) : 0u;
-    const uint32_t w = lo | (hi << 16);
-    std::memcpy(&words[i], &w, 4);
-  }
-  return push_floats(f, words.data(), words.size());
 }
 
 const HostTensor* find(const Net& n, const std::string& name) {
@@ -235,7 +211,6 @@ adn_status build_net0(adn_ctx* ctx) {
   if (D < 1 || D > kMaxLayers) return fail(ctx, ADN_ERR_INVALID, "sampling net: need layers.0.weight .. (1-12 layers)");
   const int nsplit = ctx->mlp0_terms == 3 ? 2 : 1;
   net.nsplit = nsplit;
-  net.ng = (nsplit == 2) ? 1 : 2;
   MlpProgram P{};
   P.n_layers = D;
   std::vector<uint8_t> wblob;
@@ -274,7 +249,7 @@ adn_status build_net0(adn_ctx* ctx) {
     L.out_blk0 = 0;
     L.w_off = uint32_t(wblob.size());
     pack_layer(W->data.data(), n_out, k_in, segs, nsplit, wblob);
-    L.bias_off = uint32_t(push_bias(fblob, B->data.data(), B->data.size(), nsplit == 1 && !last));
+    L.bias_off = uint32_t(push_floats(fblob, B->data.data(), B->data.size()));
     if (last) {
       net.n_out = n_out;
       P.out_cols = n_out;
@@ -283,7 +258,6 @@ adn_status build_net0(adn_ctx* ctx) {
   P.in0_blk = 0;
   P.in0_nblk = 2;
   P.in1_blk = 0;
-  P.hid_blk0 = 0;
   P.in_tile_stride = uint32_t(2 * nsplit * kBlkBytes);
   P.in0_off = 0;
   P.in0_lo_off = 2 * kBlkBytes;
@@ -336,17 +310,12 @@ adn_status build_net1(adn_ctx* ctx) {
       vb->data.size() != 128 || rb->data.size() != 3)
     return fail(ctx, ADN_ERR_INVALID, "shading net: feature/alpha/views/rgb tensors missing or wrong shape");
   net.nsplit = 1;
-  net.ng = 2;
   net.n_in = 90;
   net.n_out = 4;
-  // mlp_sh_kernel: CTA pairs, stand-alone stage 3 (the fused encoder lives in mlp_umma_kernel)
-  const bool sh = ctx->sh_kernel && ctx->cta_group == 2 && !ctx->fuse_encoder;
-  net.sh = sh;
   MlpProgram P{};
   P.n_layers = 10;
   std::vector<uint8_t> wblob;
   std::vector<float> fblob;
-  if (sh) fblob.assign(size_t(kSideFloats), 0.0f);   // fixed layout (mlp_umma.cuh: kSh*)
   const std::vector<Seg> segH = {{0, 64}, {64, 64}, {128, 64}, {192, 64}};
   for (int l = 0; l < 10; ++l) {
     MlpLayer& L = P.layers[l];
@@ -354,22 +323,12 @@ adn_status build_net1(adn_ctx* ctx) {
     const HostTensor *W, *B;
     L.out_blk0 = 1;
     L.n_half = 2;
-    L.lo_h = L.lo_s = 0xFF;
     if (l == 0) {
       segs = {{0, 63}};
       L.a_blk[0] = 0;
       L.flags = LF_RELU | LF_OUT_ACT;
       W = pw[0];
       B = pb[0];
-    } else if (l == 5 && sh) {
-      // cat[pts, h] (models.py:260-261) with the hidden blocks FIRST: the blocks half 0's epilogue overwrites in place are
-      // read by the first stage of every N half, so `lo_free` comes as early as it can
-      segs = {{63, 64}, {127, 64}, {191, 64}, {255, 64}, {0, 63}};
-      const uint8_t blk[5] = {1, 2, 3, 4, 0};
-      std::memcpy(L.a_blk, blk, 5);
-      L.flags = LF_RELU | LF_OUT_ACT | LF_LOAD_IN1_AFTER;
-      W = pw[5];
-      B = pb[5];
     } else if (l == 5) {
       segs = {{0, 63}, {63, 64}, {127, 64}, {191, 64}, {255, 64}};   // cat[pts, h] (models.py:260-261)
       const uint8_t blk[5] = {0, 1, 2, 3, 4};
@@ -401,77 +360,18 @@ adn_status build_net1(adn_ctx* ctx) {
       B = vb;
     }
     L.n_kb = uint8_t(segs.size());
+    for (size_t i = 0; i < segs.size(); ++i) L.k_cnt[i] = uint8_t((segs[i].valid + 15) / 16);
     L.w_off = uint32_t(wblob.size());
-    pack_layer(W->data.data(), int(W->rows), int(W->cols), segs, 1, wblob, sh);
-    if (sh) {
-      L.bias_off = uint32_t(256 * l);   // fp32, fixed offset: an immediate operand of the specialised epilogue
-      std::memcpy(&fblob[L.bias_off], B->data.data(), B->data.size() * 4);
-      if (L.n_half == 2 && (L.flags & LF_OUT_ACT)) {
-        // last (half, stage) in issue order that reads the blocks half 0's epilogue writes (out_blk0, out_blk0 + 1)
-        L.lo_h = L.lo_s = 0;
-        for (int h = 0; h < 2; ++h)
-          for (int kb = 0; kb < int(L.n_kb); ++kb)
-            if (L.a_blk[kb] == L.out_blk0 || L.a_blk[kb] == L.out_blk0 + 1) {
-              L.lo_h = uint8_t(h);
-              L.lo_s = uint8_t(kb / 2);
-            }
-      }
-    } else {
-      // hidden layers (activation-writing epilogues): bf16 pairs; the last layer (rgb head epilogue): fp32
-      L.bias_off = uint32_t(push_bias(fblob, B->data.data(), B->data.size(), !(L.flags & LF_FINAL_RGB)));
-    }
+    pack_layer(W->data.data(), int(W->rows), int(W->cols), segs, 1, wblob);
+    L.bias_off = uint32_t(push_floats(fblob, B->data.data(), B->data.size()));
   }
-  if (sh) {
-    // issue schedule of mlp_sh_kernel (see MlpProgram::sh_sched)
-    for (int l = 0; l < 10; ++l) {
-      const MlpLayer& L = P.layers[l];
-      const int n_st = (int(L.n_kb) + 1) / 2;
-      uint32_t seen = 0;
-      int n = 0;
-      for (int h = 0; h < int(L.n_half); ++h)
-        for (int s = 0; s < n_st; ++s) {
-          uint32_t need = 1u << h;   // accumulator half h drained by the previous layer's epilogue
-          for (int j = 0; j < 2; ++j) {
-            const int kb = 2 * s + j;
-            if (kb < int(L.n_kb) && int(L.a_blk[kb]) >= 1) need |= 1u << ((int(L.a_blk[kb]) - 1) >> 1);   // hid_blk0 = 1
-          }
-          need &= ~seen;
-          seen |= need;
-          const bool two = 2 * s + 1 < int(L.n_kb);
-          uint32_t w = uint32_t(L.a_blk[2 * s] & 15) | (uint32_t(two ? (L.a_blk[2 * s + 1] & 15) : 0) << 4) | (two ? 1u << 8 : 0u) | (need << 9);
-          if (s == n_st - 1) w |= 1u << 12;
-          if (L.lo_h != 0xFF && int(L.lo_h) == h && int(L.lo_s) == s) w |= 1u << 13;
-          w |= uint32_t(h) << 14;
-          if (s == 0) w |= 1u << 15;
-          if (!two && L.a_blk[2 * s] == 0) {   // the step's only K block is the tile input: it travels through the ring
-            w |= 1u << 16;
-            if (h == 0) w |= 1u << 17;                        // fetched here (one ring stage per slot, right after the weight stage)
-            if (h == int(L.n_half) - 1) w |= 1u << 18;        // ... and released here
-            if (L.flags & LF_WAIT_IN) w |= 1u << 19;          // view block: 27 features -> two K steps
-          }
-          w |= uint32_t(s) << 20;
-          P.sh_sched[l][n++] = w;
-        }
-      P.sh_steps[l] = uint8_t(n);
-    }
-    P.alpha_w_off = kShAlphaW;
-    P.alpha_b_off = kShAlphaB;
-    P.rgb_w_off = kShRgbW;
-    P.rgb_b_off = kShRgbB;
-    std::memcpy(&fblob[kShAlphaW], aw->data.data(), 256 * 4);
-    fblob[kShAlphaB] = ab->data[0];
-    std::memcpy(&fblob[kShRgbW], rw->data.data(), 3 * 128 * 4);
-    std::memcpy(&fblob[kShRgbB], rb->data.data(), 3 * 4);
-  } else {
-    P.alpha_w_off = uint32_t(push_floats(fblob, aw->data.data(), 256));
-    P.alpha_b_off = uint32_t(push_floats(fblob, ab->data.data(), 1));
-    P.rgb_w_off = uint32_t(push_floats(fblob, rw->data.data(), 3 * 128));
-    P.rgb_b_off = uint32_t(push_floats(fblob, rb->data.data(), 3));
-  }
+  P.alpha_w_off = uint32_t(push_floats(fblob, aw->data.data(), 256));
+  P.alpha_b_off = uint32_t(push_floats(fblob, ab->data.data(), 1));
+  P.rgb_w_off = uint32_t(push_floats(fblob, rw->data.data(), 3 * 128));
+  P.rgb_b_off = uint32_t(push_floats(fblob, rb->data.data(), 3));
   P.in0_blk = 0;
   P.in0_nblk = 1;
   P.in1_blk = 0;
-  P.hid_blk0 = 1;
   P.in_tile_stride = 2 * kBlkBytes;
   P.in0_off = 0;
   P.in0_lo_off = 0;
@@ -556,14 +456,7 @@ int64_t pad128(int64_t n) { return (n + 127) / 128 * 128; }
 adn_status run_mlp(adn_ctx* ctx, int id, const uint8_t* tiles, float* out, const long long* rows_dev, long long rows,
                    cudaStream_t st, const EncodeParams* enc = nullptr) {
   Net& n = ctx->net[id];
-  long long* trace = ctx->trace_net == id ? ctx->d_trace : nullptr;
-  cudaError_t e;
-  if (id == 1 && n.sh) {
-    if (enc) return fail(ctx, ADN_ERR_INVALID, "shading net is packed for mlp_sh_kernel: no fused encoder");
-    e = launch_mlp_sh(n.prog, n.d_wblob, tiles, out, rows_dev, rows, ctx->d_err, ctx->num_sms, st, trace);
-  } else {
-    e = launch_mlp(n.nsplit, n.ng, ctx->cta_group, n.prog, n.d_wblob, tiles, out, rows_dev, rows, ctx->d_err, ctx->num_sms, st, trace, enc);
-  }
+  const cudaError_t e = launch_mlp(n.nsplit, n.prog, n.d_wblob, tiles, out, rows_dev, rows, ctx->d_err, ctx->num_sms, st, enc);
   if (e != cudaSuccess) return cuda_fail(ctx, e, id == 0 ? "launch sampling MLP" : "launch shading MLP");
   ctx->stats.kernel_launches++;
   return ADN_OK;
@@ -590,7 +483,7 @@ adn_status render_chunk(adn_ctx* ctx, const PoseDev& pd, const float* d_dirs, co
     if ((s = ensure(ctx, ctx->s2scratch, stage2_scratch_bytes(n))) != ADN_OK) return s;
   }
   // stage 3 runs inside the shading kernel (encoder warp) unless the variant needs the stand-alone kernel
-  const bool fused_enc = ctx->fuse_encoder && ctx->cta_group == 2 && !ctx->scene.use_ndc && !ctx->net[1].sh;
+  const bool fused_enc = ctx->fuse_encoder && !ctx->scene.use_ndc;
   if (!fused_enc && (s = ensure(ctx, ctx->tiles1, size_t(pad128(cap) / 128) * 2 * kBlkBytes)) != ADN_OK) return s;
   if ((s = ensure(ctx, ctx->raw1, size_t(pad128(cap)) * 16)) != ADN_OK) return s;
 
@@ -639,8 +532,6 @@ adn_status render_chunk(adn_ctx* ctx, const PoseDev& pd, const float* d_dirs, co
     ep.K = K;
     for (int a = 0; a < 3; ++a) ep.c[a] = ctx->sc.c[a];
     ep.sqrt_max_depth = ctx->sc.sqrt_max_depth;
-    if ((s = ensure(ctx, ctx->enc_scratch, mlp_enc_scratch_bytes(ctx->num_sms))) != ADN_OK) return s;
-    ep.scratch = static_cast<uint8_t*>(ctx->enc_scratch.p);
   } else {
     ADN_CUDA(ctx, launch_stage3(ctx->sc, ray_o, ray_d, dense ? nullptr : static_cast<int32_t*>(ctx->rayidx.p),
                                 static_cast<float*>(ctx->zbuf.p), ctx->d_zlut_dense, K, cap, ctx->d_total, nullptr, tiles1, st));
@@ -728,7 +619,7 @@ adn_status check_device_error(adn_ctx* ctx) {
 // =================================================================================================
 extern "C" {
 
-const char* adn_version(void) { return "adanerf_b200 0.1 (sm_100a)"; }
+const char* adn_version(void) { return "adanerf_b200 0.1 (sm_90a)"; }
 
 const char* adn_strerror(adn_status s) {
   if (s < 0 || s > ADN_ERR_KERNEL) return "unknown status";
@@ -744,7 +635,7 @@ adn_status adn_create(adn_ctx** out, const adn_scene* scene, int device) {
   if (cudaGetDeviceCount(&n_dev) != cudaSuccess || device < 0 || device >= n_dev) return ADN_ERR_NO_DEVICE;
   cudaDeviceProp prop{};
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return ADN_ERR_NO_DEVICE;
-  if (prop.major != 10) return ADN_ERR_NO_DEVICE;  // tcgen05 / TMEM kernels: sm_100 family only, no fallback
+  if (prop.major != 9) return ADN_ERR_NO_DEVICE;  // wgmma / setmaxnreg kernels (sm_90a): Hopper only, no fallback
   if (scene->n_freq_pos != 10 || scene->n_freq_dir != 4) return ADN_ERR_INVALID;  // posEncArgs[1] "10-4" (F = 90)
   const int nfp0 = scene->n_freq_pos0 ? scene->n_freq_pos0 : scene->n_freq_pos;
   const int nfd0 = scene->n_freq_dir0 ? scene->n_freq_dir0 : scene->n_freq_dir;
@@ -753,8 +644,6 @@ adn_status adn_create(adn_ctx** out, const adn_scene* scene, int device) {
   adn_ctx* ctx = new adn_ctx();
   ctx->device = device;
   ctx->num_sms = prop.multiProcessorCount;
-  if (const char* cg = std::getenv("ADN_CTA_GROUP")) ctx->cta_group = (cg[0] == '1') ? 1 : 2;   // A/B experiments
-  if (const char* sk = std::getenv("ADN_SHADING_KERNEL")) ctx->sh_kernel = (sk[0] != '0');
   if (const char* wc = std::getenv("ADN_WEIGHT_COPIES")) ctx->weight_copies = std::max(1, std::min(64, std::atoi(wc)));
   ctx->scene = *scene;
   if (cudaSetDevice(device) != cudaSuccess) {
@@ -805,7 +694,7 @@ void adn_destroy(adn_ctx* ctx) {
   cudaSetDevice(ctx->device);
   cudaDeviceSynchronize();
   Buf* bufs[] = {&ctx->tiles0, &ctx->raw0, &ctx->x0,    &ctx->ray_o,  &ctx->ray_d, &ctx->dirs,      &ctx->count, &ctx->offset,
-                 &ctx->rayidx, &ctx->zbuf, &ctx->zpbuf, &ctx->tiles1, &ctx->raw1,  &ctx->s2scratch, &ctx->rgb,   &ctx->rgba, &ctx->x1, &ctx->metric, &ctx->enc_scratch};
+                 &ctx->rayidx, &ctx->zbuf, &ctx->zpbuf, &ctx->tiles1, &ctx->raw1,  &ctx->s2scratch, &ctx->rgb,   &ctx->rgba, &ctx->x1, &ctx->metric};
   for (Buf* b : bufs)
     if (b->p) cudaFree(b->p);
   for (auto& r : ctx->regs)
@@ -820,7 +709,6 @@ void adn_destroy(adn_ctx* ctx) {
   if (ctx->d_zlut_dense) cudaFree(ctx->d_zlut_dense);
   if (ctx->d_total) cudaFree(ctx->d_total);
   if (ctx->h_err) cudaFreeHost(ctx->h_err);
-  if (ctx->d_trace) cudaFree(ctx->d_trace);
   for (int i = 0; i < 8; ++i)
     if (ctx->ev[i]) cudaEventDestroy(ctx->ev[i]);
   if (ctx->own_stream) cudaStreamDestroy(ctx->own_stream);
@@ -860,32 +748,9 @@ adn_status adn_set_option(adn_ctx* ctx, const char* name, int64_t value) {
     ctx->profile = value != 0;
     return ADN_OK;
   }
-  if (n == "trace") {   // debug: value = net id to trace (0 / 1), -1 = off
-    ctx->trace_net = int(value);
-    if (value >= 0 && !ctx->d_trace) ADN_CUDA(ctx, cudaMalloc(&ctx->d_trace, sizeof(long long) * 131072));
-    if (ctx->d_trace) ADN_CUDA(ctx, cudaMemset(ctx->d_trace, 0, sizeof(long long) * 131072));
-    return ADN_OK;
-  }
-  // the three options below select the shading kernel (mlp_sh_kernel unless one of them rules it out): the packed weight
-  // stream differs, so the shading net is re-packed when the choice changes
-  auto repack_net1 = [&]() -> adn_status {
-    if (ctx->net[1].tensors.empty()) return ADN_OK;
-    ADN_CUDA(ctx, cudaSetDevice(ctx->device));
-    ADN_CUDA(ctx, cudaDeviceSynchronize());
-    return build_net1(ctx);
-  };
   if (n == "fuse_encoder") {   // 1: positional encoding inside the shading kernel (no tile buffer); 0 (default): stage3_kernel + packed tiles
     ctx->fuse_encoder = value != 0;
-    return repack_net1();
-  }
-  if (n == "cta_group") {   // experiments / A-B runs: 1 = single-CTA MMAs, 2 = CTA pairs (default)
-    if (value != 1 && value != 2) return fail(ctx, ADN_ERR_INVALID, "cta_group must be 1 or 2");
-    ctx->cta_group = int(value);
-    return repack_net1();
-  }
-  if (n == "shading_kernel") {   // 1 (default): mlp_sh_kernel; 0: mlp_umma_kernel<1,2,.> (round-1 kernel, A/B runs)
-    ctx->sh_kernel = value != 0;
-    return repack_net1();
+    return ADN_OK;
   }
   if (n == "mlp0_terms") {
     if (value != 1 && value != 3) return fail(ctx, ADN_ERR_INVALID, "mlp0_terms must be 1 or 3");
@@ -1195,14 +1060,6 @@ adn_status adn_probe_export_dir(const char* dir, adn_scene* scene_out, float* th
     n_tensors_out[0] = int(ex.nets[0].size());
     n_tensors_out[1] = int(ex.nets[1].size());
   }
-  return ADN_OK;
-}
-
-// Debug only (not part of the public header): copies the MLP timeline recorded after adn_set_option("trace", net).
-adn_status adn_debug_read_trace(adn_ctx* ctx, long long* out, int64_t n_words) {
-  if (!ctx || !out || !ctx->d_trace || n_words < 2 || n_words > 131072) return ADN_ERR_INVALID;
-  ADN_CUDA(ctx, cudaDeviceSynchronize());
-  ADN_CUDA(ctx, cudaMemcpy(out, ctx->d_trace, sizeof(long long) * n_words, cudaMemcpyDeviceToHost));
   return ADN_OK;
 }
 

@@ -1,0 +1,390 @@
+// Warpgroup-MMA fused MLP kernel (see mlp.cuh for the design).
+#include <cuda_bf16.h>
+#include <cuda_runtime.h>
+
+#include "mlp.cuh"
+#include "posenc.cuh"
+#include "ptx.cuh"
+
+namespace adn {
+
+__device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
+  __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&h);
+}
+
+template <int NSPLIT>
+struct MlpCfg {
+  static constexpr int kNB = (NSPLIT == 2) ? 4 : 5;                  // activation blocks per term
+  static constexpr int kStageBytes = NSPLIT * kBlkBytes;              // one [128 x 64] weight block (+ its lo part)
+  // as many ring stages as fit next to the activations and the side parameters (227 KB per block)
+  static constexpr int kStages = (NSPLIT == 2) ? 2 : 8;
+  static constexpr size_t kActBytes = size_t(NSPLIT) * kNB * kBlkBytes;
+  static constexpr size_t kSmemBytes =
+      kActBytes + size_t(kStages) * kStageBytes + size_t(kSideFloats) * 4 + 2 * kStages * 8 + 1024 /*alignment slack*/;
+};
+static_assert(MlpCfg<1>::kSmemBytes <= 232448 && MlpCfg<2>::kSmemBytes <= 232448, "shared memory per block (sm_90)");
+
+// One row of a fused-encoder input block: P (63 position features + 0) or V (27 direction features + zeros), computed
+// and packed to bf16 exactly as stage3_kernel does it (same device functions, same operation order).
+template <bool VIEW>
+__device__ __forceinline__ void encode_row(const EncodeParams& enc, long long i, long long rows, uint32_t blk, int row) {
+  float f[64];
+#pragma unroll
+  for (int k = 0; k < 64; ++k) f[k] = 0.0f;
+  if (i < rows) {
+    long long ray;
+    float zw;
+    if (enc.ray_idx) {
+      ray = enc.ray_idx[i];
+      zw = enc.z[i];
+    } else {
+      ray = i / enc.K;
+      zw = enc.zlut_dense[i - ray * enc.K];
+    }
+    float v[3];
+    if (VIEW) {
+#pragma unroll
+      for (int a = 0; a < 3; ++a) v[a] = __ldg(enc.ray_d + 3 * ray + a);
+      posenc3<4>(v, f);
+    } else {
+      // pos = o + d z, then normalization_inverse_sqrt_dist_centered (same operation order as stage3_kernel)
+#pragma unroll
+      for (int a = 0; a < 3; ++a)
+        v[a] = __fsub_rn(__fadd_rn(__ldg(enc.ray_o + 3 * ray + a), __fmul_rn(__ldg(enc.ray_d + 3 * ray + a), zw)), enc.c[a]);
+      const float nrm = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(v[0], v[0]), __fmul_rn(v[1], v[1])), __fmul_rn(v[2], v[2])));
+      const float den = __fmul_rn(enc.sqrt_max_depth, __fsqrt_rn(nrm));
+#pragma unroll
+      for (int a = 0; a < 3; ++a) v[a] = __fdiv_rn(v[a], den);
+      posenc3<10>(v, f);
+    }
+  }
+#pragma unroll
+  for (int ch = 0; ch < 8; ++ch) {
+    const float* q = f + ch * 8;
+    st_shared_v4(blk + sw128_offset(uint32_t(row), uint32_t(ch * 8)), bf16x2(q[0], q[1]), bf16x2(q[2], q[3]), bf16x2(q[4], q[5]),
+                 bf16x2(q[6], q[7]));
+  }
+}
+
+// This warpgroup's 64 rows (the first or second 8 KB) of `nblk` consecutive packed blocks, global -> shared.
+__device__ __forceinline__ void copy_rows(const uint8_t* __restrict__ src, uint32_t dst, int nblk, int wg, int tw) {
+  for (int b = 0; b < nblk; ++b) {
+    const uint4* s = reinterpret_cast<const uint4*>(src + size_t(b) * kBlkBytes + size_t(wg) * (kBlkBytes / 2));
+    const uint32_t d = dst + uint32_t(b) * kBlkBytes + uint32_t(wg) * (kBlkBytes / 2);
+    uint4 v[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) v[j] = __ldg(s + tw + 128 * j);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) st_shared_v4(d + uint32_t(tw + 128 * j) * 16u, v[j].x, v[j].y, v[j].z, v[j].w);
+  }
+}
+
+template <int NSPLIT, bool ENC>
+__global__ void __launch_bounds__(kMlpThreads, 1)
+mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ wblob, const uint8_t* __restrict__ in_tiles,
+           float* __restrict__ out, const long long* __restrict__ rows_dev, long long rows_host, int* err_flag,
+           const __grid_constant__ EncodeParams enc) {
+  static_assert(!ENC || NSPLIT == 1, "fused input encoder: shading net (plain bf16) only");
+  using Cfg = MlpCfg<NSPLIT>;
+  constexpr int NB = Cfg::kNB;
+  constexpr int STAGES = Cfg::kStages;
+  constexpr int STAGE_BYTES = Cfg::kStageBytes;
+  constexpr int kConsumerWarps = 8, kProducerWarp = 8;
+
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* act = smem;                                                   // [NSPLIT][NB] blocks
+  uint8_t* ring = act + Cfg::kActBytes;                                  // [STAGES] stages
+  float* side = reinterpret_cast<float*>(ring + size_t(STAGES) * STAGE_BYTES);
+  uint64_t* w_full = reinterpret_cast<uint64_t*>(side + kSideFloats);   // [STAGES] the stage has landed
+  uint64_t* w_empty = w_full + STAGES;                                   // [STAGES] every consumer warp's MMAs on it retired
+
+  const int warp = __shfl_sync(0xffffffffu, int(threadIdx.x >> 5), 0);
+  const int lane = threadIdx.x & 31;
+  const long long rows = rows_dev ? *rows_dev : rows_host;
+  const long long n_tiles = (rows + kTileM - 1) / kTileM;
+
+  // biases and heads: the epilogue reads a different column per lane, which the constant bank would serialise
+  for (int i = threadIdx.x; i < kSideFloats; i += blockDim.x) side[i] = prog.side[i];
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(&w_full[s], 1);
+      mbar_init(&w_empty[s], kConsumerWarps);
+    }
+    mbar_fence_init();
+  }
+  __syncthreads();
+
+  if (warp >= kProducerWarp) {
+    // ===================================================================== weight producer
+    setmaxnreg_dec<40>();
+    // Stage i of a layer is [128 N rows x 64 K] (hi, then lo when NSPLIT == 2), N half outermost: the order the
+    // consumers walk them in.
+    if (warp == kProducerWarp && lane == 0) {
+      const uint8_t* blob = wblob + size_t(blockIdx.x % prog.w_copies) * prog.w_stride;
+      int stage = 0;
+      uint32_t phase = 0;
+      for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+        for (int l = 0; l < prog.n_layers; ++l) {
+          const MlpLayer& L = prog.layers[l];
+          const int n_st = int(L.n_kb) * int(L.n_half);
+          for (int i = 0; i < n_st; ++i) {
+            mbar_wait(&w_empty[stage], phase ^ 1, err_flag, 1);
+            mbar_arrive_expect_tx(&w_full[stage], STAGE_BYTES);
+            bulk_g2s(ring + size_t(stage) * STAGE_BYTES, blob + L.w_off + size_t(i) * STAGE_BYTES, STAGE_BYTES, &w_full[stage]);
+            if (++stage == STAGES) {
+              stage = 0;
+              phase ^= 1;
+            }
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  // ============================================================================ consumer warpgroups
+  setmaxnreg_inc<232>();
+  const int wg = warp >> 2;                               // rows [64 wg, 64 wg + 64) of every tile
+  const int tw = threadIdx.x & 127;
+  const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2); // accumulator rows r0 and r0 + 8 of this thread
+  const int cq = 2 * (lane & 3);                          // column pair inside every 8-column group
+  const int bar_id = 1 + wg;                              // named barrier of this warpgroup
+  const uint32_t act_s = smem_u32(act);
+  const uint32_t ring_s = smem_u32(ring);
+  const uint32_t wg_off = uint32_t(wg) * (kBlkBytes / 2); // this warpgroup's rows inside a block
+  auto blk_addr = [&](int term, int blk) -> uint32_t { return act_s + uint32_t(term * NB + blk) * kBlkBytes; };
+  const uint64_t desc_hi = make_desc_sw128(0) & ~uint64_t(0x3FFF);
+  auto desc = [&](uint32_t addr) -> uint64_t { return desc_hi | uint64_t((addr & 0x3FFFF) >> 4); };
+
+  int stage = 0;
+  uint32_t phase = 0;
+  for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+    // tile input (the previous tile's last MMAs retired before its epilogue: the blocks are free)
+    if (ENC) {
+      if (tw < 64) encode_row<false>(enc, t * kTileM + 64 * wg + tw, rows, blk_addr(0, prog.in0_blk), 64 * wg + tw);
+    } else {
+      const uint8_t* src = in_tiles + size_t(t) * prog.in_tile_stride;
+      copy_rows(src + prog.in0_off, blk_addr(0, prog.in0_blk), prog.in0_nblk, wg, tw);
+      if (NSPLIT == 2) copy_rows(src + prog.in0_lo_off, blk_addr(1, prog.in0_blk), prog.in0_nblk, wg, tw);
+    }
+    fence_proxy_async_smem();
+    named_bar_sync(bar_id, 128);
+    float alpha[2] = {0.0f, 0.0f};
+    for (int l = 0; l < prog.n_layers; ++l) {
+      const MlpLayer& L = prog.layers[l];
+      float acc[2][64];   // written by the first MMA of each half (accumulate = 0): K block 0 has at least one K step
+      int prev = -1;   // ring stage whose MMAs may still be running
+#pragma unroll
+      for (int nh = 0; nh < 2; ++nh) {
+        if (nh >= L.n_half) break;
+        for (int kb = 0; kb < L.n_kb; ++kb) {
+          const uint32_t a_hi = blk_addr(0, L.a_blk[kb]) + wg_off;
+          const uint32_t a_lo = a_hi + uint32_t(NSPLIT - 1) * NB * kBlkBytes;
+          const uint32_t b_hi = ring_s + uint32_t(stage) * STAGE_BYTES;
+          const uint32_t b_lo = b_hi + uint32_t(NSPLIT - 1) * kBlkBytes;
+          const int nk = L.k_cnt[kb];   // zero-padded tail columns of an input block are not multiplied
+          mbar_wait(&w_full[stage], phase, err_flag, 2);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            if (k < nk) {
+              wgmma_m64n128_bf16(acc[nh], desc(a_hi + 32 * k), desc(b_hi + 32 * k), (kb > 0 || k > 0) ? 1u : 0u);
+              if (NSPLIT == 2) {
+                wgmma_m64n128_bf16(acc[nh], desc(a_lo + 32 * k), desc(b_hi + 32 * k), 1u);
+                wgmma_m64n128_bf16(acc[nh], desc(a_hi + 32 * k), desc(b_lo + 32 * k), 1u);
+              }
+            }
+          }
+          wgmma_commit();
+          wgmma_wait<1>();   // the previous stage's MMAs have retired: hand it back to the producer
+          if (prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);
+          prev = stage;
+          if (++stage == STAGES) {
+            stage = 0;
+            phase ^= 1;
+          }
+        }
+      }
+      wgmma_wait<0>();
+      if (lane == 0) mbar_arrive(&w_empty[prev]);
+      named_bar_sync(bar_id, 128);   // all of the warpgroup's MMAs retired: the A blocks may be overwritten in place
+
+      // ------------------------------------------------------------------ epilogue
+      const uint8_t flags = L.flags;
+      float rgb[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+#pragma unroll
+      for (int nh = 0; nh < 2; ++nh) {
+        if (nh >= L.n_half) break;
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+          const int col = nh * 128 + 8 * i + cq;
+          const float2 b = *reinterpret_cast<const float2*>(side + L.bias_off + col);
+#pragma unroll
+          for (int rr = 0; rr < 2; ++rr) {
+            const int row = r0 + 8 * rr;
+            float v0 = acc[nh][4 * i + 2 * rr] + b.x;
+            float v1 = acc[nh][4 * i + 2 * rr + 1] + b.y;
+            if (flags & LF_FINAL_RAW) {
+              const long long grow = t * kTileM + row;
+              if (grow < rows) *reinterpret_cast<float2*>(out + grow * prog.out_cols + col) = make_float2(v0, v1);
+              continue;
+            }
+            if (flags & LF_RELU) {
+              v0 = fmaxf(v0, 0.0f);
+              v1 = fmaxf(v1, 0.0f);
+            }
+            if (flags & LF_ALPHA_DOT) {
+              const float2 w = *reinterpret_cast<const float2*>(side + prog.alpha_w_off + col);
+              alpha[rr] = fmaf(v1, w.y, fmaf(v0, w.x, alpha[rr]));
+            }
+            if (flags & LF_OUT_ACT) {
+              const uint32_t off = uint32_t(L.out_blk0 + (col >> 6)) * kBlkBytes + sw128_offset(uint32_t(row), uint32_t(col & 63));
+              const uint32_t hi = pack_bf16x2(v0, v1);
+              asm volatile("st.shared.b32 [%0], %1;" ::"r"(act_s + off), "r"(hi) : "memory");
+              if (NSPLIT == 2) {
+                const uint32_t lo = pack_bf16x2(v0 - __uint_as_float(hi << 16), v1 - __uint_as_float(hi & 0xFFFF0000u));
+                asm volatile("st.shared.b32 [%0], %1;" ::"r"(act_s + uint32_t(NB * kBlkBytes) + off), "r"(lo) : "memory");
+              }
+            }
+            if (flags & LF_FINAL_RGB) {
+#pragma unroll
+              for (int k = 0; k < 3; ++k) {
+                const float2 w = *reinterpret_cast<const float2*>(side + prog.rgb_w_off + k * 128 + col);
+                rgb[rr][k] = fmaf(v1, w.y, fmaf(v0, w.x, rgb[rr][k]));
+              }
+            }
+          }
+        }
+      }
+      if (flags & LF_FINAL_RGB) {
+        // the four lanes of a row hold partial dot products over interleaved column pairs
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          float a = alpha[rr], c0 = rgb[rr][0], c1 = rgb[rr][1], c2 = rgb[rr][2];
+#pragma unroll
+          for (int m = 1; m <= 2; m <<= 1) {
+            a += __shfl_xor_sync(0xffffffffu, a, m);
+            c0 += __shfl_xor_sync(0xffffffffu, c0, m);
+            c1 += __shfl_xor_sync(0xffffffffu, c1, m);
+            c2 += __shfl_xor_sync(0xffffffffu, c2, m);
+          }
+          const long long grow = t * kTileM + r0 + 8 * rr;
+          if ((lane & 3) == 0 && grow < rows)
+            reinterpret_cast<float4*>(out)[grow] = make_float4(c0 + side[prog.rgb_b_off], c1 + side[prog.rgb_b_off + 1],
+                                                               c2 + side[prog.rgb_b_off + 2], a + side[prog.alpha_b_off]);
+        }
+      }
+      if (flags & LF_LOAD_IN1_AFTER) {   // the 2nd input block (view directions) replaces the tile-start block
+        if (ENC) {
+          if (tw < 64) encode_row<true>(enc, t * kTileM + 64 * wg + tw, rows, blk_addr(0, prog.in1_blk), 64 * wg + tw);
+        } else {
+          copy_rows(in_tiles + size_t(t) * prog.in_tile_stride + prog.in1_off, blk_addr(0, prog.in1_blk), 1, wg, tw);
+        }
+      }
+      fence_proxy_async_smem();        // generic-proxy stores -> visible to the next layer's wgmma reads
+      named_bar_sync(bar_id, 128);
+    }
+  }
+}
+
+// -------------------------------------------------------------------------------------------------
+// fp32 feature rows [rows, n_feat] -> packed bf16 (hi / lo) SWIZZLE_128B tile blocks.
+// One thread per (row, block, 16-byte chunk): 8 consecutive source columns.
+__global__ void pack_rows_kernel(const float* __restrict__ x, long long rows_host, const long long* __restrict__ rows_dev,
+                                 int n_feat, const __grid_constant__ InputLayout lay, uint8_t* __restrict__ tiles) {
+  const long long rows = rows_dev ? *rows_dev : rows_host;
+  const long long n_tiles = (rows + kTileM - 1) / kTileM;
+  const long long total = n_tiles * kTileM * lay.n_blk * 8;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int chunk = int(i & 7);
+    const long long rb = i >> 3;
+    const int blk = int(rb % lay.n_blk);
+    const long long row = rb / lay.n_blk;
+    const int r = int(row & (kTileM - 1));
+    const long long t = row >> 7;
+    float v[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int kk = chunk * 8 + j;
+      v[j] = (row < rows && kk < lay.valid[blk]) ? x[row * n_feat + lay.src_col0[blk] + kk] : 0.0f;
+    }
+    uint4 hi;
+    hi.x = pack_bf16x2(v[0], v[1]);
+    hi.y = pack_bf16x2(v[2], v[3]);
+    hi.z = pack_bf16x2(v[4], v[5]);
+    hi.w = pack_bf16x2(v[6], v[7]);
+    const uint32_t off = sw128_offset(uint32_t(r), uint32_t(chunk * 8));
+    uint8_t* tb = tiles + size_t(t) * lay.tile_stride;
+    *reinterpret_cast<uint4*>(tb + lay.dst_off_hi[blk] + off) = hi;
+    if (lay.nsplit == 2) {
+      const uint32_t hw[4] = {hi.x, hi.y, hi.z, hi.w};
+      float l[8];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        l[2 * e + 0] = v[2 * e + 0] - __uint_as_float(hw[e] << 16);
+        l[2 * e + 1] = v[2 * e + 1] - __uint_as_float(hw[e] & 0xFFFF0000u);
+      }
+      uint4 lo;
+      lo.x = pack_bf16x2(l[0], l[1]);
+      lo.y = pack_bf16x2(l[2], l[3]);
+      lo.z = pack_bf16x2(l[4], l[5]);
+      lo.w = pack_bf16x2(l[6], l[7]);
+      *reinterpret_cast<uint4*>(tb + lay.dst_off_lo[blk] + off) = lo;
+    }
+  }
+}
+
+// -------------------------------------------------------------------------------------------------
+cudaError_t set_max_dyn_smem_once(const void* func, int bytes, unsigned long long* done) {
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  if (dev < 64 && ((__atomic_load_n(done, __ATOMIC_ACQUIRE) >> dev) & 1ull)) return cudaSuccess;
+  e = cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e != cudaSuccess) return e;
+  if (dev < 64) __atomic_fetch_or(done, 1ull << dev, __ATOMIC_RELEASE);   // two threads may both set the (idempotent) attribute
+  return cudaSuccess;
+}
+
+template <int NSPLIT, bool ENC>
+static cudaError_t launch_mlp_t(const MlpProgram& prog, const uint8_t* wblob, const uint8_t* in_tiles, float* out,
+                                const long long* rows_dev, long long rows_host, int* err_flag, int num_sms, cudaStream_t stream,
+                                const EncodeParams& enc) {
+  static unsigned long long attr_done = 0;   // per device
+  const size_t smem = MlpCfg<NSPLIT>::kSmemBytes;
+  auto kernel = mlp_kernel<NSPLIT, ENC>;
+  cudaError_t e = set_max_dyn_smem_once(reinterpret_cast<const void*>(kernel), int(smem), &attr_done);
+  if (e != cudaSuccess) return e;
+  long long grid = num_sms;   // persistent: one CTA per SM
+  if (!rows_dev) {
+    const long long n_tiles = (rows_host + kTileM - 1) / kTileM;
+    if (n_tiles < grid) grid = n_tiles < 1 ? 1 : n_tiles;
+  }
+  kernel<<<unsigned(grid), kMlpThreads, smem, stream>>>(prog, wblob, in_tiles, out, rows_dev, rows_host, err_flag, enc);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_mlp(int nsplit, const MlpProgram& prog, const uint8_t* wblob, const uint8_t* in_tiles, float* out,
+                       const long long* rows_dev, long long rows_host, int* err_flag, int num_sms, cudaStream_t stream,
+                       const EncodeParams* enc) {
+  if (enc) {   // shading net with the fused input encoder
+    if (nsplit != 1) return cudaErrorInvalidValue;
+    return launch_mlp_t<1, true>(prog, wblob, in_tiles, out, rows_dev, rows_host, err_flag, num_sms, stream, *enc);
+  }
+  if (nsplit == 2) return launch_mlp_t<2, false>(prog, wblob, in_tiles, out, rows_dev, rows_host, err_flag, num_sms, stream, EncodeParams{});
+  return launch_mlp_t<1, false>(prog, wblob, in_tiles, out, rows_dev, rows_host, err_flag, num_sms, stream, EncodeParams{});
+}
+
+cudaError_t launch_pack_rows(const float* x, long long rows, const long long* rows_dev, int n_feat, const InputLayout& lay,
+                             uint8_t* tiles, cudaStream_t stream) {
+  long long work = ((rows + kTileM - 1) / kTileM) * kTileM * lay.n_blk * 8;
+  int grid = int((work + 255) / 256);
+  if (grid < 1) grid = 1;
+  if (grid > 132 * 16) grid = 132 * 16;
+  pack_rows_kernel<<<grid, 256, 0, stream>>>(x, rows, rows_dev, n_feat, lay, tiles);
+  return cudaGetLastError();
+}
+
+}  // namespace adn

@@ -1,0 +1,105 @@
+// Fused multi-layer perceptron on the Hopper tensor cores (wgmma), sm_90a.
+//
+// One persistent CTA per SM walks 128-row tiles of the batch through ALL layers of the network:
+//   * weights stream layer by layer from L2 into a shared-memory ring with 1-D bulk async copies
+//     (TMA engine), pre-packed on the host as K-major SWIZZLE_128B tiles in consumption order,
+//   * activations never leave the SM: two consumer warpgroups each own 64 rows of the tile, accumulate
+//     a layer in registers (wgmma m64n128k16, one 64-register accumulator per 128-column N half), add
+//     bias / ReLU, round to bf16 (optionally a hi+lo split) and write the next layer's A operand
+//     straight into swizzled shared memory; a warpgroup only ever touches its own rows, so the layers
+//     of one warpgroup need no synchronisation with the other beyond the shared weight ring,
+//   * warp roles: warpgroups 0, 1 = consumers, warpgroup 2 = weight producer (one thread issues the copies); the
+//     producer hands most of its registers to the consumers (setmaxnreg), whose accumulators take 128 per thread.
+//
+// NSPLIT = 2 is the split-precision mode of the sampling network: x = hi + lo (both bf16) for
+// activations and weights and three MMAs per K step (hi*hi + lo*hi + hi*lo), fp32 accumulate --
+// fp32-class accuracy, which the bit-exact threshold decisions downstream need (SURVEY.md 8d).
+#pragma once
+#include <cstdint>
+#include <cuda_runtime.h>
+
+namespace adn {
+
+constexpr int kTileM = 128;
+constexpr int kBlkBytes = 16384;  // one [128 x 64] bf16 SWIZZLE_128B block
+constexpr int kMaxLayers = 12;
+constexpr int kMlpThreads = 384;  // three warpgroups: two consumers, one weight producer
+constexpr int kSideFloats = 3208; // fp32 side parameters (biases, alpha / rgb heads), copied to shared memory per CTA
+
+enum : uint8_t {
+  LF_RELU = 1,
+  LF_ALPHA_DOT = 2,      // accumulate alpha = <post-activation row, alpha_w> on CUDA cores (fp32)
+  LF_OUT_ACT = 4,        // write bf16 activations for the next layer
+  LF_FINAL_RAW = 8,      // write fp32 rows to global (sampling net output / test programs)
+  LF_FINAL_RGB = 16,     // rgb_linear on CUDA cores + write float4 (rgb, alpha)
+  LF_LOAD_IN1_AFTER = 32,  // once this layer's MMAs are done, fetch the 2nd input block (view dirs)
+  LF_WAIT_IN = 64          // this layer reads that 2nd input block
+};
+
+struct MlpLayer {
+  uint32_t w_off;     // byte offset of this layer's packed weight stages (N half outermost, then K block)
+  uint32_t bias_off;  // float offset of the fp32 bias vector in MlpProgram::side
+  uint8_t n_kb;       // number of 64-wide K blocks
+  uint8_t a_blk[6];   // activation block index per K block
+  uint8_t n_half;     // N / 128  (1 or 2)
+  uint8_t flags;
+  uint8_t out_blk0;   // first activation block the epilogue writes
+  // 16-wide K steps issued per K block (4 = the whole 64-wide block; fewer when the tail columns of the block are zero
+  // padding, e.g. 90 input features -> blocks of 4 and 2 steps; 30 features -> 2 and 0).
+  uint8_t k_cnt[6];
+};
+
+struct MlpProgram {
+  int32_t n_layers;
+  int32_t in0_blk, in0_nblk;  // tile-start input: destination block, number of blocks (per term)
+  int32_t in1_blk;            // 2nd input destination block
+  uint32_t in_tile_stride;    // bytes per tile in the packed input buffer
+  uint32_t in0_off, in0_lo_off, in1_off;
+  uint32_t alpha_w_off, alpha_b_off, rgb_w_off, rgb_b_off;  // float offsets in `side`
+  int32_t out_cols;           // row stride of the FINAL_RAW output
+  // The packed weight blob is replicated w_copies times in global memory, w_stride bytes apart; CTA c streams copy
+  // c % w_copies (spreads the grid's nearly lock-step re-reads of the same lines over more L2 slices).
+  uint32_t w_copies, w_stride;
+  MlpLayer layers[kMaxLayers];
+  float side[kSideFloats];
+};
+
+// Describes how fp32 feature rows map onto the packed bf16 input blocks of a tile.
+struct InputLayout {
+  int32_t n_blk;
+  int32_t src_col0[4];
+  int32_t valid[4];
+  uint32_t dst_off_hi[4];
+  uint32_t dst_off_lo[4];
+  uint32_t tile_stride;
+  int32_t nsplit;
+};
+
+// Fused input encoder of the shading MLP (stage 3 inside the kernel): the consumer warpgroups compute the positional
+// encoding of their packed samples (RayMarchFromPoses.batch, src/features.py:458-479) straight into the tile's input
+// block, so the [M, 90] feature tensor and its packed tiles never exist in HBM.  ray_idx == nullptr: dense mode
+// (ray = sample / K, z = zlut_dense[sample % K]).
+struct EncodeParams {
+  const float* ray_o = nullptr;       // [N,3]
+  const float* ray_d = nullptr;       // [N,3] (un-normalised, as SpherePosDir hands it on)
+  const int32_t* ray_idx = nullptr;   // [M] packed sample -> ray
+  const float* z = nullptr;           // [M] world depth of the packed samples
+  const float* zlut_dense = nullptr;  // [K]
+  int K = 1;
+  float c[3] = {0.f, 0.f, 0.f};       // view_cell_center
+  float sqrt_max_depth = 1.0f;
+};
+
+// cudaFuncAttributeMaxDynamicSharedMemorySize is a per-device attribute: set it once per (kernel, device).
+// `done` is the caller's per-kernel bit mask (one static per launcher).
+cudaError_t set_max_dyn_smem_once(const void* func, int bytes, unsigned long long* done);
+
+// Launchers (defined in mlp.cu).  rows_dev may be null (then rows_host is used).  enc != nullptr: shading net with the
+// fused input encoder (in_tiles unused).
+cudaError_t launch_mlp(int nsplit, const MlpProgram& prog, const uint8_t* wblob, const uint8_t* in_tiles, float* out,
+                       const long long* rows_dev, long long rows_host, int* err_flag, int num_sms, cudaStream_t stream,
+                       const EncodeParams* enc = nullptr);
+cudaError_t launch_pack_rows(const float* x, long long rows, const long long* rows_dev, int n_feat,
+                             const InputLayout& lay, uint8_t* tiles, cudaStream_t stream);
+
+}  // namespace adn

@@ -1,5 +1,5 @@
 // Positional-encoding helpers shared by the feature kernels (stages.cu) and the shading MLP's fused input encoder
-// (mlp_umma.cu).
+// (mlp.cu).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>

@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, 1-D bulk async copy (TMA engine), tcgen05
-// (alloc / mma / commit / ld / fences) and shared-memory matrix descriptors.
+// Thin inline-PTX wrappers for sm_90a: mbarrier, 1-D bulk async copy (TMA engine), warpgroup MMA (wgmma)
+// and shared-memory matrix descriptors.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -63,25 +63,13 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   return ok != 0;
 }
 
-// Non-blocking probe (mbarrier.test_wait): used to overlap a barrier round trip with independent work.
-__device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.b32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-
 // Device-side watchdog: every wait is bounded so a protocol bug can never hang the GPU.
-// On timeout the kernel records the site in *err_flag and traps (the launch then reports an error).
+// On timeout the kernel records the site in *err_flag and traps (the launch then reports an error).  Inlined: a call
+// in a kernel that reallocates registers between warpgroups (setmaxnreg) makes ptxas's register allocation fail.
 #ifndef ADN_WATCHDOG_CYCLES
-#define ADN_WATCHDOG_CYCLES (4000000000ll)  // ~2 s at 1.9 GHz
+#define ADN_WATCHDOG_CYCLES (4000000000ll)  // ~2 s at 1.98 GHz
 #endif
-static __device__ __noinline__ void mbar_wait_slow(uint64_t* bar, uint32_t parity, int* err_flag, int site) {
+static __device__ __forceinline__ void mbar_wait_slow(uint64_t* bar, uint32_t parity, int* err_flag, int site) {
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
     if (clock64() - t0 > ADN_WATCHDOG_CYCLES) {
@@ -94,42 +82,6 @@ static __device__ __noinline__ void mbar_wait_slow(uint64_t* bar, uint32_t parit
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int* err_flag, int site) {
   if (mbar_try_wait(bar, parity)) return;
   mbar_wait_slow(bar, parity, err_flag, site);
-}
-// Polling variant (mbarrier.test_wait, no hardware suspend): lower wake-up latency, costs issue slots while waiting.
-static __device__ __noinline__ void mbar_spin_slow(uint64_t* bar, uint32_t parity, int* err_flag, int site) {
-  const long long t0 = clock64();
-  while (!mbar_test(bar, parity)) {
-    if (clock64() - t0 > ADN_WATCHDOG_CYCLES) {
-      if (err_flag) atomicExch(err_flag, 0x1000 + site);
-      __threadfence_system();
-      asm volatile("trap;");
-    }
-  }
-}
-__device__ __forceinline__ void mbar_spin(uint64_t* bar, uint32_t parity, int* err_flag, int site) {
-  if (mbar_test(bar, parity)) return;
-  mbar_spin_slow(bar, parity, err_flag, site);
-}
-
-// Warp-convergent wait on ONE MBARRIER PER LANE: every lane with `mine` set names its own barrier / parity, the warp
-// returns when all of them have completed.  Each iteration issues a single try_wait for all participating lanes
-// (divergent per-lane mbar_wait calls would be executed one lane after the other, ~200 cycles each).
-#ifndef ADN_SPIN_ISSUER
-#define ADN_SPIN_ISSUER 0   // 1: the issuer / forwarder warps poll with test_wait (no hardware suspend) -- experiment
-#endif
-__device__ __forceinline__ void mbar_wait_lanes(uint64_t* bar, uint32_t parity, bool mine, int* err_flag, int site) {
-  bool ok = !mine;
-  if (__all_sync(0xffffffffu, ok)) return;   // nothing to wait for (the early probe has seen it complete)
-  const long long t0 = clock64();
-  for (;;) {
-    if (!ok) ok = ADN_SPIN_ISSUER ? mbar_test(bar, parity) : mbar_try_wait(bar, parity);
-    if (__all_sync(0xffffffffu, ok)) break;
-    if (clock64() - t0 > ADN_WATCHDOG_CYCLES) {
-      if (err_flag) atomicExch(err_flag, 0x1000 + site);
-      __threadfence_system();
-      asm volatile("trap;");
-    }
-  }
 }
 
 // --------------------------------------------------------------------------- async bulk copy
@@ -155,149 +107,56 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
-// ---------------------------------------------------------------------------------- tcgen05
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// Register reallocation between warpgroups (all threads of a warpgroup execute it).
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc]; bf16 inputs, fp32 accumulate; issued by ONE thread.
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
+// ------------------------------------------------------------------------------------ wgmma
+// Warpgroup MMA (sm_90a): D[64 x 128] (fp32, registers) += A[64 x 16] * B[128 x 16]^T, A and B bf16 K-major in shared
+// memory, issued by all 128 threads of a warpgroup.  Accumulator fragment of thread t (warp w = t / 32, lane l):
+// d[4 i + j] is row 16 w + l / 4 + 8 (j >> 1), column 8 i + 2 (l % 4) + (j & 1).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp receives row (lane) i.
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
+// accumulate == 0: D = A * B (the registers' previous contents are ignored).
+__device__ __forceinline__ void wgmma_m64n128_bf16(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+        "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+        "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+        "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+        "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate)
       : "memory");
 }
 
-// ------------------------------------------------------------------------ CTA pairs (cta_group::2)
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of `smem_addr` (a shared::cta address) in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t smem_addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
-  return r;
-}
-// Relaxed remote arrive: a pure "event forwarded" signal.  (release.cluster would lower to MEMBAR.ALL.GPU -- ~1000
-// cycles -- and the forwarding warp has no data of its own to publish: the bytes it vouches for were made visible by
-// the mbarrier it has just acquired locally.)
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-template <int CG>
-__device__ __forceinline__ void tmem_alloc_cg(uint32_t* smem_dst, uint32_t ncols) {
-  if (CG == 2) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  } else {
-    tmem_alloc(smem_dst, ncols);
-    tmem_relinquish();
-  }
-}
-template <int CG>
-__device__ __forceinline__ void tmem_dealloc_cg(uint32_t taddr, uint32_t ncols) {
-  if (CG == 2) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-  } else {
-    tmem_dealloc(taddr, ncols);
-  }
-}
-// cta_group::2: D (both CTAs' TMEM) (+)= [A0; A1] * [B0; B1]^T -- each CTA supplies M/2 rows of A and N/2 rows of B
-// from the same shared-memory offsets; issued by ONE thread of the leader CTA.
-template <int CG>
-__device__ __forceinline__ void umma_bf16_cg(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  if (CG == 2) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else {
-    umma_bf16(d_tmem, a_desc, b_desc, idesc, accumulate);
-  }
-}
-// Same, A operand from tensor memory (each CTA's 128 rows x 16 bf16 = 8 columns of 32 bits at a_tmem): only B is read from
-// shared memory.
-__device__ __forceinline__ void umma_bf16_ts_cg2(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// commit: arrive on the mbarrier at this shared-memory offset in every CTA of the pair (mask 0b11)
-template <int CG>
-__device__ __forceinline__ void umma_commit_cg(uint64_t* bar) {
-  if (CG == 2) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)),
-                 "h"((unsigned short)3)
-                 : "memory");
-  } else {
-    umma_commit(bar);
-  }
-}
-
-// Shared-memory matrix descriptor, K-major operand, 128-byte swizzle, bf16:
+// Shared-memory matrix descriptor (sm_90 wgmma), K-major operand, 128-byte swizzle, bf16:
 // rows are 128 B (64 elements) apart, groups of 8 rows are 1024 B apart (SBO), the 16-byte chunk
 // index is XORed with (row % 8) by the hardware.  Tile base must be 1024-byte aligned; a K step of 16
 // elements advances the start address by 32 bytes.
-//   bits [0,14)  start address >> 4        bits [16,30) leading byte offset >> 4 (1 for swizzled K-major)
-//   bits [32,46) stride byte offset >> 4   bits [46,48) version = 1 (sm_100)
-//   bits [61,64) layout type: 2 = SWIZZLE_128B
+//   bits [0,14)  start address >> 4        bits [16,30) leading byte offset >> 4 (unused for swizzled K-major: 1)
+//   bits [32,46) stride byte offset >> 4   bits [62,64) layout type: 1 = SWIZZLE_128B
 __device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr_bytes & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>(1) << 16;
   d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
-}
-
-// Instruction descriptor for kind::f16 with bf16 A/B (both K-major), fp32 D, shape M x N.
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N) {
-  return (1u << 4) /*D=f32*/ | (1u << 7) /*A=bf16*/ | (1u << 10) /*B=bf16*/ | (uint32_t(N >> 3) << 17) |
-         (uint32_t(M >> 4) << 24);
 }
 
 // Byte offset of element (row, col) inside one [rows x 64] bf16 K-major SWIZZLE_128B block.

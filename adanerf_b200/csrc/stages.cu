@@ -4,7 +4,7 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 
-#include "mlp_umma.cuh"
+#include "mlp.cuh"
 #include "posenc.cuh"
 #include "ptx.cuh"
 #include "stages.cuh"
@@ -736,7 +736,7 @@ cudaError_t launch_stage3(const SceneDev& sc, const float* d_ray_o, const float*
   // n_samples is an upper bound (capacity) when d_total is given
   if (n_samples <= 0) return cudaSuccess;
   long long blocks = (n_samples + kTileM - 1) / kTileM;
-  const long long cap = 148ll * 64;
+  const long long cap = 132ll * 64;
   if (d_total && blocks > cap) blocks = cap;   // grid-stride when the true count lives on the device
   static unsigned long long attr_done = 0;   // per device
   if (set_max_dyn_smem_once(reinterpret_cast<const void*>(stage3_kernel), 2 * kBlkBytes, &attr_done) != cudaSuccess) return cudaGetLastError();

@@ -1,4 +1,4 @@
-"""Python host side of the B200 renderer: mirrors the call surface of the reference's
+"""Python host side of the H100 renderer: mirrors the call surface of the reference's
 `TrainConfig.inference` (src/train_data.py:278-299) as `render(rays, sampling_net, shading_net,
 adaptiveSamplingThreshold)` on top of the C ABI.  PyTorch is used only for device memory and streams."""
 import ctypes as C

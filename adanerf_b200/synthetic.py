@@ -2,6 +2,8 @@
 reference's shipped samples and random-init networks built in the construction order of the reference's classes
 (BaseNet.__init__ src/models.py:71-80, NeRF.__init__ src/models.py:226-250, ModelSelection order: net 0 then net 1),
 so a seed gives the reference's initial parameters.  Product-side helper: does not use anything under oracle/."""
+import os
+
 import torch
 
 # adanerf_real_time_viewer/sample/dataset_info.txt (Barbershop)
@@ -21,13 +23,25 @@ SCENE_PAVILLON = dict(
 SCENE_PAVILLON_NDC = dict(SCENE_PAVILLON, use_ndc=True, w=800, h=800)
 
 
-def load_weights_npz(path):
-    """(sampling, shading) state_dicts from an .npz with keys `sd0/<name>`, `sd1/<name>` (tests/golden/weights_pavillon.npz:
-    the initialisers of sample_pavillon_16/model{0,1}.onnx, the reference's shipped trained networks)."""
+def load_npz(path):
+    """{name: array} of an .npz, or of a directory of .npz parts (large fixtures are stored split so that no file exceeds
+    1 MB; the parts hold disjoint keys)."""
     import numpy as np
-    z = np.load(path, allow_pickle=False)
-    sd0 = {k[4:]: torch.from_numpy(z[k]) for k in z.files if k.startswith("sd0/")}
-    sd1 = {k[4:]: torch.from_numpy(z[k]) for k in z.files if k.startswith("sd1/")}
+    parts = [os.path.join(path, f) for f in sorted(os.listdir(path)) if f.endswith(".npz")] if os.path.isdir(path) else [path]
+    out = {}
+    for p in parts:
+        z = np.load(p, allow_pickle=False)
+        out.update({k: z[k] for k in z.files})
+    return out
+
+
+def load_weights_npz(path):
+    """(sampling, shading) state_dicts from an .npz (or a directory of .npz parts) with keys `sd0/<name>`, `sd1/<name>`
+    (tests/golden/weights_pavillon: the initialisers of sample_pavillon_16/model{0,1}.onnx, the reference's shipped trained
+    networks)."""
+    z = load_npz(path)
+    sd0 = {k[4:]: torch.from_numpy(v) for k, v in z.items() if k.startswith("sd0/")}
+    sd1 = {k[4:]: torch.from_numpy(v) for k, v in z.items() if k.startswith("sd1/")}
     return sd0, sd1
 
 

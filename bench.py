@@ -2,6 +2,7 @@
 """bench.py -- frames/s of the AdaNeRF hot path (BASELINE.json metric: frames/sec at 800x800 and rays/sec).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload NAME] [--single-process]
+                    [--dump-outputs DIR]
 
 A "step" is one pass of the whole hot path (rays -> sampling MLP -> threshold / compaction -> posenc -> shading MLP ->
 composite) over one frame of synthetic input: procedurally generated pinhole rays from the view-cell centre, random-init
@@ -18,6 +19,9 @@ checkpoints offline).
           4): STRONG scaling -- the 1600 x 1600 frame is fixed, rank r renders rows [1600 r / N, 1600 (r+1) / N).
   --single-process : N GPUs driven by ONE process through the multi-GPU C ABI (include/adanerf_b200_multi.h:
           ncclCommInitAll, grouped send / recv gather) instead of one torchrun rank per GPU.
+  --dump-outputs DIR : after the timed steps, write what the last timed step computed (the RGB frame, float32, of this
+          rank's band; rank 0's gathered frame at N > 1) as DIR/rgb.npy.  Inputs are seeded, so two builds can be compared
+          output for output.
   --impl reference : the reference's CPU path (the oracle port of TrainConfig.inference, torch CPU, all host threads); every
           step is a bounded ray sample of the same frame.
 """
@@ -31,6 +35,7 @@ import time
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
+sys.dont_write_bytecode = True   # the benchmark leaves the tree as it found it (it may be read-only)
 
 WORKLOADS = {
     # BASELINE.json configs[1]: 800x800, thr 0.2, K = 8 (~8 samples/ray with random-init nets: every ray saturates at K)
@@ -50,18 +55,17 @@ for _k in (8, 16):
         WORKLOADS[f"800x800_pav_thr{_t}_K{_k}"] = dict(W=800, H=800, thr=_t, K=_k, weights="pavillon", scaling="weak")
 FLOP_PER_SAMPLE_MLP1 = 1186816.0   # SURVEY.md 8(d): 2 * 593 408 MAC, unpadded
 FLOP_PER_RAY_MLP0 = 898048.0
-SHADING_KERNEL = "mlp_sh_kernel"
-PAVILLON_NPZ = os.path.join(ROOT, "tests", "golden", "weights_pavillon.npz")
+SHADING_KERNEL = "mlp_kernel"
+PAVILLON_NPZ = os.path.join(ROOT, "tests", "golden", "weights_pavillon")   # directory of .npz parts
 
 
 def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return dict(hbm_gbs=d.get("hbm_gbs", 6650.0), tflops=d.get("bf16_tflops", 1590.0), tflops_sustained=d.get("bf16_tflops_sustained", 1400.0),
-                    source="MEASURED_PEAKS.json (bf16_tflops: burst -- the kernel sits in a ~7 ms step inside a <0.5 s run; "
-                           "bf16_tflops_sustained for reference)")
-    return dict(hbm_gbs=6650.0, tflops=1590.0, tflops_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+        return dict(hbm_gbs=d.get("hbm_gbs", 3350.0), tflops=d.get("bf16_tflops", 989.0), source="MEASURED_PEAKS.json")
+    # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 -- upper bounds, not reached
+    return dict(hbm_gbs=3350.0, tflops=989.0, source="H100 SXM data sheet (dense BF16, 700 W)")
 
 
 def ncu_summary():
@@ -317,9 +321,7 @@ def run_ours(args, cfg, name):
     bands = [torch.empty((n_rays, 3), dtype=torch.float32, device="cuda") for _ in range(2)]
     frames = [torch.empty((world * n_rays, 3), dtype=torch.float32, device="cuda") for _ in range(2)] if world > 1 else None
     pending = [None, None]
-    # the gathered frame as per-rank tile views (dist.gather's gather_list); A/B modes: profiles/r2/gather_ab/ (8 GPUs, weak
-    # scaling: no collective 6.62 ms, gather to rank 0 6.70, all-gather 6.80 whether left in flight or not -- NCCL's kernel and the
-    # persistent MLP kernels do not share SMs)
+    # the gathered frame as per-rank tile views (dist.gather's gather_list); ADN_BENCH_GATHER selects A/B modes
     tiles = [list(f.view(world, n_rays, 3).unbind(0)) for f in frames] if world > 1 else None
     gather_mode = os.environ.get("ADN_BENCH_GATHER", "root")
 
@@ -365,6 +367,9 @@ def run_ours(args, cfg, name):
     e1.record()
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1)
+    if args.dump_outputs and (world == 1 or rank == 0):
+        last = (args.steps - 1) & 1
+        dump_outputs(args.dump_outputs, rgb=(frames if world > 1 else bands)[last])
     ms_by_rank = [ms / args.steps]
     if world > 1:
         t = torch.tensor([ms], device="cuda")
@@ -466,9 +471,8 @@ def run_ours(args, cfg, name):
             stage_ms=dict(zip(["stage0_features", "mlp0", "stage2_sample", "stage3_posenc", "mlp1", "stage5_composite"],
                               [round(float(x), 4) for x in stage_ms])),
             roofline=dict(kernel=f"{SHADING_KERNEL} (shading MLP, first chunk of the frame: {prof_rays} rays, {prof_samples} samples)", bound="tensor", achieved=achieved,
-                          peak=peaks["tflops"], unit="TFLOP/s", frac=achieved / peaks["tflops"],
-                          frac_of_sustained=achieved / peaks["tflops_sustained"], traffic=traffic,
-                          traffic_unit=f"bytes of DRAM read+write per launch (profiles/ncu_{tag}_summary.json, ncu --set full)",
+                          peak=peaks["tflops"], unit="TFLOP/s", frac=achieved / peaks["tflops"], traffic=traffic,
+                          traffic_unit=f"bytes of DRAM read+write per launch (profiles/ncu_{tag}_summary.json, ncu --set full)" if traffic else None,
                           peak_source=peaks["source"]),
             roofline_stages=stage_rooflines(stage_ms, prof_rays, prof_samples, thr, peaks, n_feat0=30 if cfg["weights"] == "ndc" else 90),
             cpu_baseline=dict(value=cpu["frames_per_s"], unit="frames/s", cores=cpu["cores"], kind="port", sample=cpu["sample"]),
@@ -517,9 +521,11 @@ def run_single_process(args, cfg, name):
     for _ in range(args.steps - 1):
         m.render_camera(pose, rot, W, Hn, thr, K)     # frame f + 1 enqueued before frame f is read
         m.wait_frame()
-    m.wait_frame()
+    last_frame = m.wait_frame()        # device view of the last timed frame, valid until the second next render
     secs = time.perf_counter() - t0
     clocks = sampler.stop()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, rgb=last_frame)
     render_ms, gather_ms = m.last_times()
     host = torch.empty((W * Hn, 3), dtype=torch.float32).pin_memory().numpy()   # caller-owned page-locked frame buffer
     t0 = time.perf_counter()
@@ -542,6 +548,15 @@ def run_single_process(args, cfg, name):
     m.close()
 
 
+def dump_outputs(d, **arrays):
+    """--dump-outputs: one float32 .npy per output array of the last timed step."""
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    for name, a in arrays.items():
+        a = a.detach().cpu().numpy() if hasattr(a, "detach") else np.asarray(a)
+        np.save(os.path.join(d, name + ".npy"), np.ascontiguousarray(a, dtype=np.float32))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -551,6 +566,7 @@ def main():
     ap.add_argument("--workload", default="800x800_thr0.2_K8", choices=sorted(WORKLOADS))
     ap.add_argument("--cpu-seconds", type=float, default=12.0, help="CPU baseline sample budget")
     ap.add_argument("--single-process", action="store_true", help="drive --gpus devices from one process (multi-GPU C ABI)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
     cfg = WORKLOADS[args.workload]
     if args.impl == "reference":

@@ -1,10 +1,10 @@
 /*
- * adanerf_b200 -- C ABI of the B200-native AdaNeRF inference renderer (libadanerf_b200.so).
+ * adanerf_b200 -- C ABI of the H100-native AdaNeRF inference renderer (libadanerf_b200.so).
  *
- * One data-parallel hot path, hand-written for sm_100a:
- *   rays -> SpherePosDir features -> sampling MLP (tcgen05, bf16x3 split precision)
+ * One data-parallel hot path, hand-written for sm_90a:
+ *   rays -> SpherePosDir features -> sampling MLP (wgmma, bf16x3 split precision)
  *        -> threshold / top-K / scan compaction -> positional encoding
- *        -> shading MLP (tcgen05, bf16) -> per-ray transmittance scan + alpha composite.
+ *        -> shading MLP (wgmma, bf16) -> per-ray transmittance scan + alpha composite.
  *
  * Each entry point cites the reference interface (relative to thomasneff/AdaNeRF) it replaces.
  * Conventions: plain pointers and sizes only; integer status codes (0 = ok), never exceptions;
@@ -12,7 +12,7 @@
  * owns packed weights and scratch; work is stream ordered (`stream` is a cudaStream_t passed as
  * void*, NULL = legacy default stream); no host synchronisation inside unless stated; one context
  * per device; a context is not thread safe.  There is NO CPU fallback: every call fails with
- * ADN_ERR_CUDA / ADN_ERR_NO_DEVICE when no sm_100 device is usable.
+ * ADN_ERR_CUDA / ADN_ERR_NO_DEVICE when no sm_90 device is usable.
  */
 #ifndef ADANERF_B200_H
 #define ADANERF_B200_H
@@ -106,10 +106,8 @@ adn_status adn_probe_export_dir(const char* dir, adn_scene* scene_out, float* th
 
 /* name: "chunk_rays" (rays per internal batch, 0 = auto), "profile" (0/1 per-stage event timing),
  * "mlp0_terms" (3 = bf16x3 split precision [default], 1 = plain bf16; parity experiments only),
- * "cta_group" (2 = CTA-pair MMAs [default], 1 = single-CTA MMAs; A/B runs),
- * "fuse_encoder" (1 = positional encoding of the samples inside the shading kernel: no [M,90]-sized tile buffer, ~5 %
- *   slower; 0 = separate kernel [default]),
- * "trace" (debug: net id whose MLP kernel records an in-kernel timeline, -1 = off; profiles/trace_mlp.py). */
+ * "fuse_encoder" (1 = positional encoding of the samples inside the shading kernel: no [M,90]-sized tile buffer;
+ *   0 = separate kernel [default]). */
 adn_status adn_set_option(adn_ctx* ctx, const char* name, int64_t value);
 adn_status adn_get_stats(adn_ctx* ctx, adn_stats* out);   /* synchronises the context's stream */
 

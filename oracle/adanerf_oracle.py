@@ -79,6 +79,23 @@ def posenc(v, n_freqs):
 # ----------------------------------------------------------------------------------------------
 # stage 0b: SpherePosDir.batch -- src/features.py:845-899, compute_ray_offset :769-791
 # ----------------------------------------------------------------------------------------------
+def _rotate(rot, dirs):
+    """rot [3,3] @ dirs [N,3]^T, transposed back.  fp32: the FMA chain of ATen's bmm, fma(r2, d2, fma(r1, d1, r0 d0)),
+    evaluated the same way on every host (a BLAS matmul picks its kernel, and so its rounding, by CPU).  The fp32
+    products are exact in fp64; the fp64 sum is rounded once more to fp32."""
+    if dirs.dtype != torch.float32:
+        return (rot @ dirs.T).T
+    r = rot.to(torch.float64)
+    d = dirs.to(torch.float64)
+    out = []
+    for i in range(3):
+        acc = (r[i, 0] * d[:, 0]).to(torch.float32).to(torch.float64)
+        acc = (r[i, 1] * d[:, 1] + acc).to(torch.float32).to(torch.float64)
+        acc = (r[i, 2] * d[:, 2] + acc).to(torch.float32)
+        out.append(acc)
+    return torch.stack(out, 0).T   # a [3, N] result seen transposed, like bmm's: reductions over it take the same path
+
+
 def stage0_sphere_pos_dir(pose, rot, dirs, scene, n_freq_pos=10, n_freq_dir=4):
     """pose [3], rot [3,3], dirs [N,3] -> x0 [N,90] (dir block FIRST), ray_o [N,3], ray_d [N,3]."""
     dt = dirs.dtype
@@ -86,7 +103,7 @@ def stage0_sphere_pos_dir(pose, rot, dirs, scene, n_freq_pos=10, n_freq_dir=4):
     # view_cell_radius is a float64 0-dim tensor in the reference (:761); r**2 then promotes like a
     # python scalar would, i.e. it is rounded to the working dtype when combined with fp32 tensors.
     r = float(np.linalg.norm(np.array(scene["view_cell_size"]) / 2.0))
-    nds = (rot @ dirs.T).T                                   # :858-859  bmm(rot, dirs^T)^T
+    nds = _rotate(rot, dirs)                                 # :858-859  bmm(rot, dirs^T)^T
     omc = pose - c                                           # :781
     u_dot = torch.sum(omc[None, :] * nds, dim=1)             # :784
     r_t = torch.tensor(r, dtype=torch.float64)

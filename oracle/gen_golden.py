@@ -32,10 +32,33 @@ def meta(**kw):
     return np.array(json.dumps(kw))
 
 
-def save(name, **arrays):
-    path = os.path.join(OUT, name)
-    np.savez_compressed(path, **arrays)
-    print(f"wrote {path}  ({os.path.getsize(path) / 1e6:.2f} MB)")
+def save(name, limit=900_000, **arrays):
+    """One compressed .npz; above `limit` bytes, a directory of parts with disjoint keys instead (no fixture file > 1 MB).
+    Read back with adanerf_b200.synthetic.load_npz."""
+    import io
+    sizes = {}
+    for k, v in arrays.items():
+        buf = io.BytesIO()
+        np.savez_compressed(buf, v=v)
+        sizes[k] = buf.tell()
+    if sum(sizes.values()) <= limit:
+        path = os.path.join(OUT, name)
+        np.savez_compressed(path, **arrays)
+        print(f"wrote {path}  ({os.path.getsize(path) / 1e6:.2f} MB)")
+        return
+    d = os.path.join(OUT, name[:-4] if name.endswith(".npz") else name)
+    os.makedirs(d, exist_ok=True)
+    parts, cur, size = [], [], 0
+    for k in arrays:
+        if cur and size + sizes[k] > limit:
+            parts.append(cur)
+            cur, size = [], 0
+        cur.append(k)
+        size += sizes[k]
+    parts.append(cur)
+    for i, keys in enumerate(parts):
+        np.savez_compressed(os.path.join(d, f"part{i}.npz"), **{k: arrays[k] for k in keys})
+    print(f"wrote {d}/part0..{len(parts) - 1}.npz")
 
 
 def stage_case(name, scene_name, scene, sd0, sd1, K, thr, n_rays, stride, pose_off, rot, keep_x1, w=800, h=800, ndc=False):

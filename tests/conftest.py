@@ -2,9 +2,7 @@ import json
 import os
 import sys
 
-import numpy as np
 import pytest
-import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
@@ -13,21 +11,21 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def load_golden(name):
-    z = np.load(os.path.join(GOLDEN, name + ".npz"), allow_pickle=False)
-    d = {k: z[k] for k in z.files}
+    """tests/golden/<name>.npz, or the directory tests/golden/<name>/ of its parts (fixtures above 1 MB are split)."""
+    from adanerf_b200.synthetic import load_npz
+    p = os.path.join(GOLDEN, name)
+    d = load_npz(p if os.path.isdir(p) else p + ".npz")
     d["meta"] = json.loads(str(d["meta"]))
     return d
 
 
 def load_pavillon_weights():
-    z = np.load(os.path.join(GOLDEN, "weights_pavillon.npz"), allow_pickle=False)
-    sd0 = {k[4:]: torch.from_numpy(z[k]) for k in z.files if k.startswith("sd0/")}
-    sd1 = {k[4:]: torch.from_numpy(z[k]) for k in z.files if k.startswith("sd1/")}
-    return sd0, sd1
+    from adanerf_b200.synthetic import load_weights_npz
+    return load_weights_npz(os.path.join(GOLDEN, "weights_pavillon"))
 
 
 def case_weights(case):

@@ -1,4 +1,4 @@
-"""CPU-side checks: the C-ABI library builds for sm_100a, loads, and exports every symbol the header
+"""CPU-side checks: the C-ABI library builds for sm_90a, loads, and exports every symbol the header
 declares; the product path fails loudly without a GPU (no CPU fallback)."""
 import ctypes
 import os
@@ -39,8 +39,8 @@ def test_multi_library_exports_every_header_symbol():
         assert hasattr(mlib, s), s
 
 
-def test_sass_is_blackwell_native():
-    """tcgen05.mma -> UTCHMMA, tcgen05.ld -> LDTM, bulk async copy -> UBLKCP (B200_PROFILING.md)."""
+def test_sass_is_hopper_native():
+    """wgmma.mma_async -> HGMMA, bulk async copy -> UBLKCP."""
     import shutil
     import subprocess
     import __graft_entry__ as g
@@ -48,8 +48,8 @@ def test_sass_is_blackwell_native():
     if not os.path.exists(cuobjdump):
         pytest.skip("cuobjdump not available")
     sass = subprocess.run([cuobjdump, "-sass", g.LIB], capture_output=True, text=True).stdout
-    assert "sm_100a" in sass
-    for mnemonic in ("UTCHMMA", "LDTM", "UBLKCP"):
+    assert "sm_90a" in sass
+    for mnemonic in ("HGMMA", "UBLKCP"):
         assert mnemonic in sass, mnemonic
     assert "HMMA.16816" not in sass  # no legacy mma.sync path
 

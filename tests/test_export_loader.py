@@ -55,11 +55,13 @@ def test_cxx_loader_errors(lib, tmp_path):
     assert lib.adn_probe_export_dir(str(d).encode(), None, None, None, None) == 5
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/adanerf_real_time_viewer/sample"), reason="reference not mounted")
 def test_cxx_loader_reads_shipped_sample(lib):
+    """The reference viewer's shipped sample export directory (tests/golden/viewer_sample: its config.ini and
+    dataset_info.txt, the networks shrunk to one row per initialiser by oracle/gen_live_golden.py)."""
     from adanerf_b200._lib import Scene
     sc, thr, k, n = Scene(), C.c_float(), C.c_int(), (C.c_int * 2)()
-    st = lib.adn_probe_export_dir(b"/root/reference/adanerf_real_time_viewer/sample", C.byref(sc), C.byref(thr), C.byref(k), n)
+    sample = os.path.join(ROOT, "tests", "golden", "viewer_sample").encode()
+    st = lib.adn_probe_export_dir(sample, C.byref(sc), C.byref(thr), C.byref(k), n)
     assert st == 0 and k.value == 4 and abs(thr.value - 0.15) < 1e-7 and list(n) == [16, 24]
     np.testing.assert_allclose(list(sc.view_cell_center), [2.25, 7.75, 1.5])
 

@@ -1,12 +1,12 @@
 """Pins oracle/adanerf_oracle.py against fixtures produced by the unmodified reference
-(oracle/gen_golden.py), and -- when /root/reference is mounted -- against the live reference."""
+(oracle/gen_golden.py), and against the reference's end-to-end runs on fresh seeds (oracle/gen_live_golden.py)."""
 import numpy as np
 import pytest
 import torch
 
 from conftest import load_golden, case_weights
 from oracle import adanerf_oracle as orc
-from oracle import ref_harness as rh
+from oracle.gen_live_golden import FRESH_SEEDS, digest, fresh_seed_inputs
 
 CASES = ["pav_k8_t0.2", "pav_k8_t0.5", "pav_k16_t0.15", "shaped_k8_t0.2", "rand_k8_t0.2", "ndc_k16_t0.15"]
 
@@ -130,26 +130,29 @@ def test_weight_init_is_reproducible():
     assert a1["views_linears.0.weight"].shape == (128, 283)
 
 
-@pytest.mark.skipif(not rh.available(), reason="/root/reference not mounted (GPU box)")
-@pytest.mark.parametrize("seed,K,thr", [(11, 8, 0.2), (12, 4, 0.05), (13, 16, 0.3)])
+@pytest.mark.parametrize("seed,K,thr", FRESH_SEEDS)
 def test_live_reference_fresh_seed(seed, K, thr):
-    scene = orc.SCENE_BARBERSHOP
-    ref = rh.RefRenderer(scene, K=K, thr=thr, seed=seed)
-    sd0, sd1 = orc.make_weights("rand", seed=seed)
-    assert all(torch.equal(sd0[k], v) for k, v in ref.models[0].state_dict().items())
-    assert all(torch.equal(sd1[k], v) for k, v in ref.models[1].state_dict().items())
-    # shape the sampling net so counts are ragged, then load the same weights into the reference
-    sd0["layers.7.weight"] *= 0.15
-    sd0["layers.7.bias"] = sd0["layers.7.bias"] * 0.15 - 0.2
-    ref.load_state_dicts(sd0, sd1)
-    g = torch.Generator().manual_seed(seed)
-    dirs = torch.from_numpy(orc.generate_ray_directions(800, 800, scene["fov"]).reshape(-1, 3)).float()
-    dirs = dirs[torch.randperm(dirs.shape[0], generator=g)[:512]]
-    pose = torch.tensor(scene["view_cell_center"]) + 0.1 * torch.randn(3, generator=g)
-    rot = orc.rotation_yaw(float(seed * 17))
-    st = ref.stages(pose, rot, dirs)
+    """The reference's own end-to-end run on a fresh seed (tests/golden/live_fresh_seed.npz, oracle/gen_live_golden.py):
+    its initialisation (as digests) and its raw0 / sample counts / image / weights -- bit for bit where the host's CPU
+    GEMMs round like the recording host's (raw0 identical), otherwise within the cross-host bounds of
+    test_end_to_end_matches_reference."""
+    g = load_golden("live_fresh_seed")
+    scene, pose, rot, dirs, sd0, sd1 = fresh_seed_inputs(seed)
+    init0, init1 = orc.make_weights("rand", seed=seed)
+    for i, sd in enumerate((init0, init1)):
+        keys = [k.split("/", 2)[2] for k in g if k.startswith(f"{seed}/init{i}/")]
+        assert sorted(keys) == sorted(sd)
+        assert all(digest(sd[k]) == str(g[f"{seed}/init{i}/{k}"]) for k in keys)
+    st = {k: g[f"{seed}/{k}"] for k in ("raw0", "asp", "rgb", "weights")}
     o = orc.render_rays(pose, rot, dirs, sd0, sd1, scene, thr, K, return_stages=True)
-    np.testing.assert_array_equal(o["raw0"].numpy(), st["raw0"])
+    if not np.array_equal(o["raw0"].numpy(), st["raw0"]):
+        # GEMM rounding differs between hosts (oneMKL kernel selection): close, and a borderline cell may flip a ray
+        np.testing.assert_allclose(o["raw0"].numpy(), st["raw0"], rtol=0, atol=5e-4)
+        same = (o["asp"].numpy() == st["asp"])
+        assert same.mean() > 0.98
+        assert np.abs(o["rgb"].numpy() - st["rgb"])[same].max() < 2e-3
+        assert orc.psnr(o["rgb"].numpy()[same], st["rgb"][same]) > 60.0
+        return
     np.testing.assert_array_equal(o["asp"].numpy(), st["asp"])
     np.testing.assert_array_equal(o["rgb"].numpy(), st["rgb"])
     np.testing.assert_array_equal(o["weights"].numpy(), st["weights"])
