@@ -56,8 +56,13 @@ struct adn_ctx {
   int64_t chunk_rays = 0;
   bool profile = false;
   int weight_copies = 1;   // replicas of each packed weight blob (MlpProgram::w_copies)
+  int64_t sample_budget = 0;      // B of adn_set_option "sample_budget" (0 = off)
+  bool last_budget = false;       // the last render chose its threshold on the device (in budget_thr)
+  float last_thr = 0.0f;          // the last render's threshold argument
+  bool prof_budget = false;       // the profiled render timed the selection with stage 2 (ev[7] -> ev[3])
   // scratch
   Buf tiles0, raw0, x0, ray_o, ray_d, dirs, count, offset, rayidx, zbuf, zpbuf, tiles1, raw1, s2scratch, rgb, rgba, x1, metric;
+  Buf budget_keys, budget_work, budget_thr;   // sample budget: candidate keys, histograms + select state, t*
   long long* d_total = nullptr;
   int* d_err = nullptr;           // device view of h_err
   int* h_err = nullptr;           // watchdog flag in mapped pinned host memory: still readable after a device trap
@@ -462,18 +467,38 @@ adn_status run_mlp(adn_ctx* ctx, int id, const uint8_t* tiles, float* out, const
   return ADN_OK;
 }
 
-// The whole hot path for one chunk of rays, stream ordered, no host synchronisation.
+enum { kStages01 = 1, kStages25 = 2 };
+
+// The hot path for one chunk of rays, stream ordered, no host synchronisation.  `parts`: kStages01 = stage 0 + sampling MLP
+// (writes the chunk's raw0 / ray_o / ray_d), kStages25 = stages 2-5 (reads them).  d_thr: stage 2's threshold as a device
+// float (sample budget), null = `thr`.
 adn_status render_chunk(adn_ctx* ctx, const PoseDev& pd, const float* d_dirs, const CameraRays* cam, int64_t n, float thr,
-                        int K, float* d_rgb, uint8_t* d_rgba8, int32_t* d_nsamples, float* d_oracle_w, const Stage5Aux& aux,
-                        cudaStream_t st, bool timing) {
+                        int K, float* d_rgb, uint8_t* d_rgba8, int32_t* d_nsamples, float* raw0, float* ray_o, float* ray_d,
+                        const float* d_thr, const Stage5Aux& aux, cudaStream_t st, bool timing, int parts) {
   const bool dense = (thr == 0.0f);
   const int64_t cap = n * K;
   adn_status s;
   Net& n0 = ctx->net[0];
-  if ((s = ensure(ctx, ctx->tiles0, size_t(pad128(n) / 128) * n0.prog.in_tile_stride)) != ADN_OK) return s;
-  if (!d_oracle_w && (s = ensure(ctx, ctx->raw0, size_t(n) * 128 * 4)) != ADN_OK) return s;
-  if ((s = ensure(ctx, ctx->ray_o, size_t(n) * 12)) != ADN_OK) return s;
-  if ((s = ensure(ctx, ctx->ray_d, size_t(n) * 12)) != ADN_OK) return s;
+  if (parts & kStages01) {
+    if ((s = ensure(ctx, ctx->tiles0, size_t(pad128(n) / 128) * n0.prog.in_tile_stride)) != ADN_OK) return s;
+    uint8_t* tiles0 = static_cast<uint8_t*>(ctx->tiles0.p);
+    if (timing) cudaEventRecord(ctx->ev[0], st);
+    // stage 0
+    if (n0.nsplit == 2 && (n0.n_in == 90 || n0.n_in == 30) && n0.n_in == ctx->n_feat0) {   // stage 0 writes the packed hi / lo tiles itself
+      ADN_CUDA(ctx, launch_stage0(ctx->sc, pd, d_dirs, cam, n, nullptr, ray_o, ray_d, tiles0, st));
+      ctx->stats.kernel_launches++;
+    } else {
+      if ((s = ensure(ctx, ctx->x0, size_t(n) * ctx->n_feat0 * 4)) != ADN_OK) return s;
+      ADN_CUDA(ctx, launch_stage0(ctx->sc, pd, d_dirs, cam, n, static_cast<float*>(ctx->x0.p), ray_o, ray_d, nullptr, st));
+      ADN_CUDA(ctx, launch_pack_rows(static_cast<float*>(ctx->x0.p), n, nullptr, ctx->n_feat0, n0.lay, tiles0, st));
+      ctx->stats.kernel_launches += 2;
+    }
+    if (timing) cudaEventRecord(ctx->ev[1], st);
+    // stage 1
+    if ((s = run_mlp(ctx, 0, tiles0, raw0, nullptr, n, st)) != ADN_OK) return s;
+    if (timing) cudaEventRecord(ctx->ev[2], st);
+  }
+  if (!(parts & kStages25)) return ADN_OK;
   if ((s = ensure(ctx, ctx->count, size_t(n) * 4)) != ADN_OK) return s;
   if ((s = ensure(ctx, ctx->offset, size_t(n) * 4)) != ADN_OK) return s;
   if (!dense) {
@@ -487,37 +512,18 @@ adn_status render_chunk(adn_ctx* ctx, const PoseDev& pd, const float* d_dirs, co
   if (!fused_enc && (s = ensure(ctx, ctx->tiles1, size_t(pad128(cap) / 128) * 2 * kBlkBytes)) != ADN_OK) return s;
   if ((s = ensure(ctx, ctx->raw1, size_t(pad128(cap)) * 16)) != ADN_OK) return s;
 
-  float* raw0 = d_oracle_w ? d_oracle_w : static_cast<float*>(ctx->raw0.p);
   int32_t* count = d_nsamples ? d_nsamples : static_cast<int32_t*>(ctx->count.p);
   int32_t* offset = static_cast<int32_t*>(ctx->offset.p);
-  float* ray_o = static_cast<float*>(ctx->ray_o.p);
-  float* ray_d = static_cast<float*>(ctx->ray_d.p);
-  uint8_t* tiles0 = static_cast<uint8_t*>(ctx->tiles0.p);
   uint8_t* tiles1 = static_cast<uint8_t*>(ctx->tiles1.p);   // null / stale when the encoder is fused
   float* raw1 = static_cast<float*>(ctx->raw1.p);
 
-  if (timing) cudaEventRecord(ctx->ev[0], st);
-  // stage 0
-  if (n0.nsplit == 2 && (n0.n_in == 90 || n0.n_in == 30) && n0.n_in == ctx->n_feat0) {   // stage 0 writes the packed hi / lo tiles itself
-    ADN_CUDA(ctx, launch_stage0(ctx->sc, pd, d_dirs, cam, n, nullptr, ray_o, ray_d, tiles0, st));
-    ctx->stats.kernel_launches++;
-  } else {
-    if ((s = ensure(ctx, ctx->x0, size_t(n) * ctx->n_feat0 * 4)) != ADN_OK) return s;
-    ADN_CUDA(ctx, launch_stage0(ctx->sc, pd, d_dirs, cam, n, static_cast<float*>(ctx->x0.p), ray_o, ray_d, nullptr, st));
-    ADN_CUDA(ctx, launch_pack_rows(static_cast<float*>(ctx->x0.p), n, nullptr, ctx->n_feat0, n0.lay, tiles0, st));
-    ctx->stats.kernel_launches += 2;
-  }
-  if (timing) cudaEventRecord(ctx->ev[1], st);
-  // stage 1
-  if ((s = run_mlp(ctx, 0, tiles0, raw0, nullptr, n, st)) != ADN_OK) return s;
-  if (timing) cudaEventRecord(ctx->ev[2], st);
   // stage 2
   if (dense) {
     ADN_CUDA(ctx, launch_stage2_dense(n, K, count, offset, ctx->d_total, st));
   } else {
     ADN_CUDA(ctx, launch_stage2(raw0, n, thr, K, ctx->d_zlut, count, offset, nullptr, static_cast<int32_t*>(ctx->rayidx.p),
                                 static_cast<float*>(ctx->zbuf.p), static_cast<float*>(ctx->zpbuf.p), ctx->d_total,
-                                ctx->s2scratch.p, &ctx->s2sync, st));
+                                ctx->s2scratch.p, &ctx->s2sync, st, d_thr));
   }
   ctx->stats.kernel_launches++;
   if (timing) cudaEventRecord(ctx->ev[3], st);
@@ -558,6 +564,16 @@ adn_status render_impl(adn_ctx* ctx, const float* pose, const float* rot, const 
     return fail(ctx, ADN_ERR_INVALID, "render: sampling net must be " + std::to_string(ctx->n_feat0) + " -> 128 for this scene's encoding");
   if (K < 1 || K > 128 || thr < 0.0f) return fail(ctx, ADN_ERR_INVALID, "render: need 1 <= K <= 128 and thr >= 0");
   if (thr == 0.0f && K != 128) return fail(ctx, ADN_ERR_INVALID, "render: dense mode (thr == 0) needs K == 128 (one sample per depth cell)");
+  const int64_t budget = ctx->sample_budget;
+  if (budget > 0 && thr == 0.0f)
+    return fail(ctx, ADN_ERR_INVALID, "render: sample_budget needs the adaptive path (thr > 0 is the floor threshold), not dense mode");
+  if (budget > 0 && budget < n_rays)
+    return fail(ctx, ADN_ERR_INVALID, "render: sample_budget " + std::to_string(budget) + " is below the " + std::to_string(n_rays) +
+                                          " rays of the call (every ray keeps at least one sample)");
+  if (budget > 0 && n_rays * (K - 1) >= (int64_t(1) << 32))
+    return fail(ctx, ADN_ERR_INVALID, "render: sample_budget supports at most 2^32 - 1 candidate samples (N * (K - 1)) per call");
+  if (budget > 0 && (reinterpret_cast<uintptr_t>(d_oracle_w) & 15u))
+    return fail(ctx, ADN_ERR_INVALID, "render: sample_budget needs 16-byte aligned d_oracle_weights rows");
   if (n_rays == 0) return ADN_OK;
   if (ctx->scene.use_ndc) {
     // image size behind ndc_rays: the frame being rendered (viewer, featureset.cpp:83-84) or the dataset's (features.py:350-351,430)
@@ -577,8 +593,21 @@ adn_status render_impl(adn_ctx* ctx, const float* pose, const float* rot, const 
   if (cam && chunk % cam->W) chunk = (chunk / cam->W + 1) * cam->W;  // whole rows per chunk
   const PoseDev pd = make_pose(pose, rot);
   ctx->stats.n_rays = n_rays;
-  for (int64_t r0 = 0; r0 < n_rays; r0 += chunk) {
+  ctx->last_budget = budget > 0;
+  ctx->last_thr = thr;
+  if (ctx->profile) ctx->prof_budget = budget > 0;
+  // raw0 / ray_o / ray_d: one chunk's worth, or with a sample budget the whole call's (the threshold is chosen over all of
+  // raw0 before any chunk runs stage 2)
+  const int64_t span = budget > 0 ? n_rays : std::min(chunk, n_rays);
+  if (!d_oracle_w && (s = ensure(ctx, ctx->raw0, size_t(span) * 128 * 4)) != ADN_OK) return s;
+  if ((s = ensure(ctx, ctx->ray_o, size_t(span) * 12)) != ADN_OK) return s;
+  if ((s = ensure(ctx, ctx->ray_d, size_t(span) * 12)) != ADN_OK) return s;
+  float* raw0 = d_oracle_w ? d_oracle_w : static_cast<float*>(ctx->raw0.p);
+  float* ray_o = static_cast<float*>(ctx->ray_o.p);
+  float* ray_d = static_cast<float*>(ctx->ray_d.p);
+  auto run = [&](int64_t r0, int parts, const float* d_thr) -> adn_status {
     const int64_t n = std::min(chunk, n_rays - r0);
+    const int64_t w = budget > 0 ? r0 : 0;   // window of raw0 / ray_o / ray_d
     CameraRays c{};
     if (cam) {
       c = *cam;
@@ -597,11 +626,30 @@ adn_status render_impl(adn_ctx* ctx, const float* pose, const float* rot, const 
       aux.dr_min = ctx->scene.depth_range[0];
       aux.log_range = float(std::log(double(ctx->scene.depth_range[1]) - double(ctx->scene.depth_range[0]) + 1.0));
     }
-    s = render_chunk(ctx, pd, d_dirs ? d_dirs + 3 * r0 : nullptr, cam ? &c : nullptr, n, thr, K, d_rgb ? d_rgb + 3 * r0 : nullptr,
-                     d_rgba8 ? d_rgba8 + 4 * r0 : nullptr, d_nsamples ? d_nsamples + r0 : nullptr,
-                     d_oracle_w ? d_oracle_w + 128 * r0 : nullptr, aux, st, ctx->profile && r0 == 0);
-    if (s != ADN_OK) return s;
+    return render_chunk(ctx, pd, d_dirs ? d_dirs + 3 * r0 : nullptr, cam ? &c : nullptr, n, thr, K, d_rgb ? d_rgb + 3 * r0 : nullptr,
+                        d_rgba8 ? d_rgba8 + 4 * r0 : nullptr, d_nsamples ? d_nsamples + r0 : nullptr,
+                        d_oracle_w ? d_oracle_w + 128 * r0 : raw0 + 128 * w, ray_o + 3 * w, ray_d + 3 * w, d_thr, aux, st,
+                        ctx->profile && r0 == 0, parts);
+  };
+  if (budget == 0) {
+    for (int64_t r0 = 0; r0 < n_rays; r0 += chunk)
+      if ((s = run(r0, kStages01 | kStages25, nullptr)) != ADN_OK) return s;
+    return ADN_OK;
   }
+  // sample budget: stages 0-1 of every chunk, one threshold for the call, stages 2-5 of every chunk
+  if ((s = ensure(ctx, ctx->budget_keys, size_t(std::max<int64_t>(1, n_rays * (K - 1))) * 4)) != ADN_OK) return s;
+  if ((s = ensure(ctx, ctx->budget_work, budget_work_bytes())) != ADN_OK) return s;
+  if ((s = ensure(ctx, ctx->budget_thr, sizeof(float))) != ADN_OK) return s;
+  float* d_thr = static_cast<float*>(ctx->budget_thr.p);
+  for (int64_t r0 = 0; r0 < n_rays; r0 += chunk)
+    if ((s = run(r0, kStages01, nullptr)) != ADN_OK) return s;
+  if (ctx->profile) cudaEventRecord(ctx->ev[7], st);   // the selection is timed with stage 2 of the first chunk
+  int launches = 0;
+  ADN_CUDA(ctx, launch_budget_threshold(raw0, n_rays, thr, K, budget, static_cast<uint32_t*>(ctx->budget_keys.p), ctx->budget_work.p,
+                                        d_thr, ctx->num_sms, st, &launches));
+  ctx->stats.kernel_launches += launches;
+  for (int64_t r0 = 0; r0 < n_rays; r0 += chunk)
+    if ((s = run(r0, kStages25, d_thr)) != ADN_OK) return s;
   return ADN_OK;
 }
 
@@ -694,7 +742,8 @@ void adn_destroy(adn_ctx* ctx) {
   cudaSetDevice(ctx->device);
   cudaDeviceSynchronize();
   Buf* bufs[] = {&ctx->tiles0, &ctx->raw0, &ctx->x0,    &ctx->ray_o,  &ctx->ray_d, &ctx->dirs,      &ctx->count, &ctx->offset,
-                 &ctx->rayidx, &ctx->zbuf, &ctx->zpbuf, &ctx->tiles1, &ctx->raw1,  &ctx->s2scratch, &ctx->rgb,   &ctx->rgba, &ctx->x1, &ctx->metric};
+                 &ctx->rayidx, &ctx->zbuf, &ctx->zpbuf, &ctx->tiles1, &ctx->raw1,  &ctx->s2scratch, &ctx->rgb,   &ctx->rgba, &ctx->x1, &ctx->metric,
+                 &ctx->budget_keys, &ctx->budget_work, &ctx->budget_thr};
   for (Buf* b : bufs)
     if (b->p) cudaFree(b->p);
   for (auto& r : ctx->regs)
@@ -748,6 +797,11 @@ adn_status adn_set_option(adn_ctx* ctx, const char* name, int64_t value) {
     ctx->profile = value != 0;
     return ADN_OK;
   }
+  if (n == "sample_budget") {   // B > 0: adaptive renders choose their threshold (>= thr) so that M <= B; 0 (default): off
+    if (value < 0) return fail(ctx, ADN_ERR_INVALID, "sample_budget must be >= 0");
+    ctx->sample_budget = value;
+    return ADN_OK;
+  }
   if (n == "fuse_encoder") {   // 1: positional encoding inside the shading kernel (no tile buffer); 0 (default): stage3_kernel + packed tiles
     ctx->fuse_encoder = value != 0;
     return ADN_OK;
@@ -776,10 +830,22 @@ adn_status adn_get_stats(adn_ctx* ctx, adn_stats* out) {
   if (ctx->profile) {
     for (int i = 0; i < 6; ++i) {
       float ms = 0;
-      if (cudaEventElapsedTime(&ms, ctx->ev[i], ctx->ev[i + 1]) == cudaSuccess) ctx->stats.ms_stage[i] = ms;
+      // with a sample budget, stage 2's slot starts at the threshold selection (ev[7])
+      const cudaEvent_t from = (i == 2 && ctx->prof_budget) ? ctx->ev[7] : ctx->ev[i];
+      if (cudaEventElapsedTime(&ms, from, ctx->ev[i + 1]) == cudaSuccess) ctx->stats.ms_stage[i] = ms;
     }
   }
   *out = ctx->stats;
+  return ADN_OK;
+}
+
+adn_status adn_last_threshold(adn_ctx* ctx, float* thr_out) {
+  if (!ctx || !thr_out) return fail(ctx, ADN_ERR_INVALID, "last_threshold: bad arguments");
+  ADN_CUDA(ctx, cudaSetDevice(ctx->device));
+  adn_status s = check_device_error(ctx);   // synchronises, like adn_get_stats
+  if (s != ADN_OK) return s;
+  if (ctx->last_budget) ADN_CUDA(ctx, cudaMemcpy(thr_out, ctx->budget_thr.p, sizeof(float), cudaMemcpyDeviceToHost));
+  else *thr_out = ctx->last_thr;
   return ADN_OK;
 }
 
@@ -983,6 +1049,23 @@ adn_status adn_stage2_sample(adn_ctx* ctx, const float* d_raw0, int64_t n_rays, 
   ADN_CUDA(ctx, launch_stage2(d_raw0, n_rays, thr, K, ctx->d_zlut, d_count, d_offset, d_cell, d_ray, d_z, d_zp,
                               reinterpret_cast<long long*>(d_total), ctx->s2scratch.p, &ctx->s2sync, static_cast<cudaStream_t>(stream)));
   ctx->stats.kernel_launches++;
+  return ADN_OK;
+}
+
+adn_status adn_budget_threshold(adn_ctx* ctx, const float* d_raw0, int64_t n_rays, float thr_min, int K, int64_t max_samples,
+                                float* d_thr, void* stream) {
+  if (!ctx || !d_thr || n_rays < 0 || (n_rays > 0 && !d_raw0) || K < 1 || K > 128 || !(thr_min > 0.0f) || max_samples < n_rays)
+    return fail(ctx, ADN_ERR_INVALID, "budget_threshold: bad arguments (need thr_min > 0, 1 <= K <= 128, max_samples >= n_rays)");
+  if (n_rays * (K - 1) >= (int64_t(1) << 32))
+    return fail(ctx, ADN_ERR_INVALID, "budget_threshold: at most 2^32 - 1 candidate samples (N * (K - 1))");
+  if (reinterpret_cast<uintptr_t>(d_raw0) & 15u) return fail(ctx, ADN_ERR_INVALID, "budget_threshold: d_raw0 must be 16-byte aligned");
+  ADN_CUDA(ctx, cudaSetDevice(ctx->device));
+  adn_status s = ensure(ctx, ctx->budget_keys, size_t(std::max<int64_t>(1, n_rays * (K - 1))) * 4);
+  if (s != ADN_OK || (s = ensure(ctx, ctx->budget_work, budget_work_bytes())) != ADN_OK) return s;
+  int launches = 0;
+  ADN_CUDA(ctx, launch_budget_threshold(d_raw0, n_rays, thr_min, K, max_samples, static_cast<uint32_t*>(ctx->budget_keys.p),
+                                        ctx->budget_work.p, d_thr, ctx->num_sms, static_cast<cudaStream_t>(stream), &launches));
+  ctx->stats.kernel_launches += launches;
   return ADN_OK;
 }
 

@@ -77,6 +77,20 @@ bool ImageGenerator::inference_host(const Camera& camera, float* h_rgb, int batc
   return s == ADN_OK;
 }
 
+bool ImageGenerator::set_sample_budget(int64_t max_samples) {
+  if (!ctx_) return false;
+  const adn_status s = adn_set_option(ctx_, "sample_budget", max_samples);
+  if (s != ADN_OK) err_ = adn_last_error(ctx_);
+  return s == ADN_OK;
+}
+
+bool ImageGenerator::last_threshold(float* thr) {
+  if (!ctx_) return false;
+  const adn_status s = adn_last_threshold(ctx_, thr);
+  if (s != ADN_OK) err_ = adn_last_error(ctx_);
+  return s == ADN_OK;
+}
+
 const char* ImageGenerator::last_error() const { return err_.c_str(); }
 
 bool ImageGenerator::stats(adn_stats* out) { return ctx_ && adn_get_stats(ctx_, out) == ADN_OK; }

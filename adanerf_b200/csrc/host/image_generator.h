@@ -60,6 +60,11 @@ class ImageGenerator {
   // Same into a host fp32 buffer [W*H*3] (copies inside).
   bool inference_host(const Camera& camera, float* h_rgb, int batch_size, int num_samples, int32_t* h_nsamples = nullptr);
 
+  // Frame-cost control (adn_set_option "sample_budget"): at most `max_samples` samples per inference call, the config's
+  // adaptiveSamplingThreshold being the floor; 0 = off.  last_threshold(): the threshold the last frame used (synchronises).
+  bool set_sample_budget(int64_t max_samples);
+  bool last_threshold(float* thr);
+
   const char* last_error() const;
   bool stats(adn_stats* out);
 

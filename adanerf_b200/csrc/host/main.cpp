@@ -22,6 +22,7 @@ class Encoding {};
 int main(int argc, char** argv) {
   std::string model = "sample/";
   int W = 800, H = 800, batch = -1, frames = 20, device = 0, gpus = 1;
+  long long budget = 0;   // --budget: samples per frame (0 = fixed threshold)
   bool write = false, surface = false;
   for (int i = 1; i < argc; ++i) {
     const std::string a = argv[i];
@@ -32,12 +33,14 @@ int main(int argc, char** argv) {
     else if (a == "-w" || a == "--writeImages") write = true;
     else if (a == "--surface") surface = true;   // one frame through ImageGenerator::inference(camera, cudaSurfaceObject_t, ...)
     else if ((a == "-g" || a == "--gpus") && i + 1 < argc) gpus = std::atoi(argv[++i]);
+    else if (a == "--budget" && i + 1 < argc) budget = std::atoll(argv[++i]);
     else if (a[0] != '-') model = a;
-    else { std::fprintf(stderr, "usage: %s modelPath [-s W H] [-bs raysPerBatch] [-f frames] [-dev id] [-g gpus] [--surface] [-w]\n", argv[0]); return 2; }
+    else { std::fprintf(stderr, "usage: %s modelPath [-s W H] [-bs raysPerBatch] [-f frames] [-dev id] [-g gpus] [--budget samplesPerFrame] [--surface] [-w]\n", argv[0]); return 2; }
   }
   adn_host::Config config;
   if (!config.load(model)) { std::fprintf(stderr, "couldn't read export directory %s\n", model.c_str()); return 1; }
   std::printf("model %s: K = %d, adaptiveSamplingThreshold = %g\n", model.c_str(), config.numRaymarchSamples, config.adaptiveSamplingThreshold);
+  if (gpus > 1 && budget > 0) { std::fprintf(stderr, "--budget renders on one device (each row band would choose its own threshold)\n"); return 2; }
   if (gpus > 1) {
     // Row bands over `gpus` devices of this node + one NCCL gather per frame (include/adanerf_b200_multi.h); two frames
     // in flight, so the gather of a frame overlaps the next frame's sampling MLP.
@@ -85,6 +88,8 @@ int main(int argc, char** argv) {
   }
   adn_host::ImageGenerator gen;
   if (!gen.load(config, device)) { std::fprintf(stderr, "load failed: %s\n", gen.last_error()); return 1; }
+  if (budget > 0 && !gen.set_sample_budget(budget)) { std::fprintf(stderr, "sample budget: %s\n", gen.last_error()); return 1; }
+  std::vector<int32_t> ns(budget > 0 ? size_t(W) * H : 0);   // per-ray sample counts, for M under a budget
   adn_host::Camera cam;
   cam.width = W;
   cam.height = H;
@@ -97,9 +102,19 @@ int main(int argc, char** argv) {
     cam.pos[1] += 0.3f * config.scene.view_cell_size[1] * std::sin(t);
     cam.yaw = t;
     const auto t0 = std::chrono::steady_clock::now();
-    if (!gen.inference_host(cam, rgb.data(), batch, config.numRaymarchSamples)) { std::fprintf(stderr, "inference failed: %s\n", gen.last_error()); return 1; }
+    if (!gen.inference_host(cam, rgb.data(), batch, config.numRaymarchSamples, budget > 0 ? ns.data() : nullptr)) {
+      std::fprintf(stderr, "inference failed: %s\n", gen.last_error());
+      return 1;
+    }
     const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
     if (f >= 2) total_ms += ms;   // two warm-up frames (allocation)
+    if (budget > 0 && f >= 2) {
+      float thr = 0.f;
+      long long m = 0;
+      for (int32_t c : ns) m += c;
+      if (!gen.last_threshold(&thr)) { std::fprintf(stderr, "%s\n", gen.last_error()); return 1; }
+      std::printf("frame %d: threshold %.7g, %lld samples (budget %lld)\n", f - 2, double(thr), m, budget);
+    }
   }
   if (surface) {
     // The viewer's frame path: a cudaArray with surface load / store (what cudaGraphicsGLRegisterImage hands out,

@@ -4,6 +4,8 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 
+#include <algorithm>
+
 #include "mlp.cuh"
 #include "posenc.cuh"
 #include "ptx.cuh"
@@ -333,11 +335,11 @@ __device__ __forceinline__ void s2_lookback(long long* s_prefix, int tile, int t
 }
 
 __global__ void __launch_bounds__(kS2Threads)
-stage2_kernel(const float* __restrict__ raw0, long long n_rays, float thr, int K, const float* __restrict__ zlut,
-              int32_t* __restrict__ count, int32_t* __restrict__ offset, int32_t* __restrict__ cell_out,
-              int32_t* __restrict__ ray_out, float* __restrict__ z_out, float* __restrict__ zp_out,
-              long long* __restrict__ total, unsigned long long* __restrict__ tile_state, unsigned int* __restrict__ ticket,
-              int n_tiles, uint32_t epoch, uint32_t ticket_base) {
+stage2_kernel(const float* __restrict__ raw0, long long n_rays, float thr, const float* __restrict__ d_thr, int K,
+              const float* __restrict__ zlut, int32_t* __restrict__ count, int32_t* __restrict__ offset,
+              int32_t* __restrict__ cell_out, int32_t* __restrict__ ray_out, float* __restrict__ z_out,
+              float* __restrict__ zp_out, long long* __restrict__ total, unsigned long long* __restrict__ tile_state,
+              unsigned int* __restrict__ ticket, int n_tiles, uint32_t epoch, uint32_t ticket_base) {
   __shared__ uint32_t s_sel[kS2Rays][4];
   __shared__ int s_cnt[kS2Rays];
   __shared__ int s_off[kS2Rays];
@@ -345,6 +347,7 @@ stage2_kernel(const float* __restrict__ raw0, long long n_rays, float thr, int K
   __shared__ int s_tile;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (d_thr) thr = *d_thr;   // threshold chosen on the device (sample budget)
   if (threadIdx.x == 0) s_tile = int(atomicAdd(ticket, 1u) - ticket_base);
   __syncthreads();
   const int tile = s_tile;
@@ -432,12 +435,69 @@ constexpr int kS2tRowBytes = 528;
 constexpr int kS2tGmBytes = 0;    // group maxima live in registers
 constexpr size_t kS2tSmemBytes = size_t(kS2Rays) * (kS2tRowBytes + kS2tGmBytes) + 128 * sizeof(float);
 
+// Issues the copies of one tile's 64 rows into `rows` (stride kS2tRowBytes) and commits them; the caller waits
+// (cp.async.wait_group 0 + __syncwarp) before it reads its row.  Each warp fetches the 32 rows its own threads own: one
+// 512-byte row per cp.async instruction (16 B per lane, coalesced), nothing staged in registers, and only a __syncwarp
+// between the copies and their consumers.  (A bulk copy per thread serialises into a 32-iteration uniform-register
+// waterfall.)
+__device__ __forceinline__ void s2t_fetch_rows(const float* __restrict__ raw0, long long n_rays, long long ray0, uint8_t* rows,
+                                               int warp, int lane) {
+  const float* src = raw0 + (ray0 + warp * 32) * 128 + lane * 4;
+  const uint32_t dst = smem_u32(rows + (warp * 32) * kS2tRowBytes + lane * 16);
+  const long long left = n_rays - (ray0 + warp * 32);
+#pragma unroll 8
+  for (int i = 0; i < 32; ++i) {
+    if (i < left)
+      asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst + i * kS2tRowBytes), "l"(src + i * 128) : "memory");
+  }
+  asm volatile("cp.async.commit_group;" ::: "memory");
+}
+
+// The 16 group maxima (groups of 8 cells) of a staged row.
+__device__ __forceinline__ void s2t_group_maxima(const uint8_t* row, float (&g)[16]) {
+  const float4* row4 = reinterpret_cast<const float4*>(row);
+  auto max8 = [](const float4 a, const float4 b) {
+    return fmaxf(fmaxf(fmaxf(a.x, a.y), fmaxf(a.z, a.w)), fmaxf(fmaxf(b.x, b.y), fmaxf(b.z, b.w)));
+  };
+#pragma unroll
+  for (int q = 0; q < 16; ++q) g[q] = max8(row4[2 * q], row4[2 * q + 1]);
+}
+
+// One pop round: returns the row's largest remaining value (ties: lowest cell) and its cell, and removes it (-inf in the
+// row, refreshed group maximum).
+__device__ __forceinline__ float s2t_pop(uint8_t* row, float (&g)[16], int& cell) {
+  const float NEG = __int_as_float(0xff800000);
+  const float m = fmaxf(fmaxf(fmaxf(fmaxf(g[0], g[1]), fmaxf(g[2], g[3])), fmaxf(fmaxf(g[4], g[5]), fmaxf(g[6], g[7]))),
+                        fmaxf(fmaxf(fmaxf(g[8], g[9]), fmaxf(g[10], g[11])), fmaxf(fmaxf(g[12], g[13]), fmaxf(g[14], g[15]))));
+  int gi = 0;
+#pragma unroll
+  for (int i = 15; i >= 0; --i) gi = (g[i] == m) ? i : gi;   // first group holding the maximum
+  float* grp = reinterpret_cast<float*>(row) + 8 * gi;
+  const float4 a = reinterpret_cast<const float4*>(grp)[0], b = reinterpret_cast<const float4*>(grp)[1];
+  const float x[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+  bool found = false;
+  int idx = 0;
+  float nm = NEG;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const bool e = (x[i] == m) && !found;    // first cell of the group holding the maximum
+    found = found || e;
+    idx = e ? i : idx;
+    nm = fmaxf(nm, e ? NEG : x[i]);          // the group's maximum once that cell is gone
+  }
+  grp[idx] = NEG;
+#pragma unroll
+  for (int i = 0; i < 16; ++i) g[i] = (i == gi) ? nm : g[i];
+  cell = 8 * gi + idx;
+  return m;
+}
+
 template <int KMAX>
 __global__ void __launch_bounds__(kS2Rays)
-stage2_thread_kernel(const float* __restrict__ raw0, long long n_rays, float thr, int K, const float* __restrict__ zlut,
-                     int32_t* __restrict__ count, int32_t* __restrict__ offset, int32_t* __restrict__ cell_out,
-                     int32_t* __restrict__ ray_out, float* __restrict__ z_out, float* __restrict__ zp_out,
-                     long long* __restrict__ total, unsigned long long* __restrict__ tile_state,
+stage2_thread_kernel(const float* __restrict__ raw0, long long n_rays, float thr, const float* __restrict__ d_thr, int K,
+                     const float* __restrict__ zlut, int32_t* __restrict__ count, int32_t* __restrict__ offset,
+                     int32_t* __restrict__ cell_out, int32_t* __restrict__ ray_out, float* __restrict__ z_out,
+                     float* __restrict__ zp_out, long long* __restrict__ total, unsigned long long* __restrict__ tile_state,
                      unsigned int* __restrict__ ticket, int n_tiles, uint32_t epoch, uint32_t ticket_base) {
   extern __shared__ __align__(16) uint8_t s2t_smem[];
   uint8_t* rows = s2t_smem;
@@ -450,39 +510,21 @@ stage2_thread_kernel(const float* __restrict__ raw0, long long n_rays, float thr
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   if (tid == 0) s_tile = int(atomicAdd(ticket, 1u) - ticket_base);
+  if (d_thr) thr = *d_thr;   // threshold chosen on the device (sample budget)
   __syncthreads();
   const int tile = s_tile;
   const long long ray0 = (long long)tile * kS2Rays;
   const long long r = ray0 + tid;
   const bool valid = r < n_rays;
   uint8_t* row = rows + tid * kS2tRowBytes;
-  // each warp fetches the 32 rows its own threads own: one 512-byte row per cp.async instruction (16 B per lane,
-  // coalesced), nothing staged in registers, and only a __syncwarp between the copies and their consumers.
-  // (A bulk copy per thread serialises into a 32-iteration uniform-register waterfall.)
-  {
-    const float* src = raw0 + (ray0 + warp * 32) * 128 + lane * 4;
-    const uint32_t dst = smem_u32(rows + (warp * 32) * kS2tRowBytes + lane * 16);
-    const long long left = n_rays - (ray0 + warp * 32);
-#pragma unroll 8
-    for (int i = 0; i < 32; ++i) {
-      if (i < left)
-        asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst + i * kS2tRowBytes), "l"(src + i * 128) : "memory");
-    }
-    asm volatile("cp.async.commit_group;" ::: "memory");
-  }
+  s2t_fetch_rows(raw0, n_rays, ray0, rows, warp, lane);
   zl[tid] = zlut[tid];
   zl[tid + 64] = zlut[tid + 64];
   asm volatile("cp.async.wait_group 0;" ::: "memory");
   __syncwarp();
 
-  const float NEG = __int_as_float(0xff800000);
-  const float4* row4 = reinterpret_cast<const float4*>(row);
-  auto max8 = [](const float4 a, const float4 b) {
-    return fmaxf(fmaxf(fmaxf(a.x, a.y), fmaxf(a.z, a.w)), fmaxf(fmaxf(b.x, b.y), fmaxf(b.z, b.w)));
-  };
   float g[16];   // group maxima, registers
-#pragma unroll
-  for (int q = 0; q < 16; ++q) g[q] = max8(row4[2 * q], row4[2 * q + 1]);
+  s2t_group_maxima(row, g);
 
   uint32_t mk0 = 0, mk1 = 0, mk2 = 0, mk3 = 0;   // selection mask over the 128 cells
   float mv[KMAX];                                 // popped values, pick order
@@ -496,30 +538,10 @@ stage2_thread_kernel(const float* __restrict__ raw0, long long n_rays, float thr
     mv[j] = 0.0f;
     if (j >= K) break;                                        // warp uniform
     if (!__any_sync(0xffffffffu, active)) break;              // warp uniform
-    const float m = fmaxf(fmaxf(fmaxf(fmaxf(g[0], g[1]), fmaxf(g[2], g[3])), fmaxf(fmaxf(g[4], g[5]), fmaxf(g[6], g[7]))),
-                          fmaxf(fmaxf(fmaxf(g[8], g[9]), fmaxf(g[10], g[11])), fmaxf(fmaxf(g[12], g[13]), fmaxf(g[14], g[15]))));
-    int gi = 0;
-#pragma unroll
-    for (int i = 15; i >= 0; --i) gi = (g[i] == m) ? i : gi;   // first group holding the maximum
-    float* grp = reinterpret_cast<float*>(row) + 8 * gi;
-    const float4 a = reinterpret_cast<const float4*>(grp)[0], b = reinterpret_cast<const float4*>(grp)[1];
-    const float x[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-    bool found = false;
-    int idx = 0;
-    float nm = NEG;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const bool e = (x[i] == m) && !found;    // first cell of the group holding the maximum
-      found = found || e;
-      idx = e ? i : idx;
-      nm = fmaxf(nm, e ? NEG : x[i]);          // the group's maximum once that cell is gone
-    }
-    grp[idx] = NEG;
-#pragma unroll
-    for (int i = 0; i < 16; ++i) g[i] = (i == gi) ? nm : g[i];
+    int cell;
+    const float m = s2t_pop(row, g, cell);
     const bool sel = active && (j == 0 || m >= thr);
     active = sel;
-    const int cell = 8 * gi + idx;
     const uint32_t bit = sel ? (1u << (cell & 31)) : 0u;
     const int w = cell >> 5;
     mk0 |= (w == 0) ? bit : 0u;
@@ -582,7 +604,7 @@ size_t stage2_scratch_bytes(long long n_rays) {
 
 cudaError_t launch_stage2(const float* d_raw0, long long n_rays, float thr, int K, const float* d_zlut, int32_t* d_count,
                           int32_t* d_offset, int32_t* d_cell, int32_t* d_ray, float* d_z, float* d_zp, long long* d_total,
-                          void* d_scratch, Stage2Sync* sync, cudaStream_t s) {
+                          void* d_scratch, Stage2Sync* sync, cudaStream_t s, const float* d_thr) {
   if (n_rays <= 0) return cudaMemsetAsync(d_total, 0, sizeof(long long), s);
   const int n_tiles = int((n_rays + kS2Rays - 1) / kS2Rays);
   const size_t bytes = stage2_scratch_bytes(n_rays);
@@ -603,14 +625,256 @@ cudaError_t launch_stage2(const float* d_raw0, long long n_rays, float thr, int 
   // thread-per-ray kernel whenever its assumptions hold (K <= 16, 16-byte aligned rows for the cp.async fetch)
   const bool aligned = (reinterpret_cast<uintptr_t>(d_raw0) & 15u) == 0;
   if (K <= 8 && aligned)
-    stage2_thread_kernel<8><<<n_tiles, kS2Rays, kS2tSmemBytes, s>>>(d_raw0, n_rays, thr, K, d_zlut, d_count, d_offset, d_cell, d_ray,
-                                                                   d_z, d_zp, d_total, state, ticket, n_tiles, epoch, base);
+    stage2_thread_kernel<8><<<n_tiles, kS2Rays, kS2tSmemBytes, s>>>(d_raw0, n_rays, thr, d_thr, K, d_zlut, d_count, d_offset, d_cell,
+                                                                   d_ray, d_z, d_zp, d_total, state, ticket, n_tiles, epoch, base);
   else if (K <= 16 && aligned)
-    stage2_thread_kernel<16><<<n_tiles, kS2Rays, kS2tSmemBytes, s>>>(d_raw0, n_rays, thr, K, d_zlut, d_count, d_offset, d_cell, d_ray,
-                                                                    d_z, d_zp, d_total, state, ticket, n_tiles, epoch, base);
+    stage2_thread_kernel<16><<<n_tiles, kS2Rays, kS2tSmemBytes, s>>>(d_raw0, n_rays, thr, d_thr, K, d_zlut, d_count, d_offset, d_cell,
+                                                                    d_ray, d_z, d_zp, d_total, state, ticket, n_tiles, epoch, base);
   else
-    stage2_kernel<<<n_tiles, kS2Threads, 0, s>>>(d_raw0, n_rays, thr, K, d_zlut, d_count, d_offset, d_cell, d_ray, d_z, d_zp,
+    stage2_kernel<<<n_tiles, kS2Threads, 0, s>>>(d_raw0, n_rays, thr, d_thr, K, d_zlut, d_count, d_offset, d_cell, d_ray, d_z, d_zp,
                                                  d_total, state, ticket, n_tiles, epoch, base);
+  return cudaGetLastError();
+}
+
+// ------------------------------------------------------------------------------- sample budget
+// The smallest threshold t* >= thr_min whose sample count M(t*) is at most B = max_samples, with no host round trip.
+// For t > 0 stage 2 gives ray r  n_r(t) = clamp(#{cells >= t}, 1, K)  samples (src/nerf_raymarch_common.py:726-749), so
+//   M(t) = N + #{(r, j) : 2 <= j <= K, v_r^(j) >= t},   v_r^(j) = the j-th largest raw0 value of ray r (ties counted),
+// and with S = the multiset of those rank-2..K values that are >= thr_min and Q = B - N:
+//   |S| <= Q -> t* = thr_min,   else t* = nextafterf(s_(Q+1), +inf), s_(Q+1) = the (Q+1)-th largest element of S.
+// S is positive, so float order is uint32 bit order: S is written as keys (0 = no entry) and the (Q+1)-th largest key is
+// found by a radix select over bits [31:21], [20:10], [9:0]; the first histogram is folded into the extraction pass.
+// Histograms use integer atomics (order independent), so t* is deterministic.
+constexpr int kBudgetBins = 2048;
+struct BudgetState {
+  unsigned long long k;   // rank still sought inside the current prefix (1 = largest)
+  uint32_t prefix;        // key bits fixed so far
+  uint32_t done;          // 1: |S| <= Q, t* = thr_min
+};
+size_t budget_work_bytes() { return size_t(3 * kBudgetBins) * 4 + sizeof(BudgetState); }
+
+__device__ __forceinline__ void budget_flush_hist(const uint32_t* s_hist, uint32_t* __restrict__ hist) {
+  for (int b = threadIdx.x; b < kBudgetBins; b += blockDim.x)
+    if (s_hist[b]) atomicAdd(hist + b, s_hist[b]);
+}
+
+// K <= 16: thread per ray, the group-maximum pop rounds of stage2_thread_kernel; pops 1..K-1 that are >= thr_min are the
+// ray's keys.  Keys are staged in the dead row area and written out coalesced; CTAs loop over tiles so the histogram is
+// flushed once per CTA.
+__global__ void __launch_bounds__(kS2Rays)
+budget_keys_thread_kernel(const float* __restrict__ raw0, long long n_rays, float thr_min, int K, uint32_t* __restrict__ keys,
+                          uint32_t* __restrict__ hist) {
+  __shared__ __align__(16) uint8_t rows[kS2Rays * kS2tRowBytes];
+  __shared__ uint32_t s_hist[kBudgetBins];
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int KM1 = K - 1;
+  for (int b = tid; b < kBudgetBins; b += kS2Rays) s_hist[b] = 0;
+  const long long n_tiles = (n_rays + kS2Rays - 1) / kS2Rays;
+  for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    const long long ray0 = tile * kS2Rays;
+    __syncthreads();   // the previous tile's staged keys have been written out
+    s2t_fetch_rows(raw0, n_rays, ray0, rows, warp, lane);
+    asm volatile("cp.async.wait_group 0;" ::: "memory");
+    __syncwarp();
+    uint8_t* row = rows + tid * kS2tRowBytes;
+    float g[16];
+    s2t_group_maxima(row, g);
+    uint32_t key[15];
+    bool active = ray0 + tid < n_rays;
+    int cell;
+    s2t_pop(row, g, cell);   // rank 1: every ray keeps one sample whatever the threshold
+#pragma unroll
+    for (int j = 0; j < 15; ++j) {
+      key[j] = 0u;
+      if (j >= KM1) continue;                                   // uniform
+      if (!__any_sync(0xffffffffu, active)) continue;          // warp uniform
+      const float m = s2t_pop(row, g, cell);
+      active = active && m >= thr_min;
+      key[j] = active ? __float_as_uint(m) : 0u;
+    }
+    __syncthreads();   // every row is consumed: the row area becomes the staging area
+    uint32_t* st = reinterpret_cast<uint32_t*>(rows);
+#pragma unroll
+    for (int j = 0; j < 15; ++j) {
+      if (j < KM1) st[tid * KM1 + j] = key[j];
+      if (key[j]) atomicAdd(&s_hist[key[j] >> 21], 1u);
+    }
+    __syncthreads();
+    const long long n_out = min((long long)kS2Rays, n_rays - ray0) * KM1;
+    for (int i = tid; i < n_out; i += kS2Rays) keys[ray0 * KM1 + i] = st[i];
+  }
+  __syncthreads();
+  budget_flush_hist(s_hist, hist);
+}
+
+// 16 < K <= 128: warp per ray with stage 2's select_cells; the selected cells minus one instance of
+// the largest value are the ray's keys (none when no cell reaches thr_min).
+__global__ void __launch_bounds__(kS2Threads)
+budget_keys_warp_kernel(const float* __restrict__ raw0, long long n_rays, float thr_min, int K, uint32_t* __restrict__ keys,
+                        uint32_t* __restrict__ hist) {
+  __shared__ uint32_t s_hist[kBudgetBins];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int b = threadIdx.x; b < kBudgetBins; b += kS2Threads) s_hist[b] = 0;
+  __syncthreads();
+  const int KM1 = K - 1;
+  const long long step = (long long)gridDim.x * (kS2Threads / 32);
+  for (long long r = blockIdx.x * (long long)(kS2Threads / 32) + warp; r < n_rays; r += step) {
+    const float4 v4 = __ldg(reinterpret_cast<const float4*>(raw0 + r * 128) + lane);
+    const float v[4] = {v4.x, v4.y, v4.z, v4.w};
+    uint32_t sel[4];
+    const int cnt = select_cells(v4, thr_min, K, lane, sel);
+    int n_keys = 0;
+    if (__any_sync(0xffffffffu, v[0] >= thr_min || v[1] >= thr_min || v[2] >= thr_min || v[3] >= thr_min)) {
+      // drop one instance of the largest selected value (lowest lane, then lowest j)
+      uint32_t best = 0u;
+      int bj = 0;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const uint32_t k = ((sel[j] >> lane) & 1u) ? __float_as_uint(v[j]) : 0u;
+        bj = k > best ? j : bj;
+        best = k > best ? k : best;
+      }
+      const uint32_t m = __reduce_max_sync(0xffffffffu, best);
+      const int who = __ffs(__ballot_sync(0xffffffffu, best == m)) - 1;
+      if (lane == who) sel[bj] &= ~(1u << lane);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) sel[j] = __shfl_sync(0xffffffffu, sel[j], who);
+      const uint32_t below = (1u << lane) - 1u;
+      int base = 0;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        if ((sel[j] >> lane) & 1u) {
+          const uint32_t k = __float_as_uint(v[j]);
+          keys[r * KM1 + base + __popc(sel[j] & below)] = k;
+          atomicAdd(&s_hist[k >> 21], 1u);
+        }
+        base += __popc(sel[j]);
+      }
+      n_keys = cnt - 1;
+    }
+    for (int p = n_keys + lane; p < KM1; p += 32) keys[r * KM1 + p] = 0u;
+  }
+  __syncthreads();
+  budget_flush_hist(s_hist, hist);
+}
+
+// Rounds 1 and 2 of the select: histogram of the next key bits over the keys that carry the current prefix.
+__global__ void __launch_bounds__(256)
+budget_hist_kernel(const uint32_t* __restrict__ keys, long long n_keys, const BudgetState* __restrict__ st, int round,
+                   uint32_t* __restrict__ hist) {
+  __shared__ uint32_t s_hist[kBudgetBins];
+  if (st->done) return;   // uniform
+  const uint32_t prefix = st->prefix;
+  const int match_shift = round == 1 ? 21 : 10, bin_shift = round == 1 ? 10 : 0;
+  const uint32_t mask = round == 1 ? 2047u : 1023u;
+  for (int b = threadIdx.x; b < kBudgetBins; b += 256) s_hist[b] = 0;
+  __syncthreads();
+  auto add = [&](uint32_t k) {
+    if (k && (k >> match_shift) == prefix) atomicAdd(&s_hist[(k >> bin_shift) & mask], 1u);
+  };
+  const long long n4 = n_keys >> 2;
+  const uint4* k4 = reinterpret_cast<const uint4*>(keys);
+  for (long long i = blockIdx.x * 256ll + threadIdx.x; i < n4; i += 256ll * gridDim.x) {
+    const uint4 v = __ldg(k4 + i);
+    add(v.x);
+    add(v.y);
+    add(v.z);
+    add(v.w);
+  }
+  if (blockIdx.x == 0 && threadIdx.x < (n_keys & 3)) add(keys[4 * n4 + threadIdx.x]);
+  __syncthreads();
+  budget_flush_hist(s_hist, hist);
+}
+
+// One CTA: finds the bin of the k-th largest key (descending scan over the bins) and narrows the prefix.  Round 0 also
+// decides |S| <= Q; round 2 fixes the last bits and writes t*.
+__global__ void __launch_bounds__(1024)
+budget_select_kernel(const uint32_t* __restrict__ hist_all, BudgetState* __restrict__ st, int round, unsigned long long q,
+                     float thr_min, float* __restrict__ d_thr) {
+  __shared__ unsigned long long s_warp[32];
+  if (round > 0 && st->done) return;   // uniform
+  const uint32_t* hist = hist_all + round * kBudgetBins;
+  const int nb = round == 2 ? 1024 : 2048, per = nb / 1024;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const unsigned long long k = round == 0 ? q + 1 : st->k;
+  unsigned long long s = 0;
+  for (int u = 0; u < per; ++u) s += hist[nb - 1 - (tid * per + u)];   // thread 0 owns the highest bins
+  unsigned long long x = s;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o);
+    if (lane >= o) x += y;
+  }
+  if (lane == 31) s_warp[warp] = x;
+  __syncthreads();
+  if (warp == 0) {
+    unsigned long long w = s_warp[lane];
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const unsigned long long y = __shfl_up_sync(0xffffffffu, w, o);
+      if (lane >= o) w += y;
+    }
+    s_warp[lane] = w;   // inclusive over warps
+  }
+  __syncthreads();
+  const unsigned long long incl = x + (warp > 0 ? s_warp[warp - 1] : 0ull), total = s_warp[31];
+  if (round == 0 && total < k) {   // every candidate fits: the floor threshold itself
+    if (tid == 0) {
+      st->done = 1u;
+      *d_thr = thr_min;
+    }
+    return;
+  }
+  unsigned long long excl = incl - s;
+  if (excl < k && k <= incl) {     // exactly one thread
+    for (int u = 0; u < per; ++u) {
+      const uint32_t b = uint32_t(nb - 1 - (tid * per + u));
+      const unsigned long long c = hist[b];
+      if (k <= excl + c) {
+        const uint32_t prefix = (st->prefix << (round == 2 ? 10 : 11)) | b;
+        st->prefix = prefix;
+        st->k = k - excl;
+        // nextafterf(s_(Q+1), +inf) of a positive float (+inf stays +inf)
+        if (round == 2) *d_thr = __uint_as_float(prefix >= 0x7f800000u ? 0x7f800000u : prefix + 1u);
+        break;
+      }
+      excl += c;
+    }
+  }
+}
+
+cudaError_t launch_budget_threshold(const float* d_raw0, long long n_rays, float thr_min, int K, long long max_samples,
+                                    uint32_t* d_keys, void* d_work, float* d_thr, int num_sms, cudaStream_t s, int* launches) {
+  uint32_t* hist = static_cast<uint32_t*>(d_work);
+  BudgetState* st = reinterpret_cast<BudgetState*>(hist + 3 * kBudgetBins);
+  cudaError_t e = cudaMemsetAsync(d_work, 0, budget_work_bytes(), s);
+  if (e != cudaSuccess) return e;
+  const unsigned long long q = (unsigned long long)(max_samples - n_rays);
+  const long long n_keys = n_rays * (K - 1);
+  int n = 0;
+  if (n_keys > 0) {
+    if (K <= 16) {
+      const long long n_tiles = (n_rays + kS2Rays - 1) / kS2Rays;
+      budget_keys_thread_kernel<<<unsigned(std::min<long long>(n_tiles, 5ll * num_sms)), kS2Rays, 0, s>>>(d_raw0, n_rays, thr_min, K,
+                                                                                                         d_keys, hist);
+    } else {
+      const long long blocks = (n_rays + kS2Threads / 32 - 1) / (kS2Threads / 32);
+      budget_keys_warp_kernel<<<unsigned(std::min<long long>(blocks, 8ll * num_sms)), kS2Threads, 0, s>>>(d_raw0, n_rays, thr_min, K,
+                                                                                                         d_keys, hist);
+    }
+    ++n;
+  }
+  budget_select_kernel<<<1, 1024, 0, s>>>(hist, st, 0, q, thr_min, d_thr);
+  ++n;
+  if (n_keys > 0) {
+    const unsigned grid = unsigned(std::max<long long>(1, std::min<long long>((n_keys / 4 + 255) / 256, 4ll * num_sms)));
+    for (int round = 1; round <= 2; ++round) {
+      budget_hist_kernel<<<grid, 256, 0, s>>>(d_keys, n_keys, st, round, hist + round * kBudgetBins);
+      budget_select_kernel<<<1, 1024, 0, s>>>(hist, st, round, q, thr_min, d_thr);
+      n += 2;
+    }
+  }
+  if (launches) *launches += n;
   return cudaGetLastError();
 }
 

@@ -42,9 +42,17 @@ struct Stage2Sync {
   size_t cleared_bytes = 0;
   uint32_t epoch = 0, ticket_base = 0;
 };
+// d_thr: when non-null the kernel reads the threshold from this device float (a sample-budget threshold) instead of `thr`.
 cudaError_t launch_stage2(const float* d_raw0, long long n_rays, float thr, int K, const float* d_zlut, int32_t* d_count,
                           int32_t* d_offset, int32_t* d_cell, int32_t* d_ray, float* d_z, float* d_zp, long long* d_total,
-                          void* d_scratch, Stage2Sync* sync, cudaStream_t s);
+                          void* d_scratch, Stage2Sync* sync, cudaStream_t s, const float* d_thr = nullptr);
+
+// Sample budget: writes to *d_thr the smallest threshold t >= thr_min (> 0) at which stage 2 over raw0 [n_rays, 128] with K
+// samples per ray yields at most max_samples (>= n_rays) samples in all.  d_raw0 must be 16-byte aligned.
+// d_keys: [n_rays * (K - 1)] uint32 scratch; d_work: budget_work_bytes() of scratch.  Stream ordered, no host synchronisation; adds its kernel count to *launches.
+size_t budget_work_bytes();
+cudaError_t launch_budget_threshold(const float* d_raw0, long long n_rays, float thr_min, int K, long long max_samples,
+                                    uint32_t* d_keys, void* d_work, float* d_thr, int num_sms, cudaStream_t s, int* launches);
 // Dense (thr == 0): count = K, offset = ray*K, total = N*K; no index arrays are materialised.
 cudaError_t launch_stage2_dense(long long n_rays, int K, int32_t* d_count, int32_t* d_offset, long long* d_total,
                                 cudaStream_t s);

@@ -129,6 +129,13 @@ class Renderer:
         self._check(self.lib.adn_get_stats(self.handle, C.byref(s)))
         return dict(n_rays=s.n_rays, n_samples=s.n_samples, ms_stage=list(s.ms_stage), kernel_launches=s.kernel_launches)
 
+    def last_threshold(self):
+        """The threshold the last render used: the one chosen under set_option("sample_budget", B), else the `thr` it was
+        given.  Synchronises."""
+        t = C.c_float()
+        self._check(self.lib.adn_last_threshold(self.handle, C.byref(t)))
+        return t.value
+
     # ---- helpers -------------------------------------------------------------------------
     def _dev(self):
         return torch.device("cuda", self.device)
@@ -282,6 +289,15 @@ class Renderer:
                                                self._stream()))
         m = int(total.item())
         return dict(count=count, offset=offset, cell=cell[:m], ray=ray[:m], z=z[:m], zp=zp[:m], total=m)
+
+    def budget_threshold(self, raw0, thr_min, K, max_samples, out=None):
+        """raw0 [N,128] -> [1] float32 device tensor: the smallest threshold >= thr_min at which stage 2 with K samples per
+        ray yields at most max_samples samples (the selection a "sample_budget" render makes).  Stream ordered, no sync."""
+        x = self._f32(raw0)
+        t = out if out is not None else torch.empty((1,), dtype=torch.float32, device=self._dev())
+        self._check(self.lib.adn_budget_threshold(self.handle, x.data_ptr(), x.shape[0], float(thr_min), int(K), int(max_samples),
+                                                  t.data_ptr(), self._stream()))
+        return t
 
     def stage3(self, ray_o, ray_d, ray_idx, z):
         ro, rd, zz = self._f32(ray_o), self._f32(ray_d), self._f32(z)

@@ -107,9 +107,19 @@ adn_status adn_probe_export_dir(const char* dir, adn_scene* scene_out, float* th
 /* name: "chunk_rays" (rays per internal batch, 0 = auto), "profile" (0/1 per-stage event timing),
  * "mlp0_terms" (3 = bf16x3 split precision [default], 1 = plain bf16; parity experiments only),
  * "fuse_encoder" (1 = positional encoding of the samples inside the shading kernel: no [M,90]-sized tile buffer;
- *   0 = separate kernel [default]). */
+ *   0 = separate kernel [default]),
+ * "sample_budget" (B > 0 = every adaptive render -- rays, aux, camera, rgba8, surface, *_host -- takes its `thr` as a floor
+ *   and renders with the smallest threshold t* >= thr whose total sample count M over the whole call is <= B, chosen on
+ *   the device with no host synchronisation; the picture is exactly that of a fixed-threshold call at t*.  Fails with
+ *   ADN_ERR_INVALID in dense mode (thr == 0) and when B < n_rays.  The stage-2 slot of ms_stage includes the selection.
+ *   Calls of more than one chunk keep raw0 and the ray origins / directions of the whole call (536 B per ray: the caller's
+ *   d_oracle_weights when given, else context scratch).  0 = off [default]).
+ *   The frame cost follows M, so B is a frame-time knob; row bands (multi-GPU) each choose their own t*. */
 adn_status adn_set_option(adn_ctx* ctx, const char* name, int64_t value);
 adn_status adn_get_stats(adn_ctx* ctx, adn_stats* out);   /* synchronises the context's stream */
+/* The threshold the last render call used: t* under "sample_budget", else its `thr` argument.  Synchronises like
+ * adn_get_stats. */
+adn_status adn_last_threshold(adn_ctx* ctx, float* thr_out);
 
 /* ---- the hot path ----------------------------------------------------------------------- */
 /* render(rays, sampling_net, shading_net, adaptiveSamplingThreshold): one call = what
@@ -194,6 +204,12 @@ adn_status adn_mlp0_forward(adn_ctx* ctx, const float* d_x0, int64_t n_rays, flo
 adn_status adn_stage2_sample(adn_ctx* ctx, const float* d_raw0, int64_t n_rays, float thr, int K,
                              int32_t* d_count, int32_t* d_offset, int32_t* d_cell, int32_t* d_ray,
                              float* d_z, float* d_zp, int64_t* d_total, void* stream);
+/* stage 2 threshold under a sample budget: *d_thr (device float) = the smallest t >= thr_min (> 0) with
+ * sum_r clamp(#{cells of ray r >= t}, 1, K) <= max_samples (>= n_rays) -- the sample count stage 2 gives at t
+ * (src/nerf_raymarch_common.py:726-749) -- from d_raw0 [N,128] (16-byte aligned).  Exact: a radix select over the rays'
+ * rank-2..K values. */
+adn_status adn_budget_threshold(adn_ctx* ctx, const float* d_raw0, int64_t n_rays, float thr_min, int K, int64_t max_samples,
+                                float* d_thr, void* stream);
 /* stage 3: RayMarchFromPoses.batch encode (src/features.py:458-479). d_x1 [M,90] fp32 (pos block first). */
 adn_status adn_stage3_encode(adn_ctx* ctx, const float* d_ray_o, const float* d_ray_d, const int32_t* d_ray,
                              const float* d_z, int64_t n_samples, float* d_x1, void* stream);
