@@ -55,7 +55,6 @@ struct adn_ctx {
   bool fuse_encoder = false;      // stage 3 inside the shading kernel: saves the [M, 90]-sized tile buffer
   int64_t chunk_rays = 0;
   bool profile = false;
-  int weight_copies = 1;   // replicas of each packed weight blob (MlpProgram::w_copies)
   int64_t sample_budget = 0;      // B of adn_set_option "sample_budget" (0 = off)
   bool last_budget = false;       // the last render chose its threshold on the device (in budget_thr)
   float last_thr = 0.0f;          // the last render's threshold argument
@@ -196,15 +195,8 @@ adn_status upload(adn_ctx* ctx, Net& net, const std::vector<uint8_t>& wblob, con
   std::memcpy(net.prog.side, fblob.data(), fblob.size() * 4);
   if (net.d_wblob) cudaFree(net.d_wblob);
   net.d_wblob = nullptr;
-  // replicas of the blob (see MlpProgram::w_copies): stride = size rounded up to 4 KB plus an odd number of 256-byte units,
-  // so that the same offset of different copies lands in different L2 slices
-  const uint32_t copies = uint32_t(std::max(1, ctx->weight_copies));
-  const size_t stride = ((wblob.size() + 4095) / 4096) * 4096 + 256 * 37;
-  net.prog.w_copies = copies;
-  net.prog.w_stride = uint32_t(stride);
-  ADN_CUDA(ctx, cudaMalloc(&net.d_wblob, stride * copies));
-  for (uint32_t c = 0; c < copies; ++c)
-    ADN_CUDA(ctx, cudaMemcpy(net.d_wblob + stride * c, wblob.data(), wblob.size(), cudaMemcpyHostToDevice));
+  ADN_CUDA(ctx, cudaMalloc(&net.d_wblob, wblob.size()));
+  ADN_CUDA(ctx, cudaMemcpy(net.d_wblob, wblob.data(), wblob.size(), cudaMemcpyHostToDevice));
   return ADN_OK;
 }
 
@@ -692,7 +684,6 @@ adn_status adn_create(adn_ctx** out, const adn_scene* scene, int device) {
   adn_ctx* ctx = new adn_ctx();
   ctx->device = device;
   ctx->num_sms = prop.multiProcessorCount;
-  if (const char* wc = std::getenv("ADN_WEIGHT_COPIES")) ctx->weight_copies = std::max(1, std::min(64, std::atoi(wc)));
   ctx->scene = *scene;
   if (cudaSetDevice(device) != cudaSuccess) {
     delete ctx;

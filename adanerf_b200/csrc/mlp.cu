@@ -13,6 +13,12 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
   return *reinterpret_cast<uint32_t*>(&h);
 }
 
+// A set of layer flags known at compile time: the epilogue's tests of it fold away.
+template <uint8_t V>
+struct ConstFlags {
+  __device__ constexpr operator uint8_t() const { return V; }
+};
+
 template <int NSPLIT>
 struct MlpCfg {
   static constexpr int kNB = (NSPLIT == 2) ? 4 : 5;                  // activation blocks per term
@@ -93,7 +99,9 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
   constexpr int kConsumerWarps = 8, kProducerWarp = 8;
 
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  // 1024-byte aligned.  Offsetting smem_raw (rather than rounding an integer address) keeps every pointer below in the
+  // shared state space, so the epilogue's reads of `side` and writes of `act` compile to LDS / STS, not generic accesses.
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* act = smem;                                                   // [NSPLIT][NB] blocks
   uint8_t* ring = act + Cfg::kActBytes;                                  // [STAGES] stages
   float* side = reinterpret_cast<float*>(ring + size_t(STAGES) * STAGE_BYTES);
@@ -122,7 +130,6 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
     // Stage i of a layer is [128 N rows x 64 K] (hi, then lo when NSPLIT == 2), N half outermost: the order the
     // consumers walk them in.
     if (warp == kProducerWarp && lane == 0) {
-      const uint8_t* blob = wblob + size_t(blockIdx.x % prog.w_copies) * prog.w_stride;
       int stage = 0;
       uint32_t phase = 0;
       for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) {
@@ -132,7 +139,7 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
           for (int i = 0; i < n_st; ++i) {
             mbar_wait(&w_empty[stage], phase ^ 1, err_flag, 1);
             mbar_arrive_expect_tx(&w_full[stage], STAGE_BYTES);
-            bulk_g2s(ring + size_t(stage) * STAGE_BYTES, blob + L.w_off + size_t(i) * STAGE_BYTES, STAGE_BYTES, &w_full[stage]);
+            bulk_g2s(ring + size_t(stage) * STAGE_BYTES, wblob + L.w_off + size_t(i) * STAGE_BYTES, STAGE_BYTES, &w_full[stage]);
             if (++stage == STAGES) {
               stage = 0;
               phase ^= 1;
@@ -212,71 +219,84 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
       named_bar_sync(bar_id, 128);   // all of the warpgroup's MMAs retired: the A blocks may be overwritten in place
 
       // ------------------------------------------------------------------ epilogue
-      const uint8_t flags = L.flags;
-      float rgb[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+      // Instantiated per set of layer flags (a compile-time constant for the sets the networks use): with no branches in
+      // the unrolled column loop the compiler batches the bias / head loads ahead of the dependent adds and stores.
+      auto epilogue = [&](auto flags) {
+        float rgb[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
 #pragma unroll
-      for (int nh = 0; nh < 2; ++nh) {
-        if (nh >= L.n_half) break;
+        for (int nh = 0; nh < 2; ++nh) {
+          if (nh >= L.n_half) break;
 #pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const int col = nh * 128 + 8 * i + cq;
-          const float2 b = *reinterpret_cast<const float2*>(side + L.bias_off + col);
+          for (int i = 0; i < 16; ++i) {
+            const int col = nh * 128 + 8 * i + cq;
+            const float2 b = *reinterpret_cast<const float2*>(side + L.bias_off + col);
+#pragma unroll
+            for (int rr = 0; rr < 2; ++rr) {
+              const int row = r0 + 8 * rr;
+              float v0 = acc[nh][4 * i + 2 * rr] + b.x;
+              float v1 = acc[nh][4 * i + 2 * rr + 1] + b.y;
+              if (flags & LF_FINAL_RAW) {
+                const long long grow = t * kTileM + row;
+                if (grow < rows) *reinterpret_cast<float2*>(out + grow * prog.out_cols + col) = make_float2(v0, v1);
+                continue;
+              }
+              if (flags & LF_RELU) {
+                v0 = fmaxf(v0, 0.0f);
+                v1 = fmaxf(v1, 0.0f);
+              }
+              if (flags & LF_ALPHA_DOT) {
+                const float2 w = *reinterpret_cast<const float2*>(side + prog.alpha_w_off + col);
+                alpha[rr] = fmaf(v1, w.y, fmaf(v0, w.x, alpha[rr]));
+              }
+              if (flags & LF_OUT_ACT) {
+                const uint32_t off = uint32_t(L.out_blk0 + (col >> 6)) * kBlkBytes + sw128_offset(uint32_t(row), uint32_t(col & 63));
+                const uint32_t hi = pack_bf16x2(v0, v1);
+                *reinterpret_cast<uint32_t*>(act + off) = hi;
+                if (NSPLIT == 2) {
+                  const uint32_t lo = pack_bf16x2(v0 - __uint_as_float(hi << 16), v1 - __uint_as_float(hi & 0xFFFF0000u));
+                  *reinterpret_cast<uint32_t*>(act + NB * kBlkBytes + off) = lo;
+                }
+              }
+              if (flags & LF_FINAL_RGB) {
+#pragma unroll
+                for (int k = 0; k < 3; ++k) {
+                  const float2 w = *reinterpret_cast<const float2*>(side + prog.rgb_w_off + k * 128 + col);
+                  rgb[rr][k] = fmaf(v1, w.y, fmaf(v0, w.x, rgb[rr][k]));
+                }
+              }
+            }
+          }
+        }
+        if (flags & LF_FINAL_RGB) {
+          // the four lanes of a row hold partial dot products over interleaved column pairs
 #pragma unroll
           for (int rr = 0; rr < 2; ++rr) {
-            const int row = r0 + 8 * rr;
-            float v0 = acc[nh][4 * i + 2 * rr] + b.x;
-            float v1 = acc[nh][4 * i + 2 * rr + 1] + b.y;
-            if (flags & LF_FINAL_RAW) {
-              const long long grow = t * kTileM + row;
-              if (grow < rows) *reinterpret_cast<float2*>(out + grow * prog.out_cols + col) = make_float2(v0, v1);
-              continue;
-            }
-            if (flags & LF_RELU) {
-              v0 = fmaxf(v0, 0.0f);
-              v1 = fmaxf(v1, 0.0f);
-            }
-            if (flags & LF_ALPHA_DOT) {
-              const float2 w = *reinterpret_cast<const float2*>(side + prog.alpha_w_off + col);
-              alpha[rr] = fmaf(v1, w.y, fmaf(v0, w.x, alpha[rr]));
-            }
-            if (flags & LF_OUT_ACT) {
-              const uint32_t off = uint32_t(L.out_blk0 + (col >> 6)) * kBlkBytes + sw128_offset(uint32_t(row), uint32_t(col & 63));
-              const uint32_t hi = pack_bf16x2(v0, v1);
-              asm volatile("st.shared.b32 [%0], %1;" ::"r"(act_s + off), "r"(hi) : "memory");
-              if (NSPLIT == 2) {
-                const uint32_t lo = pack_bf16x2(v0 - __uint_as_float(hi << 16), v1 - __uint_as_float(hi & 0xFFFF0000u));
-                asm volatile("st.shared.b32 [%0], %1;" ::"r"(act_s + uint32_t(NB * kBlkBytes) + off), "r"(lo) : "memory");
-              }
-            }
-            if (flags & LF_FINAL_RGB) {
+            float a = alpha[rr], c0 = rgb[rr][0], c1 = rgb[rr][1], c2 = rgb[rr][2];
 #pragma unroll
-              for (int k = 0; k < 3; ++k) {
-                const float2 w = *reinterpret_cast<const float2*>(side + prog.rgb_w_off + k * 128 + col);
-                rgb[rr][k] = fmaf(v1, w.y, fmaf(v0, w.x, rgb[rr][k]));
-              }
+            for (int m = 1; m <= 2; m <<= 1) {
+              a += __shfl_xor_sync(0xffffffffu, a, m);
+              c0 += __shfl_xor_sync(0xffffffffu, c0, m);
+              c1 += __shfl_xor_sync(0xffffffffu, c1, m);
+              c2 += __shfl_xor_sync(0xffffffffu, c2, m);
             }
+            const long long grow = t * kTileM + r0 + 8 * rr;
+            if ((lane & 3) == 0 && grow < rows)
+              reinterpret_cast<float4*>(out)[grow] = make_float4(c0 + side[prog.rgb_b_off], c1 + side[prog.rgb_b_off + 1],
+                                                                 c2 + side[prog.rgb_b_off + 2], a + side[prog.alpha_b_off]);
           }
         }
+      };
+      using F = uint8_t;
+      constexpr F kEpiFlags = LF_RELU | LF_ALPHA_DOT | LF_OUT_ACT | LF_FINAL_RAW | LF_FINAL_RGB;
+      switch (L.flags & kEpiFlags) {
+        case LF_RELU | LF_OUT_ACT: epilogue(ConstFlags<LF_RELU | LF_OUT_ACT>{}); break;
+        case LF_RELU | LF_OUT_ACT | LF_ALPHA_DOT: epilogue(ConstFlags<LF_RELU | LF_OUT_ACT | LF_ALPHA_DOT>{}); break;
+        case LF_OUT_ACT: epilogue(ConstFlags<LF_OUT_ACT>{}); break;
+        case LF_RELU | LF_FINAL_RGB: epilogue(ConstFlags<LF_RELU | LF_FINAL_RGB>{}); break;
+        case LF_FINAL_RAW: epilogue(ConstFlags<LF_FINAL_RAW>{}); break;
+        default: epilogue(F(L.flags)); break;   // any other combination: the same code with run-time tests
       }
-      if (flags & LF_FINAL_RGB) {
-        // the four lanes of a row hold partial dot products over interleaved column pairs
-#pragma unroll
-        for (int rr = 0; rr < 2; ++rr) {
-          float a = alpha[rr], c0 = rgb[rr][0], c1 = rgb[rr][1], c2 = rgb[rr][2];
-#pragma unroll
-          for (int m = 1; m <= 2; m <<= 1) {
-            a += __shfl_xor_sync(0xffffffffu, a, m);
-            c0 += __shfl_xor_sync(0xffffffffu, c0, m);
-            c1 += __shfl_xor_sync(0xffffffffu, c1, m);
-            c2 += __shfl_xor_sync(0xffffffffu, c2, m);
-          }
-          const long long grow = t * kTileM + r0 + 8 * rr;
-          if ((lane & 3) == 0 && grow < rows)
-            reinterpret_cast<float4*>(out)[grow] = make_float4(c0 + side[prog.rgb_b_off], c1 + side[prog.rgb_b_off + 1],
-                                                               c2 + side[prog.rgb_b_off + 2], a + side[prog.alpha_b_off]);
-        }
-      }
-      if (flags & LF_LOAD_IN1_AFTER) {   // the 2nd input block (view directions) replaces the tile-start block
+      if (L.flags & LF_LOAD_IN1_AFTER) {   // the 2nd input block (view directions) replaces the tile-start block
         if (ENC) {
           if (tw < 64) encode_row<true>(enc, t * kTileM + 64 * wg + tw, rows, blk_addr(0, prog.in1_blk), 64 * wg + tw);
         } else {

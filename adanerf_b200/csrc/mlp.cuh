@@ -57,9 +57,6 @@ struct MlpProgram {
   uint32_t in0_off, in0_lo_off, in1_off;
   uint32_t alpha_w_off, alpha_b_off, rgb_w_off, rgb_b_off;  // float offsets in `side`
   int32_t out_cols;           // row stride of the FINAL_RAW output
-  // The packed weight blob is replicated w_copies times in global memory, w_stride bytes apart; CTA c streams copy
-  // c % w_copies (spreads the grid's nearly lock-step re-reads of the same lines over more L2 slices).
-  uint32_t w_copies, w_stride;
   MlpLayer layers[kMaxLayers];
   float side[kSideFloats];
 };
