@@ -8,6 +8,7 @@ import torch
 
 from conftest import case_weights, load_golden
 from oracle import adanerf_oracle as orc
+from oracle import mlp_emulation as me
 
 pytestmark = pytest.mark.gpu
 
@@ -35,22 +36,33 @@ def _packed_from_golden(g, K):
 
 
 # ------------------------------------------------------------------------------- wgmma bring-up
+# Kernel vs the bf16-faithful emulation (the fp32 accumulation order is all that differs): 2x the values measured on an
+# H100 80GB HBM3 -- single layer, max abs err by terms: 7.63e-6 (3), 2.86e-6 (1); multi-layer, max err / output scale by
+# depth: 2.7e-6 (2), 6.7e-6 (3), 1.23e-5 (8).  The deeper split nets carry about what fp32 accumulation costs per layer,
+# so against fp64 they measure nearly the same.
+UMMA_SINGLE_BOUND = {3: 1.6e-5, 1: 6e-6}
+UMMA_MULTI_BOUND = {2: 6e-6, 3: 1.4e-5, 8: 2.5e-5}
 @pytest.mark.parametrize("n_out", [128, 256])
 @pytest.mark.parametrize("terms", [3, 1])
 def test_umma_single_layer(bare, n_out, terms):
-    """One Linear layer through the wgmma path == validates descriptors, swizzle, accumulator fragment layout."""
+    """One Linear layer through the wgmma path == validates descriptors, swizzle, accumulator fragment layout.  Compared
+    with the bf16-faithful emulation (same operands, float64 sums), so only the fp32 accumulation order differs."""
     g = torch.Generator().manual_seed(5)
     W = torch.randn(n_out, 90, generator=g) * 0.3
     b = torch.randn(n_out, generator=g) * 0.1
     x = torch.randn(300, 90, generator=g)
+    sd = {"layers.0.weight": W, "layers.0.bias": b}
     bare.set_option("mlp0_terms", terms)
-    bare.set_weights(0, {"layers.0.weight": W, "layers.0.bias": b})
-    out = bare.mlp0(x.cuda(), n_out=n_out).cpu()
-    ref = (x.double() @ W.double().T + b.double()).float()
-    err = (out - ref).abs().max().item()
-    print(f"single layer n_out={n_out} terms={terms}: max abs err {err:.3e}")
+    bare.set_weights(0, sd)
+    out = bare.mlp0(x.cuda(), n_out=n_out)
+    emu = me.mlp0_emulate(x.cuda(), sd, terms=terms)
+    ref64 = x.double() @ W.double().T + b.double()
+    err = (out - emu).abs().max().item()
+    err64 = (out.cpu().double() - ref64).abs().max().item()
+    print(f"single layer n_out={n_out} terms={terms}: max abs err {err:.3e} vs emulation, {err64:.3e} vs fp64")
+    assert err < UMMA_SINGLE_BOUND[terms]
     # bf16x3 keeps ~16 mantissa bits per operand: |err| ~ 2^-16 * |x||w| * sqrt(K)
-    assert err < (2e-4 if terms == 3 else 6e-2)
+    assert err64 < (2e-4 if terms == 3 else 6e-2)
     bare.set_option("mlp0_terms", 3)
 
 
@@ -64,11 +76,15 @@ def test_umma_multi_layer(bare, depth):
         sd[f"layers.{i}.bias"] = torch.randn(dims[i + 1], generator=g) * 0.1
     x = torch.randn(1000, 90, generator=g)
     bare.set_weights(0, sd)
-    out = bare.mlp0(x.cuda()).cpu()
+    out = bare.mlp0(x.cuda())
+    emu = me.mlp0_emulate(x.cuda(), sd, terms=3)
     ref = orc.mlp0_forward(x.double(), orc.to_dtype(sd, torch.float64)).float()
-    err = (out - ref).abs().max().item()
-    print(f"depth {depth}: max abs err {err:.3e} (ref scale {ref.abs().max():.2f})")
-    assert err < 1e-4 * max(1.0, ref.abs().max().item())
+    scale = max(1.0, ref.abs().max().item())
+    err = (out - emu).abs().max().item()
+    err64 = (out.cpu() - ref).abs().max().item()
+    print(f"depth {depth}: max abs err {err:.3e} vs emulation, {err64:.3e} vs fp64 (ref scale {scale:.2f})")
+    assert err < UMMA_MULTI_BOUND[depth] * scale
+    assert err64 < 1e-4 * scale
 
 
 # ------------------------------------------------------------------------------------ stage 0
