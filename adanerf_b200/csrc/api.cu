@@ -26,10 +26,8 @@ struct HostTensor {
 
 struct Net {
   bool ready = false;
-  int nsplit = 1;
   int n_in = 0, n_out = 0;
   MlpProgram prog{};
-  InputLayout lay{};
   uint8_t* d_wblob = nullptr;
   std::map<std::string, HostTensor> tensors;  // kept so "mlp0_terms" can re-pack
 };
@@ -60,7 +58,7 @@ struct adn_ctx {
   float last_thr = 0.0f;          // the last render's threshold argument
   bool prof_budget = false;       // the profiled render timed the selection with stage 2 (ev[7] -> ev[3])
   // scratch
-  Buf tiles0, raw0, x0, ray_o, ray_d, dirs, count, offset, rayidx, zbuf, zpbuf, tiles1, raw1, s2scratch, rgb, rgba, x1, metric;
+  Buf tiles0, raw0, ray_o, ray_d, dirs, count, offset, rayidx, zbuf, zpbuf, tiles1, raw1, s2scratch, rgb, rgba, metric;
   Buf budget_keys, budget_work, budget_thr;   // sample budget: candidate keys, histograms + select state, t*
   long long* d_total = nullptr;
   int* d_err = nullptr;           // device view of h_err
@@ -207,7 +205,6 @@ adn_status build_net0(adn_ctx* ctx) {
   while (find(net, "layers." + std::to_string(D) + ".weight")) ++D;
   if (D < 1 || D > kMaxLayers) return fail(ctx, ADN_ERR_INVALID, "sampling net: need layers.0.weight .. (1-12 layers)");
   const int nsplit = ctx->mlp0_terms == 3 ? 2 : 1;
-  net.nsplit = nsplit;
   MlpProgram P{};
   P.n_layers = D;
   std::vector<uint8_t> wblob;
@@ -252,27 +249,9 @@ adn_status build_net0(adn_ctx* ctx) {
       P.out_cols = n_out;
     }
   }
-  P.in0_blk = 0;
-  P.in0_nblk = 2;
-  P.in1_blk = 0;
-  P.in_tile_stride = uint32_t(2 * nsplit * kBlkBytes);
-  P.in0_off = 0;
-  P.in0_lo_off = 2 * kBlkBytes;
-  P.in1_off = 0;
+  P.in = sampling_tiles(net.n_in, nsplit);
+  P.in_nblk0 = P.in.n_blk;
   net.prog = P;
-  InputLayout lay{};
-  lay.n_blk = 2;
-  lay.src_col0[0] = 0;
-  lay.valid[0] = std::min(64, net.n_in);
-  lay.src_col0[1] = 64;
-  lay.valid[1] = std::max(0, net.n_in - 64);
-  lay.dst_off_hi[0] = 0;
-  lay.dst_off_hi[1] = kBlkBytes;
-  lay.dst_off_lo[0] = 2 * kBlkBytes;
-  lay.dst_off_lo[1] = 3 * kBlkBytes;
-  lay.tile_stride = P.in_tile_stride;
-  lay.nsplit = nsplit;
-  net.lay = lay;
   adn_status s = upload(ctx, net, wblob, fblob);
   if (s != ADN_OK) return s;
   net.ready = true;
@@ -306,7 +285,6 @@ adn_status build_net1(adn_ctx* ctx) {
   if (!fw || !fb || !aw || !ab || !vw || !vb || !rw || !rb || fb->data.size() != 256 || ab->data.size() != 1 ||
       vb->data.size() != 128 || rb->data.size() != 3)
     return fail(ctx, ADN_ERR_INVALID, "shading net: feature/alpha/views/rgb tensors missing or wrong shape");
-  net.nsplit = 1;
   net.n_in = 90;
   net.n_out = 4;
   MlpProgram P{};
@@ -366,26 +344,10 @@ adn_status build_net1(adn_ctx* ctx) {
   P.alpha_b_off = uint32_t(push_floats(fblob, ab->data.data(), 1));
   P.rgb_w_off = uint32_t(push_floats(fblob, rw->data.data(), 3 * 128));
   P.rgb_b_off = uint32_t(push_floats(fblob, rb->data.data(), 3));
-  P.in0_blk = 0;
-  P.in0_nblk = 1;
-  P.in1_blk = 0;
-  P.in_tile_stride = 2 * kBlkBytes;
-  P.in0_off = 0;
-  P.in0_lo_off = 0;
-  P.in1_off = kBlkBytes;
+  P.in = shading_tiles();
+  P.in_nblk0 = 1;   // P; V after layer 5
   P.out_cols = 4;
   net.prog = P;
-  InputLayout lay{};
-  lay.n_blk = 2;
-  lay.src_col0[0] = 0;
-  lay.valid[0] = 63;
-  lay.src_col0[1] = 63;
-  lay.valid[1] = 27;
-  lay.dst_off_hi[0] = 0;
-  lay.dst_off_hi[1] = kBlkBytes;
-  lay.tile_stride = 2 * kBlkBytes;
-  lay.nsplit = 1;
-  net.lay = lay;
   adn_status s = upload(ctx, net, wblob, fblob);
   if (s != ADN_OK) return s;
   net.ready = true;
@@ -453,7 +415,7 @@ int64_t pad128(int64_t n) { return (n + 127) / 128 * 128; }
 adn_status run_mlp(adn_ctx* ctx, int id, const uint8_t* tiles, float* out, const long long* rows_dev, long long rows,
                    cudaStream_t st, const EncodeParams* enc = nullptr) {
   Net& n = ctx->net[id];
-  const cudaError_t e = launch_mlp(n.nsplit, n.prog, n.d_wblob, tiles, out, rows_dev, rows, ctx->d_err, ctx->num_sms, st, enc);
+  const cudaError_t e = launch_mlp(n.prog, n.d_wblob, tiles, out, rows_dev, rows, ctx->d_err, ctx->num_sms, st, enc);
   if (e != cudaSuccess) return cuda_fail(ctx, e, id == 0 ? "launch sampling MLP" : "launch shading MLP");
   ctx->stats.kernel_launches++;
   return ADN_OK;
@@ -472,19 +434,12 @@ adn_status render_chunk(adn_ctx* ctx, const PoseDev& pd, const float* d_dirs, co
   adn_status s;
   Net& n0 = ctx->net[0];
   if (parts & kStages01) {
-    if ((s = ensure(ctx, ctx->tiles0, size_t(pad128(n) / 128) * n0.prog.in_tile_stride)) != ADN_OK) return s;
+    if ((s = ensure(ctx, ctx->tiles0, size_t(pad128(n) / 128) * n0.prog.in.tile_bytes())) != ADN_OK) return s;
     uint8_t* tiles0 = static_cast<uint8_t*>(ctx->tiles0.p);
     if (timing) cudaEventRecord(ctx->ev[0], st);
-    // stage 0
-    if (n0.nsplit == 2 && (n0.n_in == 90 || n0.n_in == 30) && n0.n_in == ctx->n_feat0) {   // stage 0 writes the packed hi / lo tiles itself
-      ADN_CUDA(ctx, launch_stage0(ctx->sc, pd, d_dirs, cam, n, nullptr, ray_o, ray_d, tiles0, st));
-      ctx->stats.kernel_launches++;
-    } else {
-      if ((s = ensure(ctx, ctx->x0, size_t(n) * ctx->n_feat0 * 4)) != ADN_OK) return s;
-      ADN_CUDA(ctx, launch_stage0(ctx->sc, pd, d_dirs, cam, n, static_cast<float*>(ctx->x0.p), ray_o, ray_d, nullptr, st));
-      ADN_CUDA(ctx, launch_pack_rows(static_cast<float*>(ctx->x0.p), n, nullptr, ctx->n_feat0, n0.lay, tiles0, st));
-      ctx->stats.kernel_launches += 2;
-    }
+    // stage 0 (writes the sampling net's packed input tiles)
+    ADN_CUDA(ctx, launch_stage0(ctx->sc, pd, d_dirs, cam, n, nullptr, ray_o, ray_d, tiles0, n0.prog.in.n_terms, st));
+    ctx->stats.kernel_launches++;
     if (timing) cudaEventRecord(ctx->ev[1], st);
     // stage 1
     if ((s = run_mlp(ctx, 0, tiles0, raw0, nullptr, n, st)) != ADN_OK) return s;
@@ -501,7 +456,7 @@ adn_status render_chunk(adn_ctx* ctx, const PoseDev& pd, const float* d_dirs, co
   }
   // stage 3 runs inside the shading kernel (encoder warp) unless the variant needs the stand-alone kernel
   const bool fused_enc = ctx->fuse_encoder && !ctx->scene.use_ndc;
-  if (!fused_enc && (s = ensure(ctx, ctx->tiles1, size_t(pad128(cap) / 128) * 2 * kBlkBytes)) != ADN_OK) return s;
+  if (!fused_enc && (s = ensure(ctx, ctx->tiles1, size_t(pad128(cap) / 128) * ctx->net[1].prog.in.tile_bytes())) != ADN_OK) return s;
   if ((s = ensure(ctx, ctx->raw1, size_t(pad128(cap)) * 16)) != ADN_OK) return s;
 
   int32_t* count = d_nsamples ? d_nsamples : static_cast<int32_t*>(ctx->count.p);
@@ -528,8 +483,7 @@ adn_status render_chunk(adn_ctx* ctx, const PoseDev& pd, const float* d_dirs, co
     ep.z = static_cast<float*>(ctx->zbuf.p);
     ep.zlut_dense = ctx->d_zlut_dense;
     ep.K = K;
-    for (int a = 0; a < 3; ++a) ep.c[a] = ctx->sc.c[a];
-    ep.sqrt_max_depth = ctx->sc.sqrt_max_depth;
+    ep.sc = ctx->sc;
   } else {
     ADN_CUDA(ctx, launch_stage3(ctx->sc, ray_o, ray_d, dense ? nullptr : static_cast<int32_t*>(ctx->rayidx.p),
                                 static_cast<float*>(ctx->zbuf.p), ctx->d_zlut_dense, K, cap, ctx->d_total, nullptr, tiles1, st));
@@ -732,8 +686,8 @@ void adn_destroy(adn_ctx* ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
   cudaDeviceSynchronize();
-  Buf* bufs[] = {&ctx->tiles0, &ctx->raw0, &ctx->x0,    &ctx->ray_o,  &ctx->ray_d, &ctx->dirs,      &ctx->count, &ctx->offset,
-                 &ctx->rayidx, &ctx->zbuf, &ctx->zpbuf, &ctx->tiles1, &ctx->raw1,  &ctx->s2scratch, &ctx->rgb,   &ctx->rgba, &ctx->x1, &ctx->metric,
+  Buf* bufs[] = {&ctx->tiles0, &ctx->raw0,  &ctx->ray_o,  &ctx->ray_d, &ctx->dirs,      &ctx->count, &ctx->offset,
+                 &ctx->rayidx, &ctx->zbuf,  &ctx->zpbuf,  &ctx->tiles1, &ctx->raw1,  &ctx->s2scratch, &ctx->rgb,   &ctx->rgba, &ctx->metric,
                  &ctx->budget_keys, &ctx->budget_work, &ctx->budget_thr};
   for (Buf* b : bufs)
     if (b->p) cudaFree(b->p);
@@ -1008,7 +962,7 @@ adn_status adn_stage0_features(adn_ctx* ctx, const float* pose, const float* rot
   if (!ctx || !pose || !rot || !d_dirs || n_rays < 0 || (d_ray_o == nullptr) != (d_ray_d == nullptr))
     return fail(ctx, ADN_ERR_INVALID, "stage0: bad arguments");
   ADN_CUDA(ctx, cudaSetDevice(ctx->device));
-  ADN_CUDA(ctx, launch_stage0(ctx->sc, make_pose(pose, rot), d_dirs, nullptr, n_rays, d_x0, d_ray_o, d_ray_d, nullptr,
+  ADN_CUDA(ctx, launch_stage0(ctx->sc, make_pose(pose, rot), d_dirs, nullptr, n_rays, d_x0, d_ray_o, d_ray_d, nullptr, 0,
                               static_cast<cudaStream_t>(stream)));
   ctx->stats.kernel_launches++;
   return ADN_OK;
@@ -1021,9 +975,9 @@ adn_status adn_mlp0_forward(adn_ctx* ctx, const float* d_x0, int64_t n_rays, flo
   ADN_CUDA(ctx, cudaSetDevice(ctx->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   Net& n = ctx->net[0];
-  adn_status s = ensure(ctx, ctx->tiles0, size_t(pad128(n_rays) / 128) * n.prog.in_tile_stride);
+  adn_status s = ensure(ctx, ctx->tiles0, size_t(pad128(n_rays) / 128) * n.prog.in.tile_bytes());
   if (s != ADN_OK) return s;
-  ADN_CUDA(ctx, launch_pack_rows(d_x0, n_rays, nullptr, n.n_in, n.lay, static_cast<uint8_t*>(ctx->tiles0.p), st));
+  ADN_CUDA(ctx, launch_pack_rows(d_x0, n_rays, nullptr, n.n_in, n.prog.in, static_cast<uint8_t*>(ctx->tiles0.p), st));
   ctx->stats.kernel_launches++;
   return run_mlp(ctx, 0, static_cast<uint8_t*>(ctx->tiles0.p), d_raw0, nullptr, n_rays, st);
 }
@@ -1077,9 +1031,9 @@ adn_status adn_mlp1_forward(adn_ctx* ctx, const float* d_x1, int64_t n_samples, 
   ADN_CUDA(ctx, cudaSetDevice(ctx->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   Net& n = ctx->net[1];
-  adn_status s = ensure(ctx, ctx->tiles1, size_t(pad128(n_samples) / 128) * n.prog.in_tile_stride);
+  adn_status s = ensure(ctx, ctx->tiles1, size_t(pad128(n_samples) / 128) * n.prog.in.tile_bytes());
   if (s != ADN_OK) return s;
-  ADN_CUDA(ctx, launch_pack_rows(d_x1, n_samples, nullptr, 90, n.lay, static_cast<uint8_t*>(ctx->tiles1.p), st));
+  ADN_CUDA(ctx, launch_pack_rows(d_x1, n_samples, nullptr, n.n_in, n.prog.in, static_cast<uint8_t*>(ctx->tiles1.p), st));
   ctx->stats.kernel_launches++;
   return run_mlp(ctx, 1, static_cast<uint8_t*>(ctx->tiles1.p), d_raw1, nullptr, n_samples, st);
 }

@@ -5,13 +5,9 @@
 #include "mlp.cuh"
 #include "posenc.cuh"
 #include "ptx.cuh"
+#include "tiles.cuh"
 
 namespace adn {
-
-__device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
-  __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&h);
-}
 
 // A set of layer flags known at compile time: the epilogue's tests of it fold away.
 template <uint8_t V>
@@ -31,10 +27,10 @@ struct MlpCfg {
 };
 static_assert(MlpCfg<1>::kSmemBytes <= 232448 && MlpCfg<2>::kSmemBytes <= 232448, "shared memory per block (sm_90)");
 
-// One row of a fused-encoder input block: P (63 position features + 0) or V (27 direction features + zeros), computed
-// and packed to bf16 exactly as stage3_kernel does it (same device functions, same operation order).
+// One row of a fused-encoder input block: P (the 63 position features and a zero column) or V (the 27 direction features
+// and zeros) of the shading tile format, computed and packed as stage3_kernel computes and packs them for a non-NDC scene.
 template <bool VIEW>
-__device__ __forceinline__ void encode_row(const EncodeParams& enc, long long i, long long rows, uint32_t blk, int row) {
+__device__ __forceinline__ void encode_row(const EncodeParams& enc, long long i, long long rows, uint8_t* blk, int row) {
   float f[64];
 #pragma unroll
   for (int k = 0; k < 64; ++k) f[k] = 0.0f;
@@ -48,29 +44,13 @@ __device__ __forceinline__ void encode_row(const EncodeParams& enc, long long i,
       ray = i / enc.K;
       zw = enc.zlut_dense[i - ray * enc.K];
     }
-    float v[3];
-    if (VIEW) {
-#pragma unroll
-      for (int a = 0; a < 3; ++a) v[a] = __ldg(enc.ray_d + 3 * ray + a);
-      posenc3<4>(v, f);
-    } else {
-      // pos = o + d z, then normalization_inverse_sqrt_dist_centered (same operation order as stage3_kernel)
-#pragma unroll
-      for (int a = 0; a < 3; ++a)
-        v[a] = __fsub_rn(__fadd_rn(__ldg(enc.ray_o + 3 * ray + a), __fmul_rn(__ldg(enc.ray_d + 3 * ray + a), zw)), enc.c[a]);
-      const float nrm = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(v[0], v[0]), __fmul_rn(v[1], v[1])), __fmul_rn(v[2], v[2])));
-      const float den = __fmul_rn(enc.sqrt_max_depth, __fsqrt_rn(nrm));
-#pragma unroll
-      for (int a = 0; a < 3; ++a) v[a] = __fdiv_rn(v[a], den);
-      posenc3<10>(v, f);
-    }
+    float pos[3], dir[3];
+    sample_inputs(enc.sc, false, enc.ray_o, enc.ray_d, ray, zw, pos, dir);
+    if (VIEW) posenc3<4>(dir, f);
+    else posenc3<10>(pos, f);
   }
 #pragma unroll
-  for (int ch = 0; ch < 8; ++ch) {
-    const float* q = f + ch * 8;
-    st_shared_v4(blk + sw128_offset(uint32_t(row), uint32_t(ch * 8)), bf16x2(q[0], q[1]), bf16x2(q[2], q[3]), bf16x2(q[4], q[5]),
-                 bf16x2(q[6], q[7]));
-  }
+  for (int ch = 0; ch < 8; ++ch) pack_chunk8(f + ch * 8, uint32_t(row), ch, blk, nullptr);
 }
 
 // This warpgroup's 64 rows (the first or second 8 KB) of `nblk` consecutive packed blocks, global -> shared.
@@ -170,11 +150,11 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
   for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) {
     // tile input (the previous tile's last MMAs retired before its epilogue: the blocks are free)
     if (ENC) {
-      if (tw < 64) encode_row<false>(enc, t * kTileM + 64 * wg + tw, rows, blk_addr(0, prog.in0_blk), 64 * wg + tw);
+      if (tw < 64) encode_row<false>(enc, t * kTileM + 64 * wg + tw, rows, act, 64 * wg + tw);
     } else {
-      const uint8_t* src = in_tiles + size_t(t) * prog.in_tile_stride;
-      copy_rows(src + prog.in0_off, blk_addr(0, prog.in0_blk), prog.in0_nblk, wg, tw);
-      if (NSPLIT == 2) copy_rows(src + prog.in0_lo_off, blk_addr(1, prog.in0_blk), prog.in0_nblk, wg, tw);
+#pragma unroll
+      for (int term = 0; term < NSPLIT; ++term)
+        copy_rows(in_tiles + size_t(t) * prog.in.tile_bytes() + prog.in.blk_off(term, 0), blk_addr(term, 0), prog.in_nblk0, wg, tw);
     }
     fence_proxy_async_smem();
     named_bar_sync(bar_id, 128);
@@ -250,12 +230,9 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
               }
               if (flags & LF_OUT_ACT) {
                 const uint32_t off = uint32_t(L.out_blk0 + (col >> 6)) * kBlkBytes + sw128_offset(uint32_t(row), uint32_t(col & 63));
-                const uint32_t hi = pack_bf16x2(v0, v1);
+                const uint32_t hi = bf16x2(v0, v1);
                 *reinterpret_cast<uint32_t*>(act + off) = hi;
-                if (NSPLIT == 2) {
-                  const uint32_t lo = pack_bf16x2(v0 - __uint_as_float(hi << 16), v1 - __uint_as_float(hi & 0xFFFF0000u));
-                  *reinterpret_cast<uint32_t*>(act + NB * kBlkBytes + off) = lo;
-                }
+                if (NSPLIT == 2) *reinterpret_cast<uint32_t*>(act + NB * kBlkBytes + off) = bf16x2_lo(v0, v1, hi);
               }
               if (flags & LF_FINAL_RGB) {
 #pragma unroll
@@ -296,11 +273,11 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
         case LF_FINAL_RAW: epilogue(ConstFlags<LF_FINAL_RAW>{}); break;
         default: epilogue(F(L.flags)); break;   // any other combination: the same code with run-time tests
       }
-      if (L.flags & LF_LOAD_IN1_AFTER) {   // the 2nd input block (view directions) replaces the tile-start block
+      if (L.flags & LF_LOAD_IN1_AFTER) {   // the next input block (view directions) replaces activation block 0
         if (ENC) {
-          if (tw < 64) encode_row<true>(enc, t * kTileM + 64 * wg + tw, rows, blk_addr(0, prog.in1_blk), 64 * wg + tw);
+          if (tw < 64) encode_row<true>(enc, t * kTileM + 64 * wg + tw, rows, act, 64 * wg + tw);
         } else {
-          copy_rows(in_tiles + size_t(t) * prog.in_tile_stride + prog.in1_off, blk_addr(0, prog.in1_blk), 1, wg, tw);
+          copy_rows(in_tiles + size_t(t) * prog.in.tile_bytes() + prog.in.blk_off(0, prog.in_nblk0), blk_addr(0, 0), 1, wg, tw);
         }
       }
       fence_proxy_async_smem();        // generic-proxy stores -> visible to the next layer's wgmma reads
@@ -310,49 +287,21 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
 }
 
 // -------------------------------------------------------------------------------------------------
-// fp32 feature rows [rows, n_feat] -> packed bf16 (hi / lo) SWIZZLE_128B tile blocks.
+// fp32 feature rows [rows, n_feat] -> packed tiles of format `fmt`.
 // One thread per (row, block, 16-byte chunk): 8 consecutive source columns.
 __global__ void pack_rows_kernel(const float* __restrict__ x, long long rows_host, const long long* __restrict__ rows_dev,
-                                 int n_feat, const __grid_constant__ InputLayout lay, uint8_t* __restrict__ tiles) {
+                                 int n_feat, const __grid_constant__ TileFormat fmt, uint8_t* __restrict__ tiles) {
   const long long rows = rows_dev ? *rows_dev : rows_host;
   const long long n_tiles = (rows + kTileM - 1) / kTileM;
-  const long long total = n_tiles * kTileM * lay.n_blk * 8;
+  const long long total = n_tiles * kTileM * fmt.n_blk * 8;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const int chunk = int(i & 7);
     const long long rb = i >> 3;
-    const int blk = int(rb % lay.n_blk);
-    const long long row = rb / lay.n_blk;
-    const int r = int(row & (kTileM - 1));
+    const int blk = int(rb % fmt.n_blk);
+    const long long row = rb / fmt.n_blk;
     const long long t = row >> 7;
-    float v[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int kk = chunk * 8 + j;
-      v[j] = (row < rows && kk < lay.valid[blk]) ? x[row * n_feat + lay.src_col0[blk] + kk] : 0.0f;
-    }
-    uint4 hi;
-    hi.x = pack_bf16x2(v[0], v[1]);
-    hi.y = pack_bf16x2(v[2], v[3]);
-    hi.z = pack_bf16x2(v[4], v[5]);
-    hi.w = pack_bf16x2(v[6], v[7]);
-    const uint32_t off = sw128_offset(uint32_t(r), uint32_t(chunk * 8));
-    uint8_t* tb = tiles + size_t(t) * lay.tile_stride;
-    *reinterpret_cast<uint4*>(tb + lay.dst_off_hi[blk] + off) = hi;
-    if (lay.nsplit == 2) {
-      const uint32_t hw[4] = {hi.x, hi.y, hi.z, hi.w};
-      float l[8];
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        l[2 * e + 0] = v[2 * e + 0] - __uint_as_float(hw[e] << 16);
-        l[2 * e + 1] = v[2 * e + 1] - __uint_as_float(hw[e] & 0xFFFF0000u);
-      }
-      uint4 lo;
-      lo.x = pack_bf16x2(l[0], l[1]);
-      lo.y = pack_bf16x2(l[2], l[3]);
-      lo.z = pack_bf16x2(l[4], l[5]);
-      lo.w = pack_bf16x2(l[6], l[7]);
-      *reinterpret_cast<uint4*>(tb + lay.dst_off_lo[blk] + off) = lo;
-    }
+    pack_tile_chunk(fmt, tiles + size_t(t) * fmt.tile_bytes(), blk, uint32_t(row & (kTileM - 1)), chunk,
+                    [&](int c) { return row < rows ? x[row * n_feat + c] : 0.0f; });
   }
 }
 
@@ -386,24 +335,24 @@ static cudaError_t launch_mlp_t(const MlpProgram& prog, const uint8_t* wblob, co
   return cudaGetLastError();
 }
 
-cudaError_t launch_mlp(int nsplit, const MlpProgram& prog, const uint8_t* wblob, const uint8_t* in_tiles, float* out,
+cudaError_t launch_mlp(const MlpProgram& prog, const uint8_t* wblob, const uint8_t* in_tiles, float* out,
                        const long long* rows_dev, long long rows_host, int* err_flag, int num_sms, cudaStream_t stream,
                        const EncodeParams* enc) {
   if (enc) {   // shading net with the fused input encoder
-    if (nsplit != 1) return cudaErrorInvalidValue;
+    if (prog.in.n_terms != 1) return cudaErrorInvalidValue;
     return launch_mlp_t<1, true>(prog, wblob, in_tiles, out, rows_dev, rows_host, err_flag, num_sms, stream, *enc);
   }
-  if (nsplit == 2) return launch_mlp_t<2, false>(prog, wblob, in_tiles, out, rows_dev, rows_host, err_flag, num_sms, stream, EncodeParams{});
+  if (prog.in.n_terms == 2) return launch_mlp_t<2, false>(prog, wblob, in_tiles, out, rows_dev, rows_host, err_flag, num_sms, stream, EncodeParams{});
   return launch_mlp_t<1, false>(prog, wblob, in_tiles, out, rows_dev, rows_host, err_flag, num_sms, stream, EncodeParams{});
 }
 
-cudaError_t launch_pack_rows(const float* x, long long rows, const long long* rows_dev, int n_feat, const InputLayout& lay,
+cudaError_t launch_pack_rows(const float* x, long long rows, const long long* rows_dev, int n_feat, const TileFormat& fmt,
                              uint8_t* tiles, cudaStream_t stream) {
-  long long work = ((rows + kTileM - 1) / kTileM) * kTileM * lay.n_blk * 8;
+  long long work = ((rows + kTileM - 1) / kTileM) * kTileM * fmt.n_blk * 8;
   int grid = int((work + 255) / 256);
   if (grid < 1) grid = 1;
   if (grid > 132 * 16) grid = 132 * 16;
-  pack_rows_kernel<<<grid, 256, 0, stream>>>(x, rows, rows_dev, n_feat, lay, tiles);
+  pack_rows_kernel<<<grid, 256, 0, stream>>>(x, rows, rows_dev, n_feat, fmt, tiles);
   return cudaGetLastError();
 }
 

@@ -18,10 +18,11 @@
 #include <cstdint>
 #include <cuda_runtime.h>
 
+#include "stages.cuh"
+#include "tiles.cuh"
+
 namespace adn {
 
-constexpr int kTileM = 128;
-constexpr int kBlkBytes = 16384;  // one [128 x 64] bf16 SWIZZLE_128B block
 constexpr int kMaxLayers = 12;
 constexpr int kMlpThreads = 384;  // three warpgroups: two consumers, one weight producer
 constexpr int kSideFloats = 3208; // fp32 side parameters (biases, alpha / rgb heads), copied to shared memory per CTA
@@ -32,7 +33,7 @@ enum : uint8_t {
   LF_OUT_ACT = 4,        // write bf16 activations for the next layer
   LF_FINAL_RAW = 8,      // write fp32 rows to global (sampling net output / test programs)
   LF_FINAL_RGB = 16,     // rgb_linear on CUDA cores + write float4 (rgb, alpha)
-  LF_LOAD_IN1_AFTER = 32,  // once this layer's MMAs are done, fetch the 2nd input block (view dirs)
+  LF_LOAD_IN1_AFTER = 32,  // once this layer's MMAs are done, fetch the input block after the tile-start ones (view dirs)
   LF_WAIT_IN = 64          // this layer reads that 2nd input block
 };
 
@@ -51,25 +52,13 @@ struct MlpLayer {
 
 struct MlpProgram {
   int32_t n_layers;
-  int32_t in0_blk, in0_nblk;  // tile-start input: destination block, number of blocks (per term)
-  int32_t in1_blk;            // 2nd input destination block
-  uint32_t in_tile_stride;    // bytes per tile in the packed input buffer
-  uint32_t in0_off, in0_lo_off, in1_off;
+  TileFormat in;              // the packed input tiles (in.n_terms == NSPLIT)
+  int32_t in_nblk0;           // input blocks (per term) loaded into activation blocks 0.. at tile start; the next one
+                              // replaces block 0 after the LF_LOAD_IN1_AFTER layer
   uint32_t alpha_w_off, alpha_b_off, rgb_w_off, rgb_b_off;  // float offsets in `side`
   int32_t out_cols;           // row stride of the FINAL_RAW output
   MlpLayer layers[kMaxLayers];
   float side[kSideFloats];
-};
-
-// Describes how fp32 feature rows map onto the packed bf16 input blocks of a tile.
-struct InputLayout {
-  int32_t n_blk;
-  int32_t src_col0[4];
-  int32_t valid[4];
-  uint32_t dst_off_hi[4];
-  uint32_t dst_off_lo[4];
-  uint32_t tile_stride;
-  int32_t nsplit;
 };
 
 // Fused input encoder of the shading MLP (stage 3 inside the kernel): the consumer warpgroups compute the positional
@@ -83,20 +72,20 @@ struct EncodeParams {
   const float* z = nullptr;           // [M] world depth of the packed samples
   const float* zlut_dense = nullptr;  // [K]
   int K = 1;
-  float c[3] = {0.f, 0.f, 0.f};       // view_cell_center
-  float sqrt_max_depth = 1.0f;
+  SceneDev sc{};                      // non-NDC scenes only
 };
 
 // cudaFuncAttributeMaxDynamicSharedMemorySize is a per-device attribute: set it once per (kernel, device).
 // `done` is the caller's per-kernel bit mask (one static per launcher).
 cudaError_t set_max_dyn_smem_once(const void* func, int bytes, unsigned long long* done);
 
-// Launchers (defined in mlp.cu).  rows_dev may be null (then rows_host is used).  enc != nullptr: shading net with the
-// fused input encoder (in_tiles unused).
-cudaError_t launch_mlp(int nsplit, const MlpProgram& prog, const uint8_t* wblob, const uint8_t* in_tiles, float* out,
+// Launchers (defined in mlp.cu).  rows_dev may be null (then rows_host is used).  prog.in.n_terms == 2: split precision.
+// enc != nullptr: shading net with the fused input encoder (in_tiles unused).
+cudaError_t launch_mlp(const MlpProgram& prog, const uint8_t* wblob, const uint8_t* in_tiles, float* out,
                        const long long* rows_dev, long long rows_host, int* err_flag, int num_sms, cudaStream_t stream,
                        const EncodeParams* enc = nullptr);
-cudaError_t launch_pack_rows(const float* x, long long rows, const long long* rows_dev, int n_feat,
-                             const InputLayout& lay, uint8_t* tiles, cudaStream_t stream);
+// fp32 feature rows [rows, n_feat] -> packed tiles of format `fmt`.
+cudaError_t launch_pack_rows(const float* x, long long rows, const long long* rows_dev, int n_feat, const TileFormat& fmt,
+                             uint8_t* tiles, cudaStream_t stream);
 
 }  // namespace adn

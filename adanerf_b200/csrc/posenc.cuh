@@ -1,17 +1,11 @@
 // Positional-encoding helpers shared by the feature kernels (stages.cu) and the shading MLP's fused input encoder
 // (mlp.cu).
 #pragma once
-#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 
-#include <cstdint>
+#include "stages.cuh"
 
 namespace adn {
-
-__device__ __forceinline__ uint32_t bf16x2(float a, float b) {
-  __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&h);
-}
 
 // enc_L(v) = [v, sin(2^0 v), cos(2^0 v), ..., sin(2^(L-1) v), cos(2^(L-1) v)], each term a 3-vector
 // (src/util/feature_encoding.py:60-73).  Writes 3 + 6L floats.
@@ -42,6 +36,50 @@ __device__ __forceinline__ void posenc3(const float (&v)[3], float* out) {
       out[3 + 6 * f + a] = s;
       out[3 + 6 * f + 3 + a] = c;
     }
+  }
+}
+
+// The shading net's inputs of one sample at world depth zw on ray r (RayMarchFromPoses.batch, src/features.py:458-479), in
+// the reference's operation order: the position into pos and the direction to encode into dir.  Stage 3 and the fused
+// encoder both call this, so their features are the same bits.
+__device__ __forceinline__ void sample_inputs(const SceneDev& sc, bool ndc, const float* __restrict__ ray_o,
+                                              const float* __restrict__ ray_d, long long r, float zw, float (&pos)[3],
+                                              float (&dir)[3]) {
+  float o[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    o[a] = __ldg(ray_o + 3 * r + a);
+    dir[a] = __ldg(ray_d + 3 * r + a);   // un-normalised nds, as SpherePosDir hands it on
+  }
+  if (ndc) {
+    // ndc_rays(H, W, focal, near = 1) (src/nerf_raymarch_common.py:71-88) in the reference's operation order, then
+    // pos = o' + d' z with the un-normalised NDC direction, no position normalisation, view encoding of d' / |d'|
+    const float t = __fdiv_rn(-__fadd_rn(1.0f, o[2]), dir[2]);
+    float on[3];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) on[a] = __fadd_rn(o[a], __fmul_rn(t, dir[a]));
+    const float q0 = __fdiv_rn(on[0], on[2]), q1 = __fdiv_rn(on[1], on[2]);
+    const float o0 = __fdiv_rn(__fmul_rn(sc.ndc_cw, on[0]), on[2]);
+    const float o1 = __fdiv_rn(__fmul_rn(sc.ndc_ch, on[1]), on[2]);
+    const float o2 = __fadd_rn(1.0f, __fdiv_rn(2.0f, on[2]));
+    const float d0 = __fmul_rn(sc.ndc_cw, __fsub_rn(__fdiv_rn(dir[0], dir[2]), q0));
+    const float d1 = __fmul_rn(sc.ndc_ch, __fsub_rn(__fdiv_rn(dir[1], dir[2]), q1));
+    const float d2 = __fdiv_rn(-2.0f, on[2]);
+    pos[0] = __fadd_rn(o0, __fmul_rn(d0, zw));                                                    // :458
+    pos[1] = __fadd_rn(o1, __fmul_rn(d1, zw));
+    pos[2] = __fadd_rn(o2, __fmul_rn(d2, zw));
+    const float dn = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(d0, d0), __fmul_rn(d1, d1)), __fmul_rn(d2, d2)));
+    dir[0] = __fdiv_rn(d0, dn);                                                                   // :431
+    dir[1] = __fdiv_rn(d1, dn);
+    dir[2] = __fdiv_rn(d2, dn);
+  } else {
+#pragma unroll
+    for (int a = 0; a < 3; ++a) pos[a] = __fsub_rn(__fadd_rn(o[a], __fmul_rn(dir[a], zw)), sc.c[a]);   // :458, loc = pos - c
+    // normalization_inverse_sqrt_dist_centered (src/nerf_raymarch_common.py:226-230)
+    const float nrm = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(pos[0], pos[0]), __fmul_rn(pos[1], pos[1])), __fmul_rn(pos[2], pos[2])));
+    const float den = __fmul_rn(sc.sqrt_max_depth, __fsqrt_rn(nrm));
+#pragma unroll
+    for (int a = 0; a < 3; ++a) pos[a] = __fdiv_rn(pos[a], den);
   }
 }
 

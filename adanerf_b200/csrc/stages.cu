@@ -10,6 +10,7 @@
 #include "posenc.cuh"
 #include "ptx.cuh"
 #include "stages.cuh"
+#include "tiles.cuh"
 
 namespace adn {
 
@@ -52,11 +53,12 @@ template <bool FROM_CAMERA, int NFD = kNFreqDir, int NFP = kNFreqPos>
 __global__ void __launch_bounds__(128)
 stage0_kernel(const __grid_constant__ SceneDev sc, const __grid_constant__ PoseDev pd, const float* __restrict__ dirs,
               const __grid_constant__ CameraRays cam, long long n_rays, float* __restrict__ x0, float* __restrict__ ray_o,
-              float* __restrict__ ray_d, uint8_t* __restrict__ tiles0) {
+              float* __restrict__ ray_d, uint8_t* __restrict__ tiles0, int tile_terms) {
+  constexpr int F0 = 6 + 6 * (NFD + NFP);       // 90 ("10-4") or 30 ("2-2")
   const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;   // grid covers whole 128-ray tiles
-  float f[128];
+  float f[F0];
 #pragma unroll
-  for (int j = 0; j < 128; ++j) f[j] = 0.0f;
+  for (int j = 0; j < F0; ++j) f[j] = 0.0f;
   if (i < n_rays) {
     float d[3];
     if (FROM_CAMERA) {
@@ -86,7 +88,6 @@ stage0_kernel(const __grid_constant__ SceneDev sc, const __grid_constant__ PoseD
     float dn[3];
 #pragma unroll
     for (int a = 0; a < 3; ++a) dn[a] = __fdiv_rn(nds[a], nn);
-    constexpr int F0 = 6 + 6 * (NFD + NFP);       // 90 ("10-4") or 30 ("2-2")
     posenc3<NFD>(dn, f);                           // 27 / 15: direction block FIRST (:868)
     posenc3<NFP>(p, f + 3 + 6 * NFD);              // 63 / 15
     if (ray_o) {
@@ -101,70 +102,39 @@ stage0_kernel(const __grid_constant__ SceneDev sc, const __grid_constant__ PoseD
       for (int j = 0; j < F0; ++j) x0[i * F0 + j] = f[j];
     }
   }
-  if (tiles0) {
-    // packed MLP0 input: per tile [hi blk0 | hi blk1 | lo blk0 | lo blk1], 16 KB each.  The block (= one
-    // 128-ray tile) assembles the 64 KB image in shared memory and one thread hands it to the TMA engine
-    // (bulk shared -> global copy): no strided 16-byte global stores.
+  if (tiles0) {   // the CTA's 128 rays are one tile of the sampling net's input
     extern __shared__ __align__(1024) uint8_t s_tile[];
-    const long long t = i >> 7;
-    const uint32_t r = uint32_t(i & 127);
-#pragma unroll
-    for (int b = 0; b < 2; ++b) {
-#pragma unroll
-      for (int ch = 0; ch < 8; ++ch) {
-        const float* v = f + b * 64 + ch * 8;
-        uint4 hi;
-        hi.x = bf16x2(v[0], v[1]);
-        hi.y = bf16x2(v[2], v[3]);
-        hi.z = bf16x2(v[4], v[5]);
-        hi.w = bf16x2(v[6], v[7]);
-        const uint32_t hw[4] = {hi.x, hi.y, hi.z, hi.w};
-        uint32_t lw[4];
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const float l0 = v[2 * e + 0] - __uint_as_float(hw[e] << 16);
-          const float l1 = v[2 * e + 1] - __uint_as_float(hw[e] & 0xFFFF0000u);
-          lw[e] = bf16x2(l0, l1);
-        }
-        const uint32_t off = sw128_offset(r, uint32_t(ch * 8));
-        *reinterpret_cast<uint4*>(s_tile + b * kBlkBytes + off) = hi;
-        *reinterpret_cast<uint4*>(s_tile + (2 + b) * kBlkBytes + off) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-      }
-    }
-    fence_proxy_async_smem();
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      bulk_s2g(tiles0 + size_t(t) * (4 * kBlkBytes), s_tile, 4 * kBlkBytes);
-      bulk_commit();
-      bulk_wait_all();
-    }
+    const TileFormat fmt = sampling_tiles(F0, tile_terms);
+    store_tile(fmt, f, s_tile, tiles0 + size_t(i >> 7) * fmt.tile_bytes());
+    store_tiles_drain();
   }
 }
 
 cudaError_t launch_stage0(const SceneDev& sc, const PoseDev& pd, const float* d_dirs, const CameraRays* cam,
-                          long long n_rays, float* d_x0, float* d_ray_o, float* d_ray_d, uint8_t* d_tiles0,
+                          long long n_rays, float* d_x0, float* d_ray_o, float* d_ray_d, uint8_t* d_tiles0, int tile_terms,
                           cudaStream_t s) {
   if (n_rays <= 0) return cudaSuccess;
   const long long n_pad = ((n_rays + kTileM - 1) / kTileM) * kTileM;
   const unsigned grid = unsigned((n_pad + 127) / 128);
   CameraRays c{};
-  const size_t smem = d_tiles0 ? size_t(4 * kBlkBytes) : 0;
+  const int tile_bytes = int(sampling_tiles(0, 2).tile_bytes());   // the largest sampling tile
+  const size_t smem = d_tiles0 ? sampling_tiles(0, tile_terms).tile_bytes() : 0;
   static unsigned long long attr_cam = 0, attr_rays = 0;   // per device
-  if (set_max_dyn_smem_once(reinterpret_cast<const void*>(stage0_kernel<true>), 4 * kBlkBytes, &attr_cam) != cudaSuccess ||
-      set_max_dyn_smem_once(reinterpret_cast<const void*>(stage0_kernel<false>), 4 * kBlkBytes, &attr_rays) != cudaSuccess)
+  if (set_max_dyn_smem_once(reinterpret_cast<const void*>(stage0_kernel<true>), tile_bytes, &attr_cam) != cudaSuccess ||
+      set_max_dyn_smem_once(reinterpret_cast<const void*>(stage0_kernel<false>), tile_bytes, &attr_rays) != cudaSuccess)
     return cudaGetLastError();
   if (cam) c = *cam;
-  if (sc.n_freq_pos0 == 2 && sc.n_freq_dir0 == 2) {   // "2-2" (NDC configs): 30 features, same tile image (columns 30.. are zero)
+  if (sc.n_freq_pos0 == 2 && sc.n_freq_dir0 == 2) {   // "2-2" (NDC configs): 30 features
     static unsigned long long attr_cam22 = 0, attr_rays22 = 0;
-    if (set_max_dyn_smem_once(reinterpret_cast<const void*>(stage0_kernel<true, 2, 2>), 4 * kBlkBytes, &attr_cam22) != cudaSuccess ||
-        set_max_dyn_smem_once(reinterpret_cast<const void*>(stage0_kernel<false, 2, 2>), 4 * kBlkBytes, &attr_rays22) != cudaSuccess)
+    if (set_max_dyn_smem_once(reinterpret_cast<const void*>(stage0_kernel<true, 2, 2>), tile_bytes, &attr_cam22) != cudaSuccess ||
+        set_max_dyn_smem_once(reinterpret_cast<const void*>(stage0_kernel<false, 2, 2>), tile_bytes, &attr_rays22) != cudaSuccess)
       return cudaGetLastError();
-    if (cam) stage0_kernel<true, 2, 2><<<grid, 128, smem, s>>>(sc, pd, d_dirs, c, n_rays, d_x0, d_ray_o, d_ray_d, d_tiles0);
-    else stage0_kernel<false, 2, 2><<<grid, 128, smem, s>>>(sc, pd, d_dirs, c, n_rays, d_x0, d_ray_o, d_ray_d, d_tiles0);
+    if (cam) stage0_kernel<true, 2, 2><<<grid, 128, smem, s>>>(sc, pd, d_dirs, c, n_rays, d_x0, d_ray_o, d_ray_d, d_tiles0, tile_terms);
+    else stage0_kernel<false, 2, 2><<<grid, 128, smem, s>>>(sc, pd, d_dirs, c, n_rays, d_x0, d_ray_o, d_ray_d, d_tiles0, tile_terms);
   } else if (cam) {
-    stage0_kernel<true><<<grid, 128, smem, s>>>(sc, pd, d_dirs, c, n_rays, d_x0, d_ray_o, d_ray_d, d_tiles0);
+    stage0_kernel<true><<<grid, 128, smem, s>>>(sc, pd, d_dirs, c, n_rays, d_x0, d_ray_o, d_ray_d, d_tiles0, tile_terms);
   } else {
-    stage0_kernel<false><<<grid, 128, smem, s>>>(sc, pd, d_dirs, c, n_rays, d_x0, d_ray_o, d_ray_d, d_tiles0);
+    stage0_kernel<false><<<grid, 128, smem, s>>>(sc, pd, d_dirs, c, n_rays, d_x0, d_ray_o, d_ray_d, d_tiles0, tile_terms);
   }
   return cudaGetLastError();
 }
@@ -904,9 +874,9 @@ stage3_kernel(const __grid_constant__ SceneDev sc, const float* __restrict__ ray
   const long long n_samples = n_samples_dev ? *n_samples_dev : n_samples_host;
   const long long n_pad = ((n_samples + kTileM - 1) / kTileM) * kTileM;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n_pad; i += (long long)gridDim.x * blockDim.x) {
-    float f[128];
+    float f[kFeat];
 #pragma unroll
-    for (int j = 0; j < 128; ++j) f[j] = 0.0f;
+    for (int j = 0; j < kFeat; ++j) f[j] = 0.0f;
     if (i < n_samples) {
       long long r;
       float zw;
@@ -917,81 +887,24 @@ stage3_kernel(const __grid_constant__ SceneDev sc, const float* __restrict__ ray
         r = i / K;
         zw = zlut_dense[i - r * K];
       }
-      float o[3], d[3], pos[3];
-#pragma unroll
-      for (int a = 0; a < 3; ++a) {
-        o[a] = __ldg(ray_o + 3 * r + a);
-        d[a] = __ldg(ray_d + 3 * r + a);
-      }
-      if (sc.ndc) {
-        // ndc_rays(H, W, focal, near = 1) (src/nerf_raymarch_common.py:71-88) in the reference's operation order, then
-        // pos = o' + d' z with the un-normalised NDC direction, no position normalisation, view encoding of d' / |d'|
-        const float t = __fdiv_rn(-__fadd_rn(1.0f, o[2]), d[2]);
-        float on[3];
-#pragma unroll
-        for (int a = 0; a < 3; ++a) on[a] = __fadd_rn(o[a], __fmul_rn(t, d[a]));
-        const float q0 = __fdiv_rn(on[0], on[2]), q1 = __fdiv_rn(on[1], on[2]);
-        const float o0 = __fdiv_rn(__fmul_rn(sc.ndc_cw, on[0]), on[2]);
-        const float o1 = __fdiv_rn(__fmul_rn(sc.ndc_ch, on[1]), on[2]);
-        const float o2 = __fadd_rn(1.0f, __fdiv_rn(2.0f, on[2]));
-        const float d0 = __fmul_rn(sc.ndc_cw, __fsub_rn(__fdiv_rn(d[0], d[2]), q0));
-        const float d1 = __fmul_rn(sc.ndc_ch, __fsub_rn(__fdiv_rn(d[1], d[2]), q1));
-        const float d2 = __fdiv_rn(-2.0f, on[2]);
-        pos[0] = __fadd_rn(o0, __fmul_rn(d0, zw));                                                    // :458
-        pos[1] = __fadd_rn(o1, __fmul_rn(d1, zw));
-        pos[2] = __fadd_rn(o2, __fmul_rn(d2, zw));
-        const float dn = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(d0, d0), __fmul_rn(d1, d1)), __fmul_rn(d2, d2)));
-        d[0] = __fdiv_rn(d0, dn);                                                                     // :431
-        d[1] = __fdiv_rn(d1, dn);
-        d[2] = __fdiv_rn(d2, dn);
-      } else {
-#pragma unroll
-        for (int a = 0; a < 3; ++a) pos[a] = __fsub_rn(__fadd_rn(o[a], __fmul_rn(d[a], zw)), sc.c[a]);   // :458, loc = pos - c
-        // normalization_inverse_sqrt_dist_centered (src/nerf_raymarch_common.py:226-230)
-        const float nrm = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(pos[0], pos[0]), __fmul_rn(pos[1], pos[1])), __fmul_rn(pos[2], pos[2])));
-        const float den = __fmul_rn(sc.sqrt_max_depth, __fsqrt_rn(nrm));
-#pragma unroll
-        for (int a = 0; a < 3; ++a) pos[a] = __fdiv_rn(pos[a], den);
-      }
+      float pos[3], d[3];
+      sample_inputs(sc, sc.ndc != 0, ray_o, ray_d, r, zw, pos, d);
       posenc3<kNFreqPos>(pos, f);                      // 63: position block FIRST (:473-479)
-      posenc3<kNFreqDir>(d, f + 64);                   // 27 (un-renormalised nds), staged at column 64
+      posenc3<kNFreqDir>(d, f + 63);                   // 27
       if (x1) {
 #pragma unroll
-        for (int j = 0; j < 63; ++j) x1[i * kFeat + j] = f[j];
-#pragma unroll
-        for (int j = 0; j < 27; ++j) x1[i * kFeat + 63 + j] = f[64 + j];
+        for (int j = 0; j < kFeat; ++j) x1[i * kFeat + j] = f[j];
       }
     }
-    if (tiles1) {
-      // packed MLP1 input: per tile [P: 63 pos features + 0 | V: 27 dir features + zeros], 16 KB each; staged in
-      // shared memory and written with one bulk shared -> global copy per tile (TMA engine)
+    if (tiles1) {   // the CTA's 128 samples are one tile of the shading net's input
       extern __shared__ __align__(1024) uint8_t s_tile[];
-      const long long t = i >> 7;
-      const uint32_t r = uint32_t(i & 127);
+      const TileFormat fmt = shading_tiles();
       if (threadIdx.x == 0) bulk_wait_read_all();   // the previous tile's copy has finished reading s_tile
       __syncthreads();
-#pragma unroll
-      for (int b = 0; b < 2; ++b) {
-#pragma unroll
-        for (int ch = 0; ch < 8; ++ch) {
-          const float* v = f + b * 64 + ch * 8;
-          uint4 hi;
-          hi.x = bf16x2(v[0], v[1]);
-          hi.y = bf16x2(v[2], v[3]);
-          hi.z = bf16x2(v[4], v[5]);
-          hi.w = bf16x2(v[6], v[7]);
-          *reinterpret_cast<uint4*>(s_tile + b * kBlkBytes + sw128_offset(r, uint32_t(ch * 8))) = hi;
-        }
-      }
-      fence_proxy_async_smem();
-      __syncthreads();
-      if (threadIdx.x == 0) {
-        bulk_s2g(tiles1 + size_t(t) * (2 * kBlkBytes), s_tile, 2 * kBlkBytes);
-        bulk_commit();
-      }
+      store_tile(fmt, f, s_tile, tiles1 + size_t(i >> 7) * fmt.tile_bytes());
     }
   }
-  if (tiles1 && threadIdx.x == 0) bulk_wait_all();
+  if (tiles1) store_tiles_drain();
 }
 
 cudaError_t launch_stage3(const SceneDev& sc, const float* d_ray_o, const float* d_ray_d, const int32_t* d_ray,
@@ -1003,8 +916,9 @@ cudaError_t launch_stage3(const SceneDev& sc, const float* d_ray_o, const float*
   const long long cap = 132ll * 64;
   if (d_total && blocks > cap) blocks = cap;   // grid-stride when the true count lives on the device
   static unsigned long long attr_done = 0;   // per device
-  if (set_max_dyn_smem_once(reinterpret_cast<const void*>(stage3_kernel), 2 * kBlkBytes, &attr_done) != cudaSuccess) return cudaGetLastError();
-  stage3_kernel<<<unsigned(blocks), 128, d_tiles1 ? size_t(2 * kBlkBytes) : 0, s>>>(sc, d_ray_o, d_ray_d, d_ray, d_z, d_zlut_dense, K,
+  const int tile_bytes = int(shading_tiles().tile_bytes());
+  if (set_max_dyn_smem_once(reinterpret_cast<const void*>(stage3_kernel), tile_bytes, &attr_done) != cudaSuccess) return cudaGetLastError();
+  stage3_kernel<<<unsigned(blocks), 128, d_tiles1 ? size_t(tile_bytes) : 0, s>>>(sc, d_ray_o, d_ray_d, d_ray, d_z, d_zlut_dense, K,
                                                                                       n_samples, d_total, d_x1, d_tiles1);
   return cudaGetLastError();
 }

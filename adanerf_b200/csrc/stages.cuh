@@ -27,10 +27,11 @@ struct PoseDev {
   float rot[9];
 };
 
-// Packed-tile destinations (nullptr = skip): MLP0 input tiles (hi/lo) and MLP1 input tiles.
 cudaError_t launch_gen_dirs(const CameraRays& cam, long long n_rays, float* d_dirs, cudaStream_t s);
+// Stage 0.  Any of d_x0 (fp32 features), d_ray_o / d_ray_d and d_tiles0 may be null (not written).  d_tiles0: the sampling
+// net's packed input tiles (sampling_tiles in tiles.cuh) with tile_terms terms (1 or 2).
 cudaError_t launch_stage0(const SceneDev& sc, const PoseDev& pd, const float* d_dirs, const CameraRays* cam,
-                          long long n_rays, float* d_x0, float* d_ray_o, float* d_ray_d, uint8_t* d_tiles0,
+                          long long n_rays, float* d_x0, float* d_ray_o, float* d_ray_d, uint8_t* d_tiles0, int tile_terms,
                           cudaStream_t s);
 
 // Stage 2.  tile_state: [n_ctas + 2] uint64 scratch zeroed by the launcher (memsetAsync).
@@ -58,7 +59,8 @@ cudaError_t launch_stage2_dense(long long n_rays, int K, int32_t* d_count, int32
                                 cudaStream_t s);
 
 // Stage 3.  Adaptive: sample s -> (d_ray[s], d_z[s]).  Dense (d_ray == nullptr): ray = s / K,
-// z = d_zlut_dense[s % K].  n_samples read from d_total when non-null.
+// z = d_zlut_dense[s % K].  n_samples read from d_total when non-null.  d_x1 (fp32 features) and d_tiles1 (the shading
+// net's packed input tiles, shading_tiles in tiles.cuh) may be null (not written).
 cudaError_t launch_stage3(const SceneDev& sc, const float* d_ray_o, const float* d_ray_d, const int32_t* d_ray,
                           const float* d_z, const float* d_zlut_dense, int K, long long n_samples, const long long* d_total,
                           float* d_x1, uint8_t* d_tiles1, cudaStream_t s);

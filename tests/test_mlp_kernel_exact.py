@@ -8,7 +8,7 @@
 import pytest
 import torch
 
-from conftest import load_pavillon_weights
+from conftest import case_weights, load_golden, load_pavillon_weights
 from oracle import adanerf_oracle as orc
 from oracle import mlp_emulation as me
 
@@ -153,16 +153,30 @@ def _compose(r, pose, rot, dirs, thr, K):
     return dict(rgb=out["rgb"], n_samples=s2["count"], raw0=raw0)
 
 
-@pytest.mark.parametrize("kind", ["shaped", "pav"])
+def _render_case(kind):
+    """Scene, weights, pose, rotation and (thr, K) settings of a render-equals-stages case.  "terms1": the shaped nets
+    with a plain bf16 sampling net (mlp0_terms = 1); "ndc": the golden NDC case (30-feature sampling net, ndc_rays in
+    stage 3)."""
+    if kind == "ndc":
+        g = load_golden("ndc_k16_t0.15")
+        m = g["meta"]
+        sd0, sd1 = case_weights("ndc_k16_t0.15")
+        return m["scene_params"], sd0, sd1, torch.from_numpy(g["pose"]), torch.from_numpy(g["rot"]), ((m["thr"], m["K"]),)
+    scene, sd0, sd1 = _frame_case("shaped" if kind == "terms1" else kind)
+    return scene, sd0, sd1, torch.tensor(scene["view_cell_center"]), orc.rotation_yaw(30.0), ((0.2, 8), (0.15, 16))
+
+
+@pytest.mark.parametrize("kind", ["shaped", "pav", "terms1", "ndc"])
 def test_render_equals_its_stages(kind, make_renderer):
-    """render_rays / render_camera (device row counts, all-SM grids, stage 0 writing the split tiles, stage 3 writing the
-    shading tiles or the fused encoder, chunking) == the stage entry points composed by hand, bit for bit."""
-    scene, sd0, sd1 = _frame_case(kind)
+    """render_rays / render_camera (device row counts, all-SM grids, stage 0 writing the sampling tiles, stage 3 writing
+    the shading tiles or the fused encoder, chunking) == the stage entry points composed by hand, bit for bit."""
+    scene, sd0, sd1, pose, rot, settings = _render_case(kind)
     r = make_renderer(scene, sd0, sd1)
-    pose, rot = torch.tensor(scene["view_cell_center"]), orc.rotation_yaw(30.0)
+    if kind == "terms1":
+        r.set_option("mlp0_terms", 1)
     W = H = 800
     dirs = r.generate_ray_directions(W, H)
-    for thr, K in ((0.2, 8), (0.15, 16)):
+    for thr, K in settings:
         ref = _compose(r, pose, rot, dirs, thr, K)
         for fuse in (0, 1):
             r.set_option("fuse_encoder", fuse)
