@@ -6,6 +6,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <map>
+#include <optional>
 #include <string>
 #include <vector>
 
@@ -24,17 +25,31 @@ struct HostTensor {
   int64_t rows = 0, cols = 0;
 };
 
+// Memory the context owns: grown by ensure(), freed with the context.  Device memory, or page-locked host memory.
+struct Buf {
+  enum Kind { kDevice, kPinned };
+  void* p = nullptr;
+  size_t cap = 0;
+  Kind kind;
+  explicit Buf(Kind k = kDevice) : kind(k) {}
+  Buf(const Buf&) = delete;
+  Buf& operator=(const Buf&) = delete;
+  ~Buf() { release(); }
+  cudaError_t release() {
+    const cudaError_t e = !p ? cudaSuccess : kind == kPinned ? cudaFreeHost(p) : cudaFree(p);
+    p = nullptr;
+    cap = 0;
+    return e;
+  }
+  template <class T> T* as() const { return static_cast<T*>(p); }
+};
+
 struct Net {
   bool ready = false;
   int n_in = 0, n_out = 0;
   MlpProgram prog{};
-  uint8_t* d_wblob = nullptr;
+  Buf wblob;
   std::map<std::string, HostTensor> tensors;  // kept so "mlp0_terms" can re-pack
-};
-
-struct Buf {
-  void* p = nullptr;
-  size_t cap = 0;
 };
 
 }  // namespace
@@ -44,8 +59,8 @@ struct adn_ctx {
   int num_sms = 132;
   adn_scene scene{};
   SceneDev sc{};
-  float* d_zlut = nullptr;        // [128] world depth of the cell centres (log warp)
-  float* d_zlut_dense = nullptr;  // [dense_K]
+  Buf zlut;                       // [128] world depth of the cell centres (log warp)
+  Buf zlut_dense;                 // [dense_K]
   int dense_K = 0;
   Net net[2];
   int mlp0_terms = 3;
@@ -58,14 +73,15 @@ struct adn_ctx {
   float last_thr = 0.0f;          // the last render's threshold argument
   bool prof_budget = false;       // the profiled render timed the selection with stage 2 (ev[7] -> ev[3])
   // scratch
-  Buf tiles0, raw0, ray_o, ray_d, dirs, count, offset, rayidx, zbuf, zpbuf, tiles1, raw1, s2scratch, rgb, rgba, metric;
+  Buf tiles0, raw0, ray_o, ray_d, count, offset, rayidx, zbuf, zpbuf, tiles1, raw1, s2scratch, rgba, metric;
+  Buf dirs, rgb, nsamples;        // device side of the *_host entry points
   Buf budget_keys, budget_work, budget_thr;   // sample budget: candidate keys, histograms + select state, t*
-  long long* d_total = nullptr;
-  int* d_err = nullptr;           // device view of h_err
-  int* h_err = nullptr;           // watchdog flag in mapped pinned host memory: still readable after a device trap
-  // pinned staging for the *_host entry points
+  Buf total;                      // long long: samples of the last stage 2
+  Buf watchdog{Buf::kPinned};     // int flag in mapped pinned host memory: still readable after a device trap
+  int* d_err = nullptr;           // device view of watchdog
   Stage2Sync s2sync;              // epoch / ticket base of s2scratch (no per-launch memset)
-  Buf h_in, h_out, h_ns;
+  // pinned staging for the *_host entry points
+  Buf h_in{Buf::kPinned}, h_out{Buf::kPinned}, h_ns{Buf::kPinned};
   // caller buffers page-locked in place at the caller's explicit request (adn_register_host_buffer): the *_host entry
   // points DMA straight from / to them; everything else goes through the context's pinned staging buffers
   struct Reg { const void* p = nullptr; size_t bytes = 0; };
@@ -94,23 +110,14 @@ adn_status cuda_fail(adn_ctx* ctx, cudaError_t e, const char* where) {
     if (e__ != cudaSuccess) return cuda_fail(ctx, e__, #call); \
   } while (0)
 
+// Grows b to at least `bytes` (device buffers with some slack); the old contents are not kept.
 adn_status ensure(adn_ctx* ctx, Buf& b, size_t bytes) {
   if (bytes <= b.cap) return ADN_OK;
-  if (b.p) ADN_CUDA(ctx, cudaFree(b.p));
-  b.p = nullptr;
-  b.cap = 0;
-  size_t want = bytes + bytes / 8 + 256;
-  ADN_CUDA(ctx, cudaMalloc(&b.p, want));
+  ADN_CUDA(ctx, b.release());
+  const bool pinned = b.kind == Buf::kPinned;
+  const size_t want = pinned ? bytes : bytes + bytes / 8 + 256;
+  ADN_CUDA(ctx, pinned ? cudaMallocHost(&b.p, want) : cudaMalloc(&b.p, want));
   b.cap = want;
-  return ADN_OK;
-}
-adn_status ensure_pinned(adn_ctx* ctx, Buf& b, size_t bytes) {
-  if (bytes <= b.cap) return ADN_OK;
-  if (b.p) ADN_CUDA(ctx, cudaFreeHost(b.p));
-  b.p = nullptr;
-  b.cap = 0;
-  ADN_CUDA(ctx, cudaMallocHost(&b.p, bytes));
-  b.cap = bytes;
   return ADN_OK;
 }
 
@@ -118,7 +125,7 @@ adn_status ensure_pinned(adn_ctx* ctx, Buf& b, size_t bytes) {
 // registered with adn_register_host_buffer (whose lifetime the caller vouches for), or memory the caller allocated
 // page-locked itself (cudaMallocHost / torch pin_memory).  The library never registers memory behind the caller's back:
 // a buffer that is freed and re-allocated at the same address would keep a stale registration (ADVICE r1).
-bool pin_in_place(adn_ctx* ctx, int /*slot*/, const void* p, size_t bytes) {
+bool pin_in_place(adn_ctx* ctx, const void* p, size_t bytes) {
   const char* lo = static_cast<const char*>(p);
   for (const adn_ctx::Reg& r : ctx->regs)
     if (lo >= static_cast<const char*>(r.p) && lo + bytes <= static_cast<const char*>(r.p) + r.bytes) return true;
@@ -191,10 +198,9 @@ adn_status upload(adn_ctx* ctx, Net& net, const std::vector<uint8_t>& wblob, con
   if (fblob.size() > size_t(kSideFloats)) return fail(ctx, ADN_ERR_INVALID, "network has too many fp32 side parameters");
   std::memset(net.prog.side, 0, sizeof(net.prog.side));
   std::memcpy(net.prog.side, fblob.data(), fblob.size() * 4);
-  if (net.d_wblob) cudaFree(net.d_wblob);
-  net.d_wblob = nullptr;
-  ADN_CUDA(ctx, cudaMalloc(&net.d_wblob, wblob.size()));
-  ADN_CUDA(ctx, cudaMemcpy(net.d_wblob, wblob.data(), wblob.size(), cudaMemcpyHostToDevice));
+  adn_status s = ensure(ctx, net.wblob, wblob.size());   // the callers synchronised: no kernel still reads the old blob
+  if (s != ADN_OK) return s;
+  ADN_CUDA(ctx, cudaMemcpy(net.wblob.p, wblob.data(), wblob.size(), cudaMemcpyHostToDevice));
   return ADN_OK;
 }
 
@@ -364,7 +370,7 @@ void set_ndc_projection(adn_ctx* ctx, int W, int H, float focal_in) {
 }
 
 adn_status ensure_dense_lut(adn_ctx* ctx, int K) {
-  if (ctx->dense_K == K && ctx->d_zlut_dense) return ADN_OK;
+  if (ctx->dense_K == K) return ADN_OK;
   // thr == 0 branch of FromClassifiedDepthAdaptive.generate (nerf_raymarch_common.py:708-720), fp32 steps
   std::vector<float> lut(K);
   const double max_v = double(ctx->scene.depth_range[1]) - double(ctx->scene.depth_range[0]);
@@ -377,10 +383,9 @@ adn_status ensure_dense_lut(adn_ctx* ctx, int K) {
     const float w = float(std::pow(max_v + 1.0, double(z)));
     lut[k] = ctx->scene.use_ndc ? z : (w - 1.0f) + ctx->scene.depth_range[0];   // NoDepthRange: :797-805
   }
-  if (ctx->d_zlut_dense) cudaFree(ctx->d_zlut_dense);
-  ctx->d_zlut_dense = nullptr;
-  ADN_CUDA(ctx, cudaMalloc(&ctx->d_zlut_dense, sizeof(float) * K));
-  ADN_CUDA(ctx, cudaMemcpy(ctx->d_zlut_dense, lut.data(), sizeof(float) * K, cudaMemcpyHostToDevice));
+  adn_status s = ensure(ctx, ctx->zlut_dense, sizeof(float) * K);
+  if (s != ADN_OK) return s;
+  ADN_CUDA(ctx, cudaMemcpy(ctx->zlut_dense.p, lut.data(), sizeof(float) * K, cudaMemcpyHostToDevice));
   ctx->dense_K = K;
   return ADN_OK;
 }
@@ -392,7 +397,9 @@ PoseDev make_pose(const float* pose, const float* rot) {
   return p;
 }
 
-CameraRays make_camera(const adn_ctx* ctx, int W, int H, int row0) {
+// The pinhole rays of image rows [row0, row0 + rows) of a W x H frame; none when that window does not fit the frame.
+std::optional<CameraRays> camera_rays(const adn_ctx* ctx, int W, int H, int row0, int rows) {
+  if (!ctx || W < 1 || H < 1 || row0 < 0 || rows < 0 || row0 + rows > H) return std::nullopt;
   // src/util/raygeneration.py:10-26 with focal = 0.5*W/tan(fov/2) (src/datasets.py:181-182), float64
   CameraRays c;
   const double fov = double(ctx->scene.fov);
@@ -415,37 +422,85 @@ int64_t pad128(int64_t n) { return (n + 127) / 128 * 128; }
 adn_status run_mlp(adn_ctx* ctx, int id, const uint8_t* tiles, float* out, const long long* rows_dev, long long rows,
                    cudaStream_t st, const EncodeParams* enc = nullptr) {
   Net& n = ctx->net[id];
-  const cudaError_t e = launch_mlp(n.prog, n.d_wblob, tiles, out, rows_dev, rows, ctx->d_err, ctx->num_sms, st, enc);
+  const cudaError_t e = launch_mlp(n.prog, n.wblob.as<uint8_t>(), tiles, out, rows_dev, rows, ctx->d_err, ctx->num_sms, st, enc);
   if (e != cudaSuccess) return cuda_fail(ctx, e, id == 0 ? "launch sampling MLP" : "launch shading MLP");
   ctx->stats.kernel_launches++;
   return ADN_OK;
 }
 
-enum { kStages01 = 1, kStages25 = 2 };
+// One render call: the camera pose, where the rays come from and where each output goes.  A chunk of a call is a call of
+// its own (chunk_of).
+struct RenderCall {
+  const float* pose;                // [3], host
+  const float* rot;                 // [9] row-major, host
+  const float* d_dirs = nullptr;    // the rays [n_rays, 3], or
+  std::optional<CameraRays> cam;    // image rows whose pinhole rays are generated on the device
+  int64_t n_rays;
+  float thr;
+  int K;
+  float* d_rgb = nullptr;           // [n_rays, 3]
+  uint8_t* d_rgba8 = nullptr;       // [n_rays, 4]
+  int32_t* d_nsamples = nullptr;    // [n_rays]
+  float* d_oracle_w = nullptr;      // [n_rays, 128]: the sampling net's output
+  adn_aux_outputs aux{};            // all null: none
+  cudaStream_t st;
+  RenderCall(const float* pose_, const float* rot_, int64_t n_rays_, float thr_, int K_, void* stream)
+      : pose(pose_), rot(rot_), n_rays(n_rays_), thr(thr_), K(K_), st(static_cast<cudaStream_t>(stream)) {}
+};
 
-// The hot path for one chunk of rays, stream ordered, no host synchronisation.  `parts`: kStages01 = stage 0 + sampling MLP
-// (writes the chunk's raw0 / ray_o / ray_d), kStages25 = stages 2-5 (reads them).  d_thr: stage 2's threshold as a device
-// float (sample budget), null = `thr`.
-adn_status render_chunk(adn_ctx* ctx, const PoseDev& pd, const float* d_dirs, const CameraRays* cam, int64_t n, float thr,
-                        int K, float* d_rgb, uint8_t* d_rgba8, int32_t* d_nsamples, float* raw0, float* ray_o, float* ray_d,
-                        const float* d_thr, const Stage5Aux& aux, cudaStream_t st, bool timing, int parts) {
-  const bool dense = (thr == 0.0f);
+// Rays [r0, r0 + chunk) of a call (fewer at its end): the ray source and every output start at ray r0.
+RenderCall chunk_of(const RenderCall& call, int64_t r0, int64_t chunk) {
+  RenderCall c = call;
+  c.n_rays = std::min(chunk, call.n_rays - r0);
+  if (c.d_dirs) c.d_dirs += 3 * r0;
+  if (c.cam) c.cam->row0 += int(r0 / c.cam->W);
+  if (c.d_rgb) c.d_rgb += 3 * r0;
+  if (c.d_rgba8) c.d_rgba8 += 4 * r0;
+  if (c.d_nsamples) c.d_nsamples += r0;
+  if (c.d_oracle_w) c.d_oracle_w += 128 * r0;
+  for (float** p : {&c.aux.d_weights, &c.aux.d_alpha, &c.aux.d_z_vals})
+    if (*p) *p += r0 * c.K;
+  for (float** p : {&c.aux.d_depth_map, &c.aux.d_acc_map, &c.aux.d_disp_map, &c.aux.d_depth_est})
+    if (*p) *p += r0;
+  return c;
+}
+
+// Stage 5's optional outputs: the caller's arrays and the scene's depth constants behind depth_est.
+Stage5Aux stage5_aux(const adn_ctx* ctx, const adn_aux_outputs& a) {
+  const adn_scene& sc = ctx->scene;
+  return {a.d_weights, a.d_alpha, a.d_z_vals, a.d_depth_map, a.d_acc_map, a.d_disp_map, a.d_depth_est, sc.use_ndc ? 1 : 0,
+          sc.depth_range[0], float(std::log(double(sc.depth_range[1]) - double(sc.depth_range[0]) + 1.0))};
+}
+
+// Stage 0 + the sampling MLP of one chunk, stream ordered.  Writes the chunk's raw0 [n, 128] (the caller's
+// d_oracle_weights when given, else the context's scratch from ray w on) and its ray origins / directions (scratch from ray
+// w on).  w is 0 unless a sample budget keeps the whole call's rows.  timing: record ev[0..2].
+adn_status run_stages_0_1(adn_ctx* ctx, const RenderCall& c, int64_t w, bool timing) {
+  const Net& n0 = ctx->net[0];
+  adn_status s = ensure(ctx, ctx->tiles0, size_t(pad128(c.n_rays) / 128) * n0.prog.in.tile_bytes());
+  if (s != ADN_OK) return s;
+  float* raw0 = c.d_oracle_w ? c.d_oracle_w : ctx->raw0.as<float>() + 128 * w;
+  uint8_t* tiles0 = ctx->tiles0.as<uint8_t>();
+  if (timing) cudaEventRecord(ctx->ev[0], c.st);
+  // stage 0 (writes the sampling net's packed input tiles)
+  ADN_CUDA(ctx, launch_stage0(ctx->sc, make_pose(c.pose, c.rot), c.d_dirs, c.cam ? &*c.cam : nullptr, c.n_rays, nullptr,
+                              ctx->ray_o.as<float>() + 3 * w, ctx->ray_d.as<float>() + 3 * w, tiles0, n0.prog.in.n_terms, c.st));
+  ctx->stats.kernel_launches++;
+  if (timing) cudaEventRecord(ctx->ev[1], c.st);
+  // stage 1
+  if ((s = run_mlp(ctx, 0, tiles0, raw0, nullptr, c.n_rays, c.st)) != ADN_OK) return s;
+  if (timing) cudaEventRecord(ctx->ev[2], c.st);
+  return ADN_OK;
+}
+
+// Stages 2-5 of one chunk, stream ordered: read what run_stages_0_1 wrote for the same chunk and w.  d_thr: stage 2's
+// threshold as a device float (sample budget), null = c.thr.  timing: record ev[3..6].
+adn_status run_stages_2_5(adn_ctx* ctx, const RenderCall& c, int64_t w, const float* d_thr, bool timing) {
+  const int64_t n = c.n_rays;
+  const int K = c.K;
+  const bool dense = (c.thr == 0.0f);
   const int64_t cap = n * K;
   adn_status s;
-  Net& n0 = ctx->net[0];
-  if (parts & kStages01) {
-    if ((s = ensure(ctx, ctx->tiles0, size_t(pad128(n) / 128) * n0.prog.in.tile_bytes())) != ADN_OK) return s;
-    uint8_t* tiles0 = static_cast<uint8_t*>(ctx->tiles0.p);
-    if (timing) cudaEventRecord(ctx->ev[0], st);
-    // stage 0 (writes the sampling net's packed input tiles)
-    ADN_CUDA(ctx, launch_stage0(ctx->sc, pd, d_dirs, cam, n, nullptr, ray_o, ray_d, tiles0, n0.prog.in.n_terms, st));
-    ctx->stats.kernel_launches++;
-    if (timing) cudaEventRecord(ctx->ev[1], st);
-    // stage 1
-    if ((s = run_mlp(ctx, 0, tiles0, raw0, nullptr, n, st)) != ADN_OK) return s;
-    if (timing) cudaEventRecord(ctx->ev[2], st);
-  }
-  if (!(parts & kStages25)) return ADN_OK;
   if ((s = ensure(ctx, ctx->count, size_t(n) * 4)) != ADN_OK) return s;
   if ((s = ensure(ctx, ctx->offset, size_t(n) * 4)) != ADN_OK) return s;
   if (!dense) {
@@ -459,52 +514,53 @@ adn_status render_chunk(adn_ctx* ctx, const PoseDev& pd, const float* d_dirs, co
   if (!fused_enc && (s = ensure(ctx, ctx->tiles1, size_t(pad128(cap) / 128) * ctx->net[1].prog.in.tile_bytes())) != ADN_OK) return s;
   if ((s = ensure(ctx, ctx->raw1, size_t(pad128(cap)) * 16)) != ADN_OK) return s;
 
-  int32_t* count = d_nsamples ? d_nsamples : static_cast<int32_t*>(ctx->count.p);
-  int32_t* offset = static_cast<int32_t*>(ctx->offset.p);
-  uint8_t* tiles1 = static_cast<uint8_t*>(ctx->tiles1.p);   // null / stale when the encoder is fused
-  float* raw1 = static_cast<float*>(ctx->raw1.p);
+  float* raw0 = c.d_oracle_w ? c.d_oracle_w : ctx->raw0.as<float>() + 128 * w;
+  const float* ray_o = ctx->ray_o.as<float>() + 3 * w;
+  const float* ray_d = ctx->ray_d.as<float>() + 3 * w;
+  int32_t* count = c.d_nsamples ? c.d_nsamples : ctx->count.as<int32_t>();
+  int32_t* offset = ctx->offset.as<int32_t>();
+  int32_t* rayidx = dense ? nullptr : ctx->rayidx.as<int32_t>();
+  float* z = ctx->zbuf.as<float>();
+  uint8_t* tiles1 = ctx->tiles1.as<uint8_t>();   // null / stale when the encoder is fused
+  float* raw1 = ctx->raw1.as<float>();
+  long long* total = ctx->total.as<long long>();
 
   // stage 2
   if (dense) {
-    ADN_CUDA(ctx, launch_stage2_dense(n, K, count, offset, ctx->d_total, st));
+    ADN_CUDA(ctx, launch_stage2_dense(n, K, count, offset, total, c.st));
   } else {
-    ADN_CUDA(ctx, launch_stage2(raw0, n, thr, K, ctx->d_zlut, count, offset, nullptr, static_cast<int32_t*>(ctx->rayidx.p),
-                                static_cast<float*>(ctx->zbuf.p), static_cast<float*>(ctx->zpbuf.p), ctx->d_total,
-                                ctx->s2scratch.p, &ctx->s2sync, st, d_thr));
+    ADN_CUDA(ctx, launch_stage2(raw0, n, c.thr, K, ctx->zlut.as<float>(), count, offset, nullptr, rayidx, z,
+                                ctx->zpbuf.as<float>(), total, ctx->s2scratch.p, &ctx->s2sync, c.st, d_thr));
   }
   ctx->stats.kernel_launches++;
-  if (timing) cudaEventRecord(ctx->ev[3], st);
+  if (timing) cudaEventRecord(ctx->ev[3], c.st);
   // stage 3 (+ 4)
-  EncodeParams ep;
-  if (fused_enc) {
-    ep.ray_o = ray_o;
-    ep.ray_d = ray_d;
-    ep.ray_idx = dense ? nullptr : static_cast<int32_t*>(ctx->rayidx.p);
-    ep.z = static_cast<float*>(ctx->zbuf.p);
-    ep.zlut_dense = ctx->d_zlut_dense;
-    ep.K = K;
-    ep.sc = ctx->sc;
-  } else {
-    ADN_CUDA(ctx, launch_stage3(ctx->sc, ray_o, ray_d, dense ? nullptr : static_cast<int32_t*>(ctx->rayidx.p),
-                                static_cast<float*>(ctx->zbuf.p), ctx->d_zlut_dense, K, cap, ctx->d_total, nullptr, tiles1, st));
+  const EncodeParams ep{ray_o, ray_d, rayidx, z, ctx->zlut_dense.as<float>(), K, ctx->sc};   // read when fused_enc
+  if (!fused_enc) {
+    ADN_CUDA(ctx, launch_stage3(ctx->sc, ray_o, ray_d, rayidx, z, ctx->zlut_dense.as<float>(), K, cap, total, nullptr, tiles1,
+                                ctx->num_sms, c.st));
     ctx->stats.kernel_launches++;
   }
-  if (timing) cudaEventRecord(ctx->ev[4], st);
+  if (timing) cudaEventRecord(ctx->ev[4], c.st);
   // stage 4
-  if ((s = run_mlp(ctx, 1, fused_enc ? nullptr : tiles1, raw1, ctx->d_total, cap, st, fused_enc ? &ep : nullptr)) != ADN_OK) return s;
-  if (timing) cudaEventRecord(ctx->ev[5], st);
+  if ((s = run_mlp(ctx, 1, fused_enc ? nullptr : tiles1, raw1, total, cap, c.st, fused_enc ? &ep : nullptr)) != ADN_OK) return s;
+  if (timing) cudaEventRecord(ctx->ev[5], c.st);
   // stage 5
-  ADN_CUDA(ctx, launch_stage5(raw1, dense ? raw0 : static_cast<float*>(ctx->zpbuf.p), static_cast<float*>(ctx->zbuf.p),
-                              ctx->d_zlut_dense, offset, count, n, K, dense ? 1 : 0, d_rgb, d_rgba8, aux, st));
+  ADN_CUDA(ctx, launch_stage5(raw1, dense ? raw0 : ctx->zpbuf.as<float>(), z, ctx->zlut_dense.as<float>(), offset, count, n, K,
+                              dense ? 1 : 0, c.d_rgb, c.d_rgba8, stage5_aux(ctx, c.aux), c.st));
   ctx->stats.kernel_launches++;
-  if (timing) cudaEventRecord(ctx->ev[6], st);
+  if (timing) cudaEventRecord(ctx->ev[6], c.st);
   return ADN_OK;
 }
 
-adn_status render_impl(adn_ctx* ctx, const float* pose, const float* rot, const float* d_dirs, const CameraRays* cam,
-                       int64_t n_rays, float thr, int K, float* d_rgb, uint8_t* d_rgba8, int32_t* d_nsamples,
-                       float* d_oracle_w, cudaStream_t st, const adn_aux_outputs* ax = nullptr) {
-  if (!ctx || !pose || !rot || n_rays < 0 || (!d_rgb && !d_rgba8)) return fail(ctx, ADN_ERR_INVALID, "render: bad arguments");
+// The hot path for every render entry point: stream ordered, no host synchronisation.  The call runs in chunks of rays;
+// with a sample budget, stages 0-1 of every chunk, then one threshold for the whole call, then stages 2-5 of every chunk.
+adn_status render(adn_ctx* ctx, const RenderCall& call) {
+  const int64_t n_rays = call.n_rays;
+  const float thr = call.thr;
+  const int K = call.K;
+  if (!ctx || !call.pose || !call.rot || n_rays < 0 || (!call.d_rgb && !call.d_rgba8))
+    return fail(ctx, ADN_ERR_INVALID, "render: bad arguments");
   if (!ctx->net[0].ready || !ctx->net[1].ready) return fail(ctx, ADN_ERR_NO_WEIGHTS, "render: set both networks first");
   if (ctx->net[0].n_in != ctx->n_feat0 || ctx->net[0].n_out != 128)
     return fail(ctx, ADN_ERR_INVALID, "render: sampling net must be " + std::to_string(ctx->n_feat0) + " -> 128 for this scene's encoding");
@@ -518,12 +574,12 @@ adn_status render_impl(adn_ctx* ctx, const float* pose, const float* rot, const 
                                           " rays of the call (every ray keeps at least one sample)");
   if (budget > 0 && n_rays * (K - 1) >= (int64_t(1) << 32))
     return fail(ctx, ADN_ERR_INVALID, "render: sample_budget supports at most 2^32 - 1 candidate samples (N * (K - 1)) per call");
-  if (budget > 0 && (reinterpret_cast<uintptr_t>(d_oracle_w) & 15u))
+  if (budget > 0 && (reinterpret_cast<uintptr_t>(call.d_oracle_w) & 15u))
     return fail(ctx, ADN_ERR_INVALID, "render: sample_budget needs 16-byte aligned d_oracle_weights rows");
   if (n_rays == 0) return ADN_OK;
   if (ctx->scene.use_ndc) {
     // image size behind ndc_rays: the frame being rendered (viewer, featureset.cpp:83-84) or the dataset's (features.py:350-351,430)
-    if (cam) set_ndc_projection(ctx, cam->W, cam->H, 0.0f);
+    if (call.cam) set_ndc_projection(ctx, call.cam->W, call.cam->H, 0.0f);
     else if (ctx->scene.ndc_w > 0 && ctx->scene.ndc_h > 0) set_ndc_projection(ctx, ctx->scene.ndc_w, ctx->scene.ndc_h, ctx->scene.ndc_focal);
     else return fail(ctx, ADN_ERR_INVALID, "render: NDC scene needs ndc_w / ndc_h when rays are passed explicitly");
   }
@@ -536,8 +592,7 @@ adn_status render_impl(adn_ctx* ctx, const float* pose, const float* rot, const 
     if (chunk < 8192) chunk = 8192;
   }
   chunk = pad128(chunk);
-  if (cam && chunk % cam->W) chunk = (chunk / cam->W + 1) * cam->W;  // whole rows per chunk
-  const PoseDev pd = make_pose(pose, rot);
+  if (call.cam && chunk % call.cam->W) chunk = (chunk / call.cam->W + 1) * call.cam->W;  // whole rows per chunk
   ctx->stats.n_rays = n_rays;
   ctx->last_budget = budget > 0;
   ctx->last_thr = thr;
@@ -545,67 +600,79 @@ adn_status render_impl(adn_ctx* ctx, const float* pose, const float* rot, const 
   // raw0 / ray_o / ray_d: one chunk's worth, or with a sample budget the whole call's (the threshold is chosen over all of
   // raw0 before any chunk runs stage 2)
   const int64_t span = budget > 0 ? n_rays : std::min(chunk, n_rays);
-  if (!d_oracle_w && (s = ensure(ctx, ctx->raw0, size_t(span) * 128 * 4)) != ADN_OK) return s;
+  if (!call.d_oracle_w && (s = ensure(ctx, ctx->raw0, size_t(span) * 128 * 4)) != ADN_OK) return s;
   if ((s = ensure(ctx, ctx->ray_o, size_t(span) * 12)) != ADN_OK) return s;
   if ((s = ensure(ctx, ctx->ray_d, size_t(span) * 12)) != ADN_OK) return s;
-  float* raw0 = d_oracle_w ? d_oracle_w : static_cast<float*>(ctx->raw0.p);
-  float* ray_o = static_cast<float*>(ctx->ray_o.p);
-  float* ray_d = static_cast<float*>(ctx->ray_d.p);
-  auto run = [&](int64_t r0, int parts, const float* d_thr) -> adn_status {
-    const int64_t n = std::min(chunk, n_rays - r0);
-    const int64_t w = budget > 0 ? r0 : 0;   // window of raw0 / ray_o / ray_d
-    CameraRays c{};
-    if (cam) {
-      c = *cam;
-      c.row0 = cam->row0 + int(r0 / cam->W);
-    }
-    Stage5Aux aux;
-    if (ax) {   // this chunk's window of the caller's per-ray / per-slot buffers
-      aux.weights = ax->d_weights ? ax->d_weights + r0 * K : nullptr;
-      aux.alpha = ax->d_alpha ? ax->d_alpha + r0 * K : nullptr;
-      aux.z_vals = ax->d_z_vals ? ax->d_z_vals + r0 * K : nullptr;
-      aux.depth_map = ax->d_depth_map ? ax->d_depth_map + r0 : nullptr;
-      aux.acc_map = ax->d_acc_map ? ax->d_acc_map + r0 : nullptr;
-      aux.disp_map = ax->d_disp_map ? ax->d_disp_map + r0 : nullptr;
-      aux.depth_est = ax->d_depth_est ? ax->d_depth_est + r0 : nullptr;
-      aux.linear_depth = ctx->scene.use_ndc ? 1 : 0;
-      aux.dr_min = ctx->scene.depth_range[0];
-      aux.log_range = float(std::log(double(ctx->scene.depth_range[1]) - double(ctx->scene.depth_range[0]) + 1.0));
-    }
-    return render_chunk(ctx, pd, d_dirs ? d_dirs + 3 * r0 : nullptr, cam ? &c : nullptr, n, thr, K, d_rgb ? d_rgb + 3 * r0 : nullptr,
-                        d_rgba8 ? d_rgba8 + 4 * r0 : nullptr, d_nsamples ? d_nsamples + r0 : nullptr,
-                        d_oracle_w ? d_oracle_w + 128 * r0 : raw0 + 128 * w, ray_o + 3 * w, ray_d + 3 * w, d_thr, aux, st,
-                        ctx->profile && r0 == 0, parts);
-  };
   if (budget == 0) {
-    for (int64_t r0 = 0; r0 < n_rays; r0 += chunk)
-      if ((s = run(r0, kStages01 | kStages25, nullptr)) != ADN_OK) return s;
+    for (int64_t r0 = 0; r0 < n_rays; r0 += chunk) {
+      const RenderCall c = chunk_of(call, r0, chunk);
+      const bool timing = ctx->profile && r0 == 0;
+      if ((s = run_stages_0_1(ctx, c, 0, timing)) != ADN_OK || (s = run_stages_2_5(ctx, c, 0, nullptr, timing)) != ADN_OK) return s;
+    }
     return ADN_OK;
   }
-  // sample budget: stages 0-1 of every chunk, one threshold for the call, stages 2-5 of every chunk
   if ((s = ensure(ctx, ctx->budget_keys, size_t(std::max<int64_t>(1, n_rays * (K - 1))) * 4)) != ADN_OK) return s;
   if ((s = ensure(ctx, ctx->budget_work, budget_work_bytes())) != ADN_OK) return s;
   if ((s = ensure(ctx, ctx->budget_thr, sizeof(float))) != ADN_OK) return s;
-  float* d_thr = static_cast<float*>(ctx->budget_thr.p);
+  float* d_thr = ctx->budget_thr.as<float>();
   for (int64_t r0 = 0; r0 < n_rays; r0 += chunk)
-    if ((s = run(r0, kStages01, nullptr)) != ADN_OK) return s;
-  if (ctx->profile) cudaEventRecord(ctx->ev[7], st);   // the selection is timed with stage 2 of the first chunk
+    if ((s = run_stages_0_1(ctx, chunk_of(call, r0, chunk), r0, ctx->profile && r0 == 0)) != ADN_OK) return s;
+  if (ctx->profile) cudaEventRecord(ctx->ev[7], call.st);   // the selection is timed with stage 2 of the first chunk
   int launches = 0;
-  ADN_CUDA(ctx, launch_budget_threshold(raw0, n_rays, thr, K, budget, static_cast<uint32_t*>(ctx->budget_keys.p), ctx->budget_work.p,
-                                        d_thr, ctx->num_sms, st, &launches));
+  ADN_CUDA(ctx, launch_budget_threshold(call.d_oracle_w ? call.d_oracle_w : ctx->raw0.as<float>(), n_rays, thr, K, budget,
+                                        ctx->budget_keys.as<uint32_t>(), ctx->budget_work.p, d_thr, ctx->num_sms, call.st, &launches));
   ctx->stats.kernel_launches += launches;
   for (int64_t r0 = 0; r0 < n_rays; r0 += chunk)
-    if ((s = run(r0, kStages25, d_thr)) != ADN_OK) return s;
+    if ((s = run_stages_2_5(ctx, chunk_of(call, r0, chunk), r0, d_thr, ctx->profile && r0 == 0)) != ADN_OK) return s;
   return ADN_OK;
 }
 
 adn_status check_device_error(adn_ctx* ctx) {
   int err = 0;
   cudaError_t e = cudaDeviceSynchronize();
-  err = *reinterpret_cast<volatile int*>(ctx->h_err);
+  err = *ctx->watchdog.as<volatile int>();
   if (e != cudaSuccess && !err) return cuda_fail(ctx, e, "device synchronize");
   if (err) return fail(ctx, ADN_ERR_KERNEL, "device watchdog: mbarrier wait timed out at site " + std::to_string(err & 0xfff));
   return ADN_OK;
+}
+
+// Enqueues the copy of `bytes` from device memory d to the caller's host array h: straight into h when pin_in_place allows,
+// otherwise into the pinned staging buffer `stage`, from which the caller copies on once the stream has synchronised
+// (*staged).
+adn_status copy_out(adn_ctx* ctx, void* h, const void* d, size_t bytes, Buf& stage, cudaStream_t st, bool* staged) {
+  adn_status s;
+  *staged = !pin_in_place(ctx, h, bytes);
+  if (*staged && (s = ensure(ctx, stage, bytes)) != ADN_OK) return s;
+  ADN_CUDA(ctx, cudaMemcpyAsync(*staged ? stage.p : h, d, bytes, cudaMemcpyDeviceToHost, st));
+  return ADN_OK;
+}
+
+// The *_host entry points: the rays are copied in from h_dirs when given (else generated from c.cam), rendered on the
+// context's stream, and rgb / n_samples copied out to the caller's arrays.  Returns once they have landed.
+adn_status render_host(adn_ctx* ctx, RenderCall c, const float* h_dirs, float* h_rgb, int32_t* h_nsamples) {
+  const size_t n = size_t(c.n_rays);
+  ADN_CUDA(ctx, cudaSetDevice(ctx->device));
+  adn_status s;
+  c.st = ctx->own_stream;
+  if (h_dirs) {
+    const bool staged = !pin_in_place(ctx, h_dirs, n * 12);
+    if ((s = ensure(ctx, ctx->dirs, n * 12)) != ADN_OK || (staged && (s = ensure(ctx, ctx->h_in, n * 12)) != ADN_OK)) return s;
+    if (staged) std::memcpy(ctx->h_in.p, h_dirs, n * 12);
+    ADN_CUDA(ctx, cudaMemcpyAsync(ctx->dirs.p, staged ? ctx->h_in.p : h_dirs, n * 12, cudaMemcpyHostToDevice, c.st));
+    c.d_dirs = ctx->dirs.as<float>();
+  }
+  if ((s = ensure(ctx, ctx->rgb, n * 12)) != ADN_OK) return s;
+  if (h_nsamples && (s = ensure(ctx, ctx->nsamples, n * 4)) != ADN_OK) return s;
+  c.d_rgb = ctx->rgb.as<float>();
+  c.d_nsamples = h_nsamples ? ctx->nsamples.as<int32_t>() : nullptr;
+  if ((s = render(ctx, c)) != ADN_OK) return s;
+  bool rgb_staged = false, ns_staged = false;
+  if ((s = copy_out(ctx, h_rgb, c.d_rgb, n * 12, ctx->h_out, c.st, &rgb_staged)) != ADN_OK) return s;
+  if (h_nsamples && (s = copy_out(ctx, h_nsamples, c.d_nsamples, n * 4, ctx->h_ns, c.st, &ns_staged)) != ADN_OK) return s;
+  ADN_CUDA(ctx, cudaStreamSynchronize(c.st));
+  if (rgb_staged) std::memcpy(h_rgb, ctx->h_out.p, n * 12);
+  if (ns_staged) std::memcpy(h_nsamples, ctx->h_ns.p, n * 4);
+  return check_device_error(ctx);
 }
 
 }  // namespace
@@ -666,12 +733,12 @@ adn_status adn_create(adn_ctx** out, const adn_scene* scene, int device) {
     // FromClassifiedDepthAdaptiveNoDepthRange (NDC configs): the cell centre itself (nerf_raymarch_common.py:826-833)
     lut[i] = scene->use_ndc ? z : (w - 1.0f) + scene->depth_range[0];
   }
-  bool ok = cudaMalloc(&ctx->d_zlut, sizeof(lut)) == cudaSuccess &&
-            cudaMemcpy(ctx->d_zlut, lut, sizeof(lut), cudaMemcpyHostToDevice) == cudaSuccess &&
-            cudaMalloc(&ctx->d_total, sizeof(long long)) == cudaSuccess &&
-            cudaMemset(ctx->d_total, 0, sizeof(long long)) == cudaSuccess &&
-            cudaHostAlloc(&ctx->h_err, sizeof(int), cudaHostAllocMapped) == cudaSuccess &&
-            cudaHostGetDevicePointer(&ctx->d_err, ctx->h_err, 0) == cudaSuccess && (*ctx->h_err = 0, true) &&
+  bool ok = ensure(ctx, ctx->zlut, sizeof(lut)) == ADN_OK &&
+            cudaMemcpy(ctx->zlut.p, lut, sizeof(lut), cudaMemcpyHostToDevice) == cudaSuccess &&
+            ensure(ctx, ctx->total, sizeof(long long)) == ADN_OK &&
+            cudaMemset(ctx->total.p, 0, sizeof(long long)) == cudaSuccess &&
+            cudaHostAlloc(&ctx->watchdog.p, sizeof(int), cudaHostAllocMapped) == cudaSuccess &&
+            cudaHostGetDevicePointer(&ctx->d_err, ctx->watchdog.p, 0) == cudaSuccess && (*ctx->watchdog.as<int>() = 0, true) &&
             cudaStreamCreateWithFlags(&ctx->own_stream, cudaStreamNonBlocking) == cudaSuccess;
   for (int i = 0; ok && i < 8; ++i) ok = cudaEventCreate(&ctx->ev[i]) == cudaSuccess;
   if (!ok) {
@@ -686,27 +753,12 @@ void adn_destroy(adn_ctx* ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
   cudaDeviceSynchronize();
-  Buf* bufs[] = {&ctx->tiles0, &ctx->raw0,  &ctx->ray_o,  &ctx->ray_d, &ctx->dirs,      &ctx->count, &ctx->offset,
-                 &ctx->rayidx, &ctx->zbuf,  &ctx->zpbuf,  &ctx->tiles1, &ctx->raw1,  &ctx->s2scratch, &ctx->rgb,   &ctx->rgba, &ctx->metric,
-                 &ctx->budget_keys, &ctx->budget_work, &ctx->budget_thr};
-  for (Buf* b : bufs)
-    if (b->p) cudaFree(b->p);
   for (auto& r : ctx->regs)
     if (r.p) cudaHostUnregister(const_cast<void*>(r.p));
-  Buf* pinned[] = {&ctx->h_in, &ctx->h_out, &ctx->h_ns};
-  for (Buf* b : pinned)
-    if (b->p) cudaFreeHost(b->p);
-  for (int i = 0; i < 2; ++i) {
-    if (ctx->net[i].d_wblob) cudaFree(ctx->net[i].d_wblob);
-  }
-  if (ctx->d_zlut) cudaFree(ctx->d_zlut);
-  if (ctx->d_zlut_dense) cudaFree(ctx->d_zlut_dense);
-  if (ctx->d_total) cudaFree(ctx->d_total);
-  if (ctx->h_err) cudaFreeHost(ctx->h_err);
   for (int i = 0; i < 8; ++i)
     if (ctx->ev[i]) cudaEventDestroy(ctx->ev[i]);
   if (ctx->own_stream) cudaStreamDestroy(ctx->own_stream);
-  delete ctx;
+  delete ctx;   // frees every Buf on this device
 }
 
 adn_status adn_set_weights(adn_ctx* ctx, int net_id, const adn_tensor_desc* tensors, int n_tensors) {
@@ -770,7 +822,7 @@ adn_status adn_get_stats(adn_ctx* ctx, adn_stats* out) {
   adn_status s = check_device_error(ctx);   // synchronises; reports a tripped device watchdog with its site
   if (s != ADN_OK) return s;
   long long total = 0;
-  ADN_CUDA(ctx, cudaMemcpy(&total, ctx->d_total, sizeof(total), cudaMemcpyDeviceToHost));
+  ADN_CUDA(ctx, cudaMemcpy(&total, ctx->total.p, sizeof(total), cudaMemcpyDeviceToHost));
   ctx->stats.n_samples = total;
   if (ctx->profile) {
     for (int i = 0; i < 6; ++i) {
@@ -798,8 +850,7 @@ adn_status adn_render_rays(adn_ctx* ctx, const float* pose, const float* rot, co
                            int K, float* d_rgb, int32_t* d_nsamples, float* d_oracle_weights, void* stream) {
   if (ctx && n_rays == 0) return ADN_OK;   // empty batch: nothing to read or write
   if (!d_dirs) return fail(ctx, ADN_ERR_INVALID, "render_rays: d_dirs is null");
-  return render_impl(ctx, pose, rot, d_dirs, nullptr, n_rays, thr, K, d_rgb, nullptr, d_nsamples, d_oracle_weights,
-                     static_cast<cudaStream_t>(stream));
+  return adn_render_rays_aux(ctx, pose, rot, d_dirs, n_rays, thr, K, d_rgb, d_nsamples, d_oracle_weights, nullptr, stream);
 }
 
 adn_status adn_render_rays_aux(adn_ctx* ctx, const float* pose, const float* rot, const float* d_dirs, int64_t n_rays, float thr,
@@ -807,38 +858,45 @@ adn_status adn_render_rays_aux(adn_ctx* ctx, const float* pose, const float* rot
                                void* stream) {
   if (ctx && n_rays == 0) return ADN_OK;
   if (!d_dirs) return fail(ctx, ADN_ERR_INVALID, "render_rays_aux: d_dirs is null");
-  return render_impl(ctx, pose, rot, d_dirs, nullptr, n_rays, thr, K, d_rgb, nullptr, d_nsamples, d_oracle_weights,
-                     static_cast<cudaStream_t>(stream), aux);
+  RenderCall c(pose, rot, n_rays, thr, K, stream);
+  c.d_dirs = d_dirs;
+  c.d_rgb = d_rgb;
+  c.d_nsamples = d_nsamples;
+  c.d_oracle_w = d_oracle_weights;
+  if (aux) c.aux = *aux;
+  return render(ctx, c);
 }
 
 adn_status adn_render_camera(adn_ctx* ctx, const float* pose, const float* rot, int W, int H, int row0, int rows, float thr,
                              int K, float* d_rgb, int32_t* d_nsamples, void* stream) {
-  if (!ctx || W < 1 || H < 1 || row0 < 0 || rows < 0 || row0 + rows > H) return fail(ctx, ADN_ERR_INVALID, "render_camera: bad image window");
-  const CameraRays cam = make_camera(ctx, W, H, row0);
-  return render_impl(ctx, pose, rot, nullptr, &cam, int64_t(rows) * W, thr, K, d_rgb, nullptr, d_nsamples, nullptr,
-                     static_cast<cudaStream_t>(stream));
+  RenderCall c(pose, rot, int64_t(rows) * W, thr, K, stream);
+  c.cam = camera_rays(ctx, W, H, row0, rows);
+  if (!c.cam) return fail(ctx, ADN_ERR_INVALID, "render_camera: bad image window");
+  c.d_rgb = d_rgb;
+  c.d_nsamples = d_nsamples;
+  return render(ctx, c);
 }
 
 adn_status adn_render_camera_rgba8(adn_ctx* ctx, const float* pose, const float* rot, int W, int H, int row0, int rows,
                                    float thr, int K, uint8_t* d_rgba8, void* stream) {
-  if (!ctx || W < 1 || H < 1 || row0 < 0 || rows < 0 || row0 + rows > H) return fail(ctx, ADN_ERR_INVALID, "render_camera: bad image window");
-  const CameraRays cam = make_camera(ctx, W, H, row0);
-  return render_impl(ctx, pose, rot, nullptr, &cam, int64_t(rows) * W, thr, K, nullptr, d_rgba8, nullptr, nullptr,
-                     static_cast<cudaStream_t>(stream));
+  RenderCall c(pose, rot, int64_t(rows) * W, thr, K, stream);
+  c.cam = camera_rays(ctx, W, H, row0, rows);
+  if (!c.cam) return fail(ctx, ADN_ERR_INVALID, "render_camera: bad image window");
+  c.d_rgba8 = d_rgba8;
+  return render(ctx, c);
 }
 
 adn_status adn_render_camera_surface(adn_ctx* ctx, const float* pose, const float* rot, int W, int H, int row0, int rows,
                                      float thr, int K, unsigned long long surface, void* stream) {
-  if (!ctx || W < 1 || H < 1 || row0 < 0 || rows < 0 || row0 + rows > H || !surface)
-    return fail(ctx, ADN_ERR_INVALID, "render_camera_surface: bad image window / surface");
+  RenderCall c(pose, rot, int64_t(rows) * W, thr, K, stream);
+  c.cam = camera_rays(ctx, W, H, row0, rows);
+  if (!c.cam || !surface) return fail(ctx, ADN_ERR_INVALID, "render_camera_surface: bad image window / surface");
   ADN_CUDA(ctx, cudaSetDevice(ctx->device));
   adn_status s = ensure(ctx, ctx->rgba, size_t(rows) * W * 4);
   if (s != ADN_OK) return s;
-  uint8_t* px = static_cast<uint8_t*>(ctx->rgba.p);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  s = adn_render_camera_rgba8(ctx, pose, rot, W, H, row0, rows, thr, K, px, stream);
-  if (s != ADN_OK) return s;
-  ADN_CUDA(ctx, launch_rgba_to_surface(px, W, row0, rows, surface, st));
+  c.d_rgba8 = ctx->rgba.as<uint8_t>();
+  if ((s = render(ctx, c)) != ADN_OK) return s;
+  ADN_CUDA(ctx, launch_rgba_to_surface(c.d_rgba8, W, row0, rows, surface, c.st));
   ctx->stats.kernel_launches++;
   return ADN_OK;
 }
@@ -878,81 +936,24 @@ adn_status adn_render_rays_host(adn_ctx* ctx, const float* pose, const float* ro
                                 float thr, int K, float* h_rgb, int32_t* h_nsamples) {
   if (!ctx || !h_dirs || !h_rgb || n_rays < 0) return fail(ctx, ADN_ERR_INVALID, "render_rays_host: bad arguments");
   if (n_rays == 0) return ADN_OK;
-  ADN_CUDA(ctx, cudaSetDevice(ctx->device));
-  adn_status s;
-  if ((s = ensure(ctx, ctx->dirs, size_t(n_rays) * 12)) != ADN_OK) return s;
-  if ((s = ensure(ctx, ctx->rgb, size_t(n_rays) * 12)) != ADN_OK) return s;
-  if ((s = ensure(ctx, ctx->count, size_t(n_rays) * 4)) != ADN_OK) return s;
-  if ((s = ensure_pinned(ctx, ctx->h_in, size_t(n_rays) * 12)) != ADN_OK) return s;
-  if ((s = ensure_pinned(ctx, ctx->h_out, size_t(n_rays) * 12)) != ADN_OK) return s;
-  if (h_nsamples && (s = ensure_pinned(ctx, ctx->h_ns, size_t(n_rays) * 4)) != ADN_OK) return s;
-  cudaStream_t st = ctx->own_stream;
-  const bool in_pinned = pin_in_place(ctx, 0, h_dirs, size_t(n_rays) * 12);
-  const bool out_pinned = pin_in_place(ctx, 1, h_rgb, size_t(n_rays) * 12);
-  const bool ns_pinned = h_nsamples && pin_in_place(ctx, 2, h_nsamples, size_t(n_rays) * 4);
-  const void* src = h_dirs;
-  if (!in_pinned) {
-    std::memcpy(ctx->h_in.p, h_dirs, size_t(n_rays) * 12);
-    src = ctx->h_in.p;
-  }
-  ADN_CUDA(ctx, cudaMemcpyAsync(ctx->dirs.p, src, size_t(n_rays) * 12, cudaMemcpyHostToDevice, st));
-  int32_t* d_ns = nullptr;
-  if (h_nsamples) {
-    if ((s = ensure(ctx, ctx->rgba, size_t(n_rays) * 4)) != ADN_OK) return s;
-    d_ns = static_cast<int32_t*>(ctx->rgba.p);
-  }
-  s = render_impl(ctx, pose, rot, static_cast<float*>(ctx->dirs.p), nullptr, n_rays, thr, K, static_cast<float*>(ctx->rgb.p),
-                  nullptr, d_ns, nullptr, st);
-  if (s != ADN_OK) return s;
-  ADN_CUDA(ctx, cudaMemcpyAsync(out_pinned ? static_cast<void*>(h_rgb) : ctx->h_out.p, ctx->rgb.p, size_t(n_rays) * 12,
-                                cudaMemcpyDeviceToHost, st));
-  if (h_nsamples)
-    ADN_CUDA(ctx, cudaMemcpyAsync(ns_pinned ? static_cast<void*>(h_nsamples) : ctx->h_ns.p, d_ns, size_t(n_rays) * 4,
-                                  cudaMemcpyDeviceToHost, st));
-  ADN_CUDA(ctx, cudaStreamSynchronize(st));
-  if (!out_pinned) std::memcpy(h_rgb, ctx->h_out.p, size_t(n_rays) * 12);
-  if (h_nsamples && !ns_pinned) std::memcpy(h_nsamples, ctx->h_ns.p, size_t(n_rays) * 4);
-  return check_device_error(ctx);
+  return render_host(ctx, RenderCall(pose, rot, n_rays, thr, K, nullptr), h_dirs, h_rgb, h_nsamples);
 }
 
 adn_status adn_render_camera_host(adn_ctx* ctx, const float* pose, const float* rot, int W, int H, int row0, int rows,
                                   float thr, int K, float* h_rgb, int32_t* h_nsamples) {
-  if (!ctx || !h_rgb || W < 1 || H < 1 || row0 < 0 || rows < 0 || row0 + rows > H) return fail(ctx, ADN_ERR_INVALID, "render_camera_host: bad arguments");
-  const int64_t n_rays = int64_t(rows) * W;
-  if (n_rays == 0) return ADN_OK;
-  ADN_CUDA(ctx, cudaSetDevice(ctx->device));
-  adn_status s;
-  if ((s = ensure(ctx, ctx->rgb, size_t(n_rays) * 12)) != ADN_OK) return s;
-  if ((s = ensure_pinned(ctx, ctx->h_out, size_t(n_rays) * 12)) != ADN_OK) return s;
-  int32_t* d_ns = nullptr;
-  if (h_nsamples) {
-    if ((s = ensure(ctx, ctx->rgba, size_t(n_rays) * 4)) != ADN_OK) return s;
-    if ((s = ensure_pinned(ctx, ctx->h_ns, size_t(n_rays) * 4)) != ADN_OK) return s;
-    d_ns = static_cast<int32_t*>(ctx->rgba.p);
-  }
-  cudaStream_t st = ctx->own_stream;
-  const bool out_pinned = pin_in_place(ctx, 1, h_rgb, size_t(n_rays) * 12);
-  const bool ns_pinned = h_nsamples && pin_in_place(ctx, 2, h_nsamples, size_t(n_rays) * 4);
-  const CameraRays cam = make_camera(ctx, W, H, row0);
-  s = render_impl(ctx, pose, rot, nullptr, &cam, n_rays, thr, K, static_cast<float*>(ctx->rgb.p), nullptr, d_ns, nullptr, st);
-  if (s != ADN_OK) return s;
-  ADN_CUDA(ctx, cudaMemcpyAsync(out_pinned ? static_cast<void*>(h_rgb) : ctx->h_out.p, ctx->rgb.p, size_t(n_rays) * 12,
-                                cudaMemcpyDeviceToHost, st));
-  if (h_nsamples)
-    ADN_CUDA(ctx, cudaMemcpyAsync(ns_pinned ? static_cast<void*>(h_nsamples) : ctx->h_ns.p, d_ns, size_t(n_rays) * 4,
-                                  cudaMemcpyDeviceToHost, st));
-  ADN_CUDA(ctx, cudaStreamSynchronize(st));
-  if (!out_pinned) std::memcpy(h_rgb, ctx->h_out.p, size_t(n_rays) * 12);
-  if (h_nsamples && !ns_pinned) std::memcpy(h_nsamples, ctx->h_ns.p, size_t(n_rays) * 4);
-  return check_device_error(ctx);
+  RenderCall c(pose, rot, int64_t(rows) * W, thr, K, nullptr);
+  c.cam = camera_rays(ctx, W, H, row0, rows);
+  if (!c.cam || !h_rgb) return fail(ctx, ADN_ERR_INVALID, "render_camera_host: bad arguments");
+  if (c.n_rays == 0) return ADN_OK;
+  return render_host(ctx, c, nullptr, h_rgb, h_nsamples);
 }
 
 // ---- stage-level entry points --------------------------------------------------------------------
 adn_status adn_generate_ray_directions(adn_ctx* ctx, int W, int H, int row0, int rows, float* d_dirs, void* stream) {
-  if (!ctx || !d_dirs || W < 1 || H < 1 || row0 < 0 || rows < 0 || row0 + rows > H) return fail(ctx, ADN_ERR_INVALID, "generate_ray_directions: bad arguments");
+  const std::optional<CameraRays> cam = camera_rays(ctx, W, H, row0, rows);
+  if (!cam || !d_dirs) return fail(ctx, ADN_ERR_INVALID, "generate_ray_directions: bad arguments");
   ADN_CUDA(ctx, cudaSetDevice(ctx->device));
-  const CameraRays cam = make_camera(ctx, W, H, row0);
-  ADN_CUDA(ctx, launch_gen_dirs(cam, int64_t(rows) * W, d_dirs, static_cast<cudaStream_t>(stream)));
+  ADN_CUDA(ctx, launch_gen_dirs(*cam, int64_t(rows) * W, d_dirs, static_cast<cudaStream_t>(stream)));
   ctx->stats.kernel_launches++;
   return ADN_OK;
 }
@@ -977,7 +978,7 @@ adn_status adn_mlp0_forward(adn_ctx* ctx, const float* d_x0, int64_t n_rays, flo
   Net& n = ctx->net[0];
   adn_status s = ensure(ctx, ctx->tiles0, size_t(pad128(n_rays) / 128) * n.prog.in.tile_bytes());
   if (s != ADN_OK) return s;
-  ADN_CUDA(ctx, launch_pack_rows(d_x0, n_rays, nullptr, n.n_in, n.prog.in, static_cast<uint8_t*>(ctx->tiles0.p), st));
+  ADN_CUDA(ctx, launch_pack_rows(d_x0, n_rays, nullptr, n.n_in, n.prog.in, static_cast<uint8_t*>(ctx->tiles0.p), ctx->num_sms, st));
   ctx->stats.kernel_launches++;
   return run_mlp(ctx, 0, static_cast<uint8_t*>(ctx->tiles0.p), d_raw0, nullptr, n_rays, st);
 }
@@ -991,7 +992,7 @@ adn_status adn_stage2_sample(adn_ctx* ctx, const float* d_raw0, int64_t n_rays, 
   ADN_CUDA(ctx, cudaSetDevice(ctx->device));
   adn_status s = ensure(ctx, ctx->s2scratch, stage2_scratch_bytes(n_rays));
   if (s != ADN_OK) return s;
-  ADN_CUDA(ctx, launch_stage2(d_raw0, n_rays, thr, K, ctx->d_zlut, d_count, d_offset, d_cell, d_ray, d_z, d_zp,
+  ADN_CUDA(ctx, launch_stage2(d_raw0, n_rays, thr, K, ctx->zlut.as<float>(), d_count, d_offset, d_cell, d_ray, d_z, d_zp,
                               reinterpret_cast<long long*>(d_total), ctx->s2scratch.p, &ctx->s2sync, static_cast<cudaStream_t>(stream)));
   ctx->stats.kernel_launches++;
   return ADN_OK;
@@ -1018,7 +1019,7 @@ adn_status adn_stage3_encode(adn_ctx* ctx, const float* d_ray_o, const float* d_
                              int64_t n_samples, float* d_x1, void* stream) {
   if (!ctx || !d_ray_o || !d_ray_d || !d_ray || !d_z || !d_x1 || n_samples < 0) return fail(ctx, ADN_ERR_INVALID, "stage3: bad arguments");
   ADN_CUDA(ctx, cudaSetDevice(ctx->device));
-  ADN_CUDA(ctx, launch_stage3(ctx->sc, d_ray_o, d_ray_d, d_ray, d_z, nullptr, 1, n_samples, nullptr, d_x1, nullptr,
+  ADN_CUDA(ctx, launch_stage3(ctx->sc, d_ray_o, d_ray_d, d_ray, d_z, nullptr, 1, n_samples, nullptr, d_x1, nullptr, ctx->num_sms,
                               static_cast<cudaStream_t>(stream)));
   ctx->stats.kernel_launches++;
   return ADN_OK;
@@ -1033,7 +1034,7 @@ adn_status adn_mlp1_forward(adn_ctx* ctx, const float* d_x1, int64_t n_samples, 
   Net& n = ctx->net[1];
   adn_status s = ensure(ctx, ctx->tiles1, size_t(pad128(n_samples) / 128) * n.prog.in.tile_bytes());
   if (s != ADN_OK) return s;
-  ADN_CUDA(ctx, launch_pack_rows(d_x1, n_samples, nullptr, n.n_in, n.prog.in, static_cast<uint8_t*>(ctx->tiles1.p), st));
+  ADN_CUDA(ctx, launch_pack_rows(d_x1, n_samples, nullptr, n.n_in, n.prog.in, static_cast<uint8_t*>(ctx->tiles1.p), ctx->num_sms, st));
   ctx->stats.kernel_launches++;
   return run_mlp(ctx, 1, static_cast<uint8_t*>(ctx->tiles1.p), d_raw1, nullptr, n_samples, st);
 }

@@ -347,11 +347,11 @@ cudaError_t launch_mlp(const MlpProgram& prog, const uint8_t* wblob, const uint8
 }
 
 cudaError_t launch_pack_rows(const float* x, long long rows, const long long* rows_dev, int n_feat, const TileFormat& fmt,
-                             uint8_t* tiles, cudaStream_t stream) {
+                             uint8_t* tiles, int num_sms, cudaStream_t stream) {
   long long work = ((rows + kTileM - 1) / kTileM) * kTileM * fmt.n_blk * 8;
   int grid = int((work + 255) / 256);
   if (grid < 1) grid = 1;
-  if (grid > 132 * 16) grid = 132 * 16;
+  if (grid > 16 * num_sms) grid = 16 * num_sms;
   pack_rows_kernel<<<grid, 256, 0, stream>>>(x, rows, rows_dev, n_feat, fmt, tiles);
   return cudaGetLastError();
 }

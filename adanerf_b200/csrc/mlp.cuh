@@ -86,6 +86,6 @@ cudaError_t launch_mlp(const MlpProgram& prog, const uint8_t* wblob, const uint8
                        const EncodeParams* enc = nullptr);
 // fp32 feature rows [rows, n_feat] -> packed tiles of format `fmt`.
 cudaError_t launch_pack_rows(const float* x, long long rows, const long long* rows_dev, int n_feat, const TileFormat& fmt,
-                             uint8_t* tiles, cudaStream_t stream);
+                             uint8_t* tiles, int num_sms, cudaStream_t stream);
 
 }  // namespace adn

@@ -909,11 +909,11 @@ stage3_kernel(const __grid_constant__ SceneDev sc, const float* __restrict__ ray
 
 cudaError_t launch_stage3(const SceneDev& sc, const float* d_ray_o, const float* d_ray_d, const int32_t* d_ray,
                           const float* d_z, const float* d_zlut_dense, int K, long long n_samples, const long long* d_total,
-                          float* d_x1, uint8_t* d_tiles1, cudaStream_t s) {
+                          float* d_x1, uint8_t* d_tiles1, int num_sms, cudaStream_t s) {
   // n_samples is an upper bound (capacity) when d_total is given
   if (n_samples <= 0) return cudaSuccess;
   long long blocks = (n_samples + kTileM - 1) / kTileM;
-  const long long cap = 132ll * 64;
+  const long long cap = 64ll * num_sms;
   if (d_total && blocks > cap) blocks = cap;   // grid-stride when the true count lives on the device
   static unsigned long long attr_done = 0;   // per device
   const int tile_bytes = int(shading_tiles().tile_bytes());

@@ -63,7 +63,7 @@ cudaError_t launch_stage2_dense(long long n_rays, int K, int32_t* d_count, int32
 // net's packed input tiles, shading_tiles in tiles.cuh) may be null (not written).
 cudaError_t launch_stage3(const SceneDev& sc, const float* d_ray_o, const float* d_ray_d, const int32_t* d_ray,
                           const float* d_z, const float* d_zlut_dense, int K, long long n_samples, const long long* d_total,
-                          float* d_x1, uint8_t* d_tiles1, cudaStream_t s);
+                          float* d_x1, uint8_t* d_tiles1, int num_sms, cudaStream_t s);
 
 // Optional per-ray / per-slot outputs of the composite (adaptive_raw2outputs' other return values and the tensors
 // RayMarchFromPoses.postprocess puts into the inference dict, src/features.py:536-577).  Any pointer may be null.

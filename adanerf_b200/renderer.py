@@ -171,23 +171,20 @@ class Renderer:
         ns = torch.empty((n,), dtype=torch.int32, device=self._dev()) if want_nsamples else None
         ow = torch.empty((n, 128), dtype=torch.float32, device=self._dev()) if want_oracle_weights else None
         out = dict(rgb=rgb, n_samples=ns, oracle_weights=ow)
+        aux = None
+        if want_aux:
+            aux = AuxOutputs()
+            for k in self.AUX_KEYS if want_aux is True else tuple(want_aux):
+                if k not in self.AUX_KEYS:
+                    raise KeyError(f"unknown auxiliary output {k!r}")
+                t = torch.empty((n, int(K)) if k in ("weights", "alpha", "z_vals") else (n,), dtype=torch.float32, device=self._dev())
+                out[k] = t
+                setattr(aux, "d_" + k, t.data_ptr())
         with torch.cuda.device(self.device):
-            if want_aux:
-                keys = self.AUX_KEYS if want_aux is True else tuple(want_aux)
-                aux = AuxOutputs()
-                for k in keys:
-                    if k not in self.AUX_KEYS:
-                        raise KeyError(f"unknown auxiliary output {k!r}")
-                    t = torch.empty((n, int(K)) if k in ("weights", "alpha", "z_vals") else (n,), dtype=torch.float32, device=self._dev())
-                    out[k] = t
-                    setattr(aux, "d_" + k, t.data_ptr())
-                self._check(self.lib.adn_render_rays_aux(self.handle, _fptr(p), _fptr(r), d.data_ptr(), n, float(thr), int(K),
-                                                         rgb.data_ptr(), ns.data_ptr() if ns is not None else None,
-                                                         ow.data_ptr() if ow is not None else None, C.byref(aux), self._stream()))
-            else:
-                self._check(self.lib.adn_render_rays(self.handle, _fptr(p), _fptr(r), d.data_ptr(), n, float(thr), int(K),
+            self._check(self.lib.adn_render_rays_aux(self.handle, _fptr(p), _fptr(r), d.data_ptr(), n, float(thr), int(K),
                                                      rgb.data_ptr(), ns.data_ptr() if ns is not None else None,
-                                                     ow.data_ptr() if ow is not None else None, self._stream()))
+                                                     ow.data_ptr() if ow is not None else None,
+                                                     C.byref(aux) if aux is not None else None, self._stream()))
         return out
 
     def render_camera(self, pose, rot, W, H, thr, K, row0=0, rows=None, out=None, want_nsamples=False):

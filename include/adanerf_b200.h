@@ -31,7 +31,7 @@ enum {
   ADN_OK = 0,
   ADN_ERR_INVALID = 1,      /* bad argument / unsupported shape */
   ADN_ERR_CUDA = 2,         /* CUDA runtime error (see adn_last_error) */
-  ADN_ERR_NO_DEVICE = 3,    /* no CUDA device / not compute capability 10.x */
+  ADN_ERR_NO_DEVICE = 3,    /* no CUDA device / not compute capability 9.x (Hopper) */
   ADN_ERR_NO_WEIGHTS = 4,   /* render called before both nets were set */
   ADN_ERR_IO = 5,           /* export directory / file problems */
   ADN_ERR_KERNEL = 6        /* device-side watchdog tripped (mbarrier timeout) */

@@ -441,6 +441,55 @@ def test_error_paths(bare):
     r.close()
 
 
+def _entry_status(r, entry, thr=0.2, K=8, row0=0, rows=8, W=8, H=8):
+    """Status of one call of a render entry point straight through the C ABI (the Python wrappers size their outputs from
+    the arguments first).  The rays entry points take rows * W rays."""
+    import ctypes as C
+    from adanerf_b200._lib import AuxOutputs
+    n = rows * W
+    pose = (C.c_float * 3)(*orc.SCENE_BARBERSHOP["view_cell_center"])
+    rot = (C.c_float * 9)(1, 0, 0, 0, 1, 0, 0, 0, 1)
+    dirs = torch.from_numpy(orc.generate_ray_directions(W, H, orc.SCENE_BARBERSHOP["fov"]).reshape(-1, 3)).float()
+    d_dirs, d_out = dirs.cuda(), torch.empty((W * H, 4), dtype=torch.float32, device="cuda")
+    d_ns = torch.empty((W * H,), dtype=torch.int32, device="cuda")
+    h_dirs, h_rgb, h_ns = dirs.numpy(), np.empty((W * H, 3), np.float32), np.empty((W * H,), np.int32)
+    lib, h = r.lib, r.handle
+    calls = {
+        "rays": lambda: lib.adn_render_rays(h, pose, rot, d_dirs.data_ptr(), n, thr, K, d_out.data_ptr(), d_ns.data_ptr(), None, None),
+        "rays_aux": lambda: lib.adn_render_rays_aux(h, pose, rot, d_dirs.data_ptr(), n, thr, K, d_out.data_ptr(), d_ns.data_ptr(),
+                                                    None, C.byref(AuxOutputs()), None),
+        "camera": lambda: lib.adn_render_camera(h, pose, rot, W, H, row0, rows, thr, K, d_out.data_ptr(), d_ns.data_ptr(), None),
+        "rgba8": lambda: lib.adn_render_camera_rgba8(h, pose, rot, W, H, row0, rows, thr, K, d_out.data_ptr(), None),
+        "rays_host": lambda: lib.adn_render_rays_host(h, pose, rot, h_dirs.ctypes.data, n, thr, K, h_rgb.ctypes.data, h_ns.ctypes.data),
+        "camera_host": lambda: lib.adn_render_camera_host(h, pose, rot, W, H, row0, rows, thr, K, h_rgb.ctypes.data, h_ns.ctypes.data),
+        "generate_ray_directions": lambda: lib.adn_generate_ray_directions(h, W, H, row0, rows, d_out.data_ptr(), None),
+    }
+    status = calls[entry]()
+    torch.cuda.synchronize()
+    return status
+
+
+@pytest.mark.parametrize("entry", ["rays", "rays_aux", "camera", "rgba8", "rays_host", "camera_host", "generate_ray_directions"])
+def test_render_entry_point_status_codes(entry):
+    """Each render entry point rejects every invalid argument it takes with ADN_ERR_INVALID (1), a render without
+    weights with ADN_ERR_NO_WEIGHTS (4), and returns ADN_OK (0) for an empty call (no rays / no rows)."""
+    renders = entry != "generate_ray_directions"
+    windowed = entry not in ("rays", "rays_aux", "rays_host")
+    cases = [(dict(K=0), 1), (dict(thr=-0.1), 1), (dict(thr=0.0, K=8), 1)] if renders else []   # thr 0: dense, needs K 128
+    if windowed:
+        cases += [(dict(row0=4, rows=5), 1), (dict(rows=-1), 1)]                                # row0 + rows > H
+    cases.append((dict(rows=0), 0))
+    bare = _renderer(orc.SCENE_BARBERSHOP)
+    assert _entry_status(bare, entry) == (4 if renders else 0)
+    bare.close()
+    sd0, sd1 = orc.make_weights("rand", seed=0)
+    r = _renderer(orc.SCENE_BARBERSHOP, sd0, sd1)
+    for args, status in cases:
+        assert _entry_status(r, entry, **args) == status, args
+    assert _entry_status(r, entry) == 0
+    r.close()
+
+
 @pytest.mark.parametrize("K", [8, 16])
 def test_threshold_sweep_vs_oracle(K, pavillon_weights):
     """BASELINE config 5: thr in {0.05, 0.1, 0.2, 0.3, 0.5} with the trained Pavillon weights (ragged sample counts at

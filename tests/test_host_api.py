@@ -1,5 +1,7 @@
 """Host-side behaviour of the public entry points (GPU): render() always uses the current parameters, explicit host
 buffer registration, several contexts in one process."""
+import ctypes
+
 import numpy as np
 import pytest
 import torch
@@ -61,9 +63,9 @@ def test_render_uses_the_current_parameters():
 
 
 def test_host_buffers_registered_explicitly_or_staged():
-    """render_rays_host: identical results whether the arrays are registered (DMA in place), plain (staged), or temporaries
-    created by a dtype conversion that die right after the call (ADVICE r1: implicit cudaHostRegister on such
-    temporaries left stale registrations behind)."""
+    """render_rays_host / render_camera_host: identical results whether the arrays are registered (DMA in place), plain
+    (staged), or temporaries created by a dtype conversion that die right after the call (ADVICE r1: implicit
+    cudaHostRegister on such temporaries left stale registrations behind)."""
     from adanerf_b200 import Renderer
     scene = orc.SCENE_BARBERSHOP
     sd0, sd1 = orc.make_weights("shaped", seed=0)
@@ -90,6 +92,22 @@ def test_host_buffers_registered_explicitly_or_staged():
         np.testing.assert_array_equal(got["rgb"], ref["rgb"].cpu().numpy())
         junk = [np.empty(dirs.shape, np.float32) for _ in range(3)]   # churn the allocator between calls
         del junk
+    # render_camera_host == render_camera, into plain (staged) arrays and into registered ones (DMA in place)
+    W, H, row0, rows = 800, 800, 300, 64
+    cam = r.render_camera(rays["pose"], rays["rot"], W, H, 0.2, 8, row0=row0, rows=rows, want_nsamples=True)
+    want_rgb, want_ns = cam["rgb"].cpu().numpy(), cam["n_samples"].cpu().numpy()
+    plain = r.render_camera_host(rays["pose"], rays["rot"], W, H, 0.2, 8, row0=row0, rows=rows, want_nsamples=True)
+    np.testing.assert_array_equal(plain["rgb"], want_rgb)
+    np.testing.assert_array_equal(plain["n_samples"], want_ns)
+    rgb, ns = np.empty((rows * W, 3), np.float32), np.empty((rows * W,), np.int32)
+    r.register_host_buffer(rgb)
+    r.register_host_buffer(ns)
+    p, q = (np.ascontiguousarray(np.asarray(x, np.float32).reshape(-1)) for x in (rays["pose"], rays["rot"]))
+    assert r.lib.adn_render_camera_host(r.handle, p.ctypes.data_as(ctypes.POINTER(ctypes.c_float)),
+                                        q.ctypes.data_as(ctypes.POINTER(ctypes.c_float)), W, H, row0, rows, 0.2, 8,
+                                        rgb.ctypes.data, ns.ctypes.data) == 0
+    np.testing.assert_array_equal(rgb, want_rgb)
+    np.testing.assert_array_equal(ns, want_ns)
     r.close()
 
 
