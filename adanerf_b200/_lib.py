@@ -41,7 +41,7 @@ class Stats(C.Structure):
 # every symbol include/adanerf_b200.h declares (tests/test_abi.py checks the .so exports all of them)
 SYMBOLS = [
     "adn_create", "adn_destroy", "adn_strerror", "adn_last_error", "adn_version", "adn_set_weights",
-    "adn_create_from_export_dir", "adn_probe_export_dir", "adn_render_camera_surface", "adn_register_host_buffer", "adn_unregister_host_buffer", "adn_net_dims", "adn_set_option", "adn_get_stats", "adn_last_threshold", "adn_render_rays", "adn_render_rays_aux", "adn_render_camera",
+    "adn_create_from_export_dir", "adn_probe_export_dir", "adn_render_camera_surface", "adn_register_host_buffer", "adn_unregister_host_buffer", "adn_net_dims", "adn_net_shape", "adn_set_option", "adn_get_stats", "adn_last_threshold", "adn_render_rays", "adn_render_rays_aux", "adn_render_camera",
     "adn_render_camera_rgba8", "adn_render_rays_host", "adn_render_camera_host", "adn_stage0_features",
     "adn_generate_ray_directions", "adn_mlp0_forward", "adn_stage2_sample", "adn_budget_threshold", "adn_stage3_encode",
     "adn_mlp1_forward", "adn_stage5_composite", "adn_image_metrics",
@@ -76,6 +76,7 @@ def load_library():
     lib.adn_register_host_buffer.argtypes = [vp, vp, C.c_size_t]
     lib.adn_unregister_host_buffer.argtypes = [vp, vp]
     lib.adn_net_dims.argtypes = [vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
+    lib.adn_net_shape.argtypes = [vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.adn_get_stats.argtypes = [vp, C.POINTER(Stats)]
     lib.adn_last_threshold.argtypes = [vp, fp]
     lib.adn_render_rays.argtypes = [vp, fp, fp, f32p, i64, C.c_float, C.c_int, f32p, i32p, f32p, vp]

@@ -16,7 +16,7 @@ from collections import OrderedDict
 
 import torch
 
-from .onnx_weights import write_export_dir
+from .onnx_weights import net_shapes, write_export_dir
 
 SAMPLING_KEYS = ("layers.0.weight", "layers.0.bias")
 SHADING_KEYS = ("pts_linears.0.weight", "views_linears.0.weight", "feature_linear.weight", "alpha_linear.weight",
@@ -41,7 +41,10 @@ def load_weights_file(path, allow_pickle=False):
 
 
 def check_state_dicts(sd0, sd1):
-    """The architecture the hot path implements: BaseNet sampling net, NeRF shading net with a view branch."""
+    """The architecture the hot path implements: BaseNet sampling net, NeRF shading net with a view branch, in the shapes
+    adn_set_weights accepts (include/adanerf_b200.h): sampling net 1-12 layers of hidden width 128 or 256, 128 outputs,
+    no skips; shading net 1-10 pts layers of width W = 128 or 256, at most one skip, view branch W/2.
+    Returns net_shapes(sd0, sd1); raises ValueError naming the offending tensor."""
     for k in SAMPLING_KEYS:
         if k not in sd0:
             raise ValueError(f"sampling net: missing {k} (expected BaseNet layers.{{i}}.weight/bias, src/models.py:71-76)")
@@ -49,7 +52,40 @@ def check_state_dicts(sd0, sd1):
         if k not in sd1:
             raise ValueError(f"shading net: missing {k} (expected NeRF with use_viewdirs, src/models.py:214-250)")
     if sd0["layers.0.weight"].shape[1] not in (90, 30) or sd1["pts_linears.0.weight"].shape[1] != 63:
-        raise ValueError("posEncArgs other than [10-4, 10-4] / [2-2, 10-4] (90 or 30 / 63+27 input features) are not supported")
+        raise ValueError(f"layers.0.weight / pts_linears.0.weight read {sd0['layers.0.weight'].shape[1]} / "
+                         f"{sd1['pts_linears.0.weight'].shape[1]} columns: posEncArgs other than [10-4, 10-4] / [2-2, 10-4] "
+                         "(90 or 30 / 63+27 input features) are not supported")
+    shapes = net_shapes(sd0, sd1)
+    (d0, w0, _), (d1, w1, _) = shapes
+
+    def expect(sd, name, rows, cols, what):
+        have = tuple(sd[name].shape) if name in sd else None
+        if have != (rows, cols):
+            raise ValueError(f"{what}: {name} is {list(have) if have else 'missing'}, expected [{rows}, {cols}]")
+
+    if not 1 <= d0 <= 12:
+        raise ValueError(f"sampling net: layers.0 .. layers.{d0 - 1}: {d0} layers, 1-12 are supported")
+    for i in range(d0):
+        n_out = 128 if i == d0 - 1 else w0
+        if n_out not in (128, 256):
+            raise ValueError(f"sampling net: layers.{i}.weight has {n_out} outputs; the hidden width must be 128 or 256")
+        expect(sd0, f"layers.{i}.weight", n_out, sd0["layers.0.weight"].shape[1] if i == 0 else w0,
+               "sampling net (no skips; layer widths must chain, 128 outputs)")
+    if w1 not in (128, 256):
+        raise ValueError(f"shading net: pts_linears.0.weight has {w1} rows; the width W must be 128 or 256")
+    if not 1 <= d1 <= 10:
+        raise ValueError(f"shading net: pts_linears.0 .. pts_linears.{d1 - 1}: {d1} layers, 1-10 are supported")
+    n_skips = 0
+    for i in range(1, d1):
+        k = int(sd1[f"pts_linears.{i}.weight"].shape[1])
+        n_skips += int(k == w1 + 63)
+        if n_skips > 1:
+            raise ValueError(f"shading net: pts_linears.{i}.weight reads cat[pts, h] a second time; at most one skip is supported")
+        expect(sd1, f"pts_linears.{i}.weight", w1, k if k == w1 + 63 else w1, f"shading net (W = {w1}, a skip reads W + 63)")
+    for name, rows, cols in (("feature_linear", w1, w1), ("alpha_linear", 1, w1), ("views_linears.0", w1 // 2, w1 + 27),
+                             ("rgb_linear", 3, w1 // 2)):
+        expect(sd1, name + ".weight", rows, cols, f"shading net (W = {w1}, posEnc 10-4)")
+    return shapes
 
 
 def read_dataset_info(path):

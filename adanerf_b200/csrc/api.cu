@@ -1,6 +1,7 @@
 // C ABI + host-side context of the H100 AdaNeRF renderer (see include/adanerf_b200.h).
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -47,6 +48,7 @@ struct Buf {
 struct Net {
   bool ready = false;
   int n_in = 0, n_out = 0;
+  int depth = 0, width = 0, skip = -1;   // the shape build_net0 / build_net1 inferred from the tensors (adn_net_shape)
   MlpProgram prog{};
   Buf wblob;
   std::map<std::string, HostTensor> tensors;  // kept so "mlp0_terms" can re-pack
@@ -195,7 +197,9 @@ const HostTensor* find(const Net& n, const std::string& name) {
 }
 
 adn_status upload(adn_ctx* ctx, Net& net, const std::vector<uint8_t>& wblob, const std::vector<float>& fblob) {
-  if (fblob.size() > size_t(kSideFloats)) return fail(ctx, ADN_ERR_INVALID, "network has too many fp32 side parameters");
+  if (fblob.size() > size_t(kSideFloats))
+    return fail(ctx, ADN_ERR_INVALID, "network has " + std::to_string(fblob.size()) + " fp32 side parameters (biases and heads), more than " +
+                                          std::to_string(kSideFloats) + " fit in shared memory");
   std::memset(net.prog.side, 0, sizeof(net.prog.side));
   std::memcpy(net.prog.side, fblob.data(), fblob.size() * 4);
   adn_status s = ensure(ctx, net.wblob, wblob.size());   // the callers synchronised: no kernel still reads the old blob
@@ -204,39 +208,52 @@ adn_status upload(adn_ctx* ctx, Net& net, const std::vector<uint8_t>& wblob, con
   return ADN_OK;
 }
 
-// Sampling net: BaseNet without skips (src/models.py:71-76,183-195): layers.{i}.weight/bias.
+// The layer programs of the two networks are derived here, from the tensor shapes, and nowhere else in the library.
+//
+// Sampling net: BaseNet without skips (src/models.py:71-76,183-195): layers.{i}.weight/bias, D = 1-12 layers, n_in <= 128
+// inputs, every hidden layer W = 128 or 256 wide, 128 or 256 outputs.  Layer 0 reads the input blocks, every other layer
+// the W/64 activation blocks, which its epilogue overwrites in place.
 adn_status build_net0(adn_ctx* ctx) {
   Net& net = ctx->net[0];
+  auto bad = [&](const std::string& msg) { return fail(ctx, ADN_ERR_INVALID, "sampling net: " + msg); };
   int D = 0;
   while (find(net, "layers." + std::to_string(D) + ".weight")) ++D;
-  if (D < 1 || D > kMaxLayers) return fail(ctx, ADN_ERR_INVALID, "sampling net: need layers.0.weight .. (1-12 layers)");
+  if (D < 1 || D > kMaxLayers) return bad("need layers.0.weight .. (1-12 layers)");
   const int nsplit = ctx->mlp0_terms == 3 ? 2 : 1;
+  const int width = int(find(net, "layers.0.weight")->rows);   // the hidden width W (the output width of a 1-layer net)
   MlpProgram P{};
   P.n_layers = D;
   std::vector<uint8_t> wblob;
   std::vector<float> fblob;
   int prev = -1;
   for (int l = 0; l < D; ++l) {
-    const HostTensor* W = find(net, "layers." + std::to_string(l) + ".weight");
-    const HostTensor* B = find(net, "layers." + std::to_string(l) + ".bias");
-    if (!B || int64_t(B->data.size()) != W->rows) return fail(ctx, ADN_ERR_INVALID, "sampling net: missing/odd bias");
+    const std::string name = "layers." + std::to_string(l);
+    const HostTensor* W = find(net, name + ".weight");
+    const HostTensor* B = find(net, name + ".bias");
+    if (!B || int64_t(B->data.size()) != W->rows) return bad(name + ".bias is missing or not [" + std::to_string(W->rows) + "]");
     const int n_out = int(W->rows), k_in = int(W->cols);
     const bool last = (l == D - 1);
     if (l == 0) {
-      if (k_in < 1 || k_in > 128) return fail(ctx, ADN_ERR_INVALID, "sampling net: input width must be <= 128");
+      if (k_in < 1 || k_in > 128) return bad(name + ".weight has " + std::to_string(k_in) + " input columns; the input width must be 1-128");
       net.n_in = k_in;
     } else if (k_in != prev) {
-      return fail(ctx, ADN_ERR_INVALID, "sampling net: layer widths do not chain");
+      return bad(name + ".weight has " + std::to_string(k_in) + " input columns but layers." + std::to_string(l - 1) + " has " +
+                 std::to_string(prev) + " outputs: layer widths must chain (BaseNet skips are not supported)");
     }
-    if (!last && n_out != 256) return fail(ctx, ADN_ERR_INVALID, "sampling net: hidden width must be 256");
-    if (last && n_out != 128 && n_out != 256) return fail(ctx, ADN_ERR_INVALID, "sampling net: output width must be 128 or 256");
+    if (!last && n_out != width)
+      return bad(name + ".weight has " + std::to_string(n_out) + " outputs; every hidden layer must be as wide as layers.0 (" +
+                 std::to_string(width) + ")");
+    if (!last && n_out != 128 && n_out != 256)
+      return bad(name + ".weight has " + std::to_string(n_out) + " outputs; the hidden width must be 128 or 256");
+    if (last && n_out != 128 && n_out != 256)
+      return bad(name + ".weight has " + std::to_string(n_out) + " outputs; the output width must be 128 or 256");
     prev = n_out;
     MlpLayer& L = P.layers[l];
     std::vector<Seg> segs;
     if (l == 0) {
       segs = {{0, std::min(64, k_in)}, {64, std::max(0, k_in - 64)}};
     } else {
-      segs = {{0, 64}, {64, 64}, {128, 64}, {192, 64}};
+      for (int c = 0; c < k_in; c += 64) segs.push_back({c, 64});
     }
     L.n_kb = uint8_t(segs.size());
     for (size_t i = 0; i < segs.size(); ++i) {
@@ -260,102 +277,139 @@ adn_status build_net0(adn_ctx* ctx) {
   net.prog = P;
   adn_status s = upload(ctx, net, wblob, fblob);
   if (s != ADN_OK) return s;
+  net.depth = D;
+  net.width = width;
+  net.skip = -1;
   net.ready = true;
   return ADN_OK;
 }
 
-// Shading net: NeRF(D=8, W=256, skips=[4], use_viewdirs=True) (src/models.py:199-277).
+// Shading net: NeRF(D, W, skips, use_viewdirs=True) (src/models.py:199-277) with posEnc 10-4 (63 position + 27 direction
+// features).  D = 1-10 pts_linears (D + feature + view layer <= kMaxLayers), W = 128 or 256, the view branch W/2.  A skip
+// after pts layer i shows as pts_linears.{i+1} reading W + 63 columns, cat[pts, h] (models.py:226-228, 260-261); at most
+// one.  The program, activation block 0 holding the input block P (then V) and blocks 1.. the W/64 hidden blocks:
+//   pts layer 0 reads P; the skip consumer reads P and the hidden blocks; the other pts layers read the hidden blocks; the
+//   last pts layer also forms alpha (LF_ALPHA_DOT); V replaces P after the skip consumer, or after layer 0 without a skip;
+//   feature_linear: W -> W without activation; views_linears.0 on cat[feature, V] -> W/2, with rgb_linear in its epilogue.
+// At W = 128 the view layer's 64 outputs are padded to the kernel's 128 rows with zero weights, zero biases and zero
+// rgb_linear columns: ReLU(0) = 0 adds nothing to the rgb dot products, so the result is exact.
 adn_status build_net1(adn_ctx* ctx) {
   Net& net = ctx->net[1];
-  auto need = [&](const std::string& n, int64_t r, int64_t c) -> const HostTensor* {
-    const HostTensor* t = find(net, n);
-    if (!t || t->rows != r || t->cols != c) return nullptr;
-    return t;
-  };
-  const HostTensor *pw[8], *pb[8];
-  for (int i = 0; i < 8; ++i) {
-    const int64_t k = (i == 0) ? 63 : (i == 5 ? 319 : 256);
-    pw[i] = need("pts_linears." + std::to_string(i) + ".weight", 256, k);
-    pb[i] = find(net, "pts_linears." + std::to_string(i) + ".bias");
-    if (!pw[i] || !pb[i] || pb[i]->data.size() != 256)
-      return fail(ctx, ADN_ERR_INVALID, "shading net: pts_linears." + std::to_string(i) + " has the wrong shape (expect NeRF 8x256, skip 4, posEnc 10-4)");
+  constexpr int kP = 63, kV = 27;
+  auto bad = [&](const std::string& msg) { return fail(ctx, ADN_ERR_INVALID, "shading net: " + msg); };
+  auto shape = [](int64_t r, int64_t c) { return "[" + std::to_string(r) + ", " + std::to_string(c) + "]"; };
+  const HostTensor* w0 = find(net, "pts_linears.0.weight");
+  if (!w0 || w0->cols != kP)
+    return bad("pts_linears.0.weight must be [W, 63] (posEnc 10-4)" + (w0 ? ", not " + shape(w0->rows, w0->cols) : std::string(", missing")));
+  const int W = int(w0->rows);
+  if (W != 128 && W != 256) return bad("pts_linears.0.weight has " + std::to_string(W) + " rows; the width W must be 128 or 256");
+  int D = 0;
+  while (find(net, "pts_linears." + std::to_string(D) + ".weight")) ++D;
+  if (D > kMaxLayers - 2) return bad("pts_linears.0 .. " + std::to_string(D - 1) + ": " + std::to_string(D) + " layers, at most 10 are supported");
+  const HostTensor *pw[kMaxLayers], *pb[kMaxLayers];
+  int skip = -1;
+  for (int i = 0; i < D; ++i) {
+    const std::string name = "pts_linears." + std::to_string(i);
+    pw[i] = find(net, name + ".weight");
+    pb[i] = find(net, name + ".bias");
+    if (pw[i]->rows != W) return bad(name + ".weight has " + std::to_string(pw[i]->rows) + " rows; every pts layer must be W = " + std::to_string(W) + " wide");
+    if (i > 0 && pw[i]->cols == W + kP) {
+      if (skip >= 0)
+        return bad(name + ".weight reads cat[pts, h] after the skip at layer " + std::to_string(skip) + "; at most one skip is supported");
+      skip = i - 1;
+    } else if (i > 0 && pw[i]->cols != W) {
+      return bad(name + ".weight has " + std::to_string(pw[i]->cols) + " input columns; expect W = " + std::to_string(W) +
+                 " or W + 63 = " + std::to_string(W + kP) + " (a skip)");
+    }
+    if (!pb[i] || int64_t(pb[i]->data.size()) != W) return bad(name + ".bias is missing or not [" + std::to_string(W) + "]");
   }
-  const HostTensor* fw = need("feature_linear.weight", 256, 256);
-  const HostTensor* fb = find(net, "feature_linear.bias");
-  const HostTensor* aw = need("alpha_linear.weight", 1, 256);
-  const HostTensor* ab = find(net, "alpha_linear.bias");
-  const HostTensor* vw = need("views_linears.0.weight", 128, 283);
-  const HostTensor* vb = find(net, "views_linears.0.bias");
-  const HostTensor* rw = need("rgb_linear.weight", 3, 128);
-  const HostTensor* rb = find(net, "rgb_linear.bias");
-  if (!fw || !fb || !aw || !ab || !vw || !vb || !rw || !rb || fb->data.size() != 256 || ab->data.size() != 1 ||
-      vb->data.size() != 128 || rb->data.size() != 3)
-    return fail(ctx, ADN_ERR_INVALID, "shading net: feature/alpha/views/rgb tensors missing or wrong shape");
-  net.n_in = 90;
+  struct Want {
+    const char* name;
+    int64_t rows, cols;
+  };
+  const Want want[4] = {{"feature_linear", W, W}, {"alpha_linear", 1, W}, {"views_linears.0", W / 2, W + kV}, {"rgb_linear", 3, W / 2}};
+  const HostTensor *hw[4], *hb[4];
+  for (int j = 0; j < 4; ++j) {
+    const std::string name(want[j].name);
+    hw[j] = find(net, name + ".weight");
+    hb[j] = find(net, name + ".bias");
+    if (!hw[j] || hw[j]->rows != want[j].rows || hw[j]->cols != want[j].cols)
+      return bad(name + ".weight must be " + shape(want[j].rows, want[j].cols) + " for W = " + std::to_string(W) + " (posEnc 10-4)" +
+                 (hw[j] ? ", not " + shape(hw[j]->rows, hw[j]->cols) : std::string(", missing")));
+    if (!hb[j] || int64_t(hb[j]->data.size()) != want[j].rows) return bad(name + ".bias is missing or not [" + std::to_string(want[j].rows) + "]");
+  }
+  const HostTensor *fw = hw[0], *fb = hb[0], *aw = hw[1], *ab = hb[1], *vw = hw[2], *vb = hb[2], *rw = hw[3], *rb = hb[3];
+  net.n_in = kP + kV;
   net.n_out = 4;
+  const int nh = W / 64;                       // hidden activation blocks 1 .. nh
+  const int load_v = skip >= 0 ? skip + 1 : 0;   // the layer after which V replaces P
   MlpProgram P{};
-  P.n_layers = 10;
+  P.n_layers = D + 2;
   std::vector<uint8_t> wblob;
   std::vector<float> fblob;
-  const std::vector<Seg> segH = {{0, 64}, {64, 64}, {128, 64}, {192, 64}};
-  for (int l = 0; l < 10; ++l) {
+  for (int l = 0; l < D + 2; ++l) {
     MlpLayer& L = P.layers[l];
     std::vector<Seg> segs;
-    const HostTensor *W, *B;
+    std::vector<uint8_t> blk;
+    auto read_p = [&] { segs.push_back({0, kP}), blk.push_back(0); };
+    auto read_hidden = [&](int col0) {
+      for (int b = 0; b < nh; ++b) segs.push_back({col0 + 64 * b, 64}), blk.push_back(uint8_t(1 + b));
+    };
+    const HostTensor *Wt, *B;
     L.out_blk0 = 1;
-    L.n_half = 2;
-    if (l == 0) {
-      segs = {{0, 63}};
-      L.a_blk[0] = 0;
-      L.flags = LF_RELU | LF_OUT_ACT;
-      W = pw[0];
-      B = pb[0];
-    } else if (l == 5) {
-      segs = {{0, 63}, {63, 64}, {127, 64}, {191, 64}, {255, 64}};   // cat[pts, h] (models.py:260-261)
-      const uint8_t blk[5] = {0, 1, 2, 3, 4};
-      std::memcpy(L.a_blk, blk, 5);
-      L.flags = LF_RELU | LF_OUT_ACT | LF_LOAD_IN1_AFTER;
-      W = pw[5];
-      B = pb[5];
-    } else if (l <= 7) {
-      segs = segH;
-      const uint8_t blk[5] = {1, 2, 3, 4, 0};
-      std::memcpy(L.a_blk, blk, 5);
-      L.flags = LF_RELU | LF_OUT_ACT | (l == 7 ? LF_ALPHA_DOT : 0);
-      W = pw[l];
+    L.n_half = uint8_t(W / 128);
+    if (l < D) {
+      if (l == 0) {
+        read_p();
+      } else if (l == skip + 1) {   // cat[pts, h]
+        read_p();
+        read_hidden(kP);
+      } else {
+        read_hidden(0);
+      }
+      L.flags = LF_RELU | LF_OUT_ACT | (l == D - 1 ? LF_ALPHA_DOT : 0) | (l == load_v ? LF_LOAD_IN1_AFTER : 0);
+      Wt = pw[l];
       B = pb[l];
-    } else if (l == 8) {  // feature_linear: no activation (models.py:265)
-      segs = segH;
-      const uint8_t blk[5] = {1, 2, 3, 4, 0};
-      std::memcpy(L.a_blk, blk, 5);
+    } else if (l == D) {  // feature_linear: no activation (models.py:265)
+      read_hidden(0);
       L.flags = LF_OUT_ACT;
-      W = fw;
+      Wt = fw;
       B = fb;
     } else {  // views_linears.0 on cat[feature, views] (models.py:266-269) + rgb_linear in the epilogue
-      segs = {{0, 64}, {64, 64}, {128, 64}, {192, 64}, {256, 27}};
-      const uint8_t blk[5] = {1, 2, 3, 4, 0};
-      std::memcpy(L.a_blk, blk, 5);
+      read_hidden(0);
+      segs.push_back({W, kV});
+      blk.push_back(0);
       L.flags = LF_RELU | LF_FINAL_RGB | LF_WAIT_IN;
       L.n_half = 1;
-      W = vw;
+      Wt = vw;
       B = vb;
     }
     L.n_kb = uint8_t(segs.size());
-    for (size_t i = 0; i < segs.size(); ++i) L.k_cnt[i] = uint8_t((segs[i].valid + 15) / 16);
+    for (size_t i = 0; i < segs.size(); ++i) {
+      L.a_blk[i] = blk[i];
+      L.k_cnt[i] = uint8_t((segs[i].valid + 15) / 16);
+    }
     L.w_off = uint32_t(wblob.size());
-    pack_layer(W->data.data(), int(W->rows), int(W->cols), segs, 1, wblob);
-    L.bias_off = uint32_t(push_floats(fblob, B->data.data(), B->data.size()));
+    pack_layer(Wt->data.data(), int(Wt->rows), int(Wt->cols), segs, 1, wblob);
+    std::vector<float> bias(size_t(L.n_half) * 128, 0.0f);   // zero rows past the view layer's W/2 outputs
+    std::copy(B->data.begin(), B->data.end(), bias.begin());
+    L.bias_off = uint32_t(push_floats(fblob, bias.data(), bias.size()));
   }
-  P.alpha_w_off = uint32_t(push_floats(fblob, aw->data.data(), 256));
+  std::vector<float> rgb_w(3 * 128, 0.0f);   // rgb_linear at the kernel's row stride of 128
+  for (int k = 0; k < 3; ++k) std::copy_n(rw->data.data() + size_t(k) * (W / 2), W / 2, rgb_w.data() + k * 128);
+  P.alpha_w_off = uint32_t(push_floats(fblob, aw->data.data(), size_t(W)));
   P.alpha_b_off = uint32_t(push_floats(fblob, ab->data.data(), 1));
-  P.rgb_w_off = uint32_t(push_floats(fblob, rw->data.data(), 3 * 128));
+  P.rgb_w_off = uint32_t(push_floats(fblob, rgb_w.data(), rgb_w.size()));
   P.rgb_b_off = uint32_t(push_floats(fblob, rb->data.data(), 3));
   P.in = shading_tiles();
-  P.in_nblk0 = 1;   // P; V after layer 5
+  P.in_nblk0 = 1;   // P; V after layer load_v
   P.out_cols = 4;
   net.prog = P;
   adn_status s = upload(ctx, net, wblob, fblob);
   if (s != ADN_OK) return s;
+  net.depth = D;
+  net.width = W;
+  net.skip = skip;
   net.ready = true;
   return ADN_OK;
 }
@@ -929,6 +983,16 @@ adn_status adn_net_dims(adn_ctx* ctx, int net_id, int* n_in, int* n_out) {
   if (!ctx->net[net_id].ready) return fail(ctx, ADN_ERR_NO_WEIGHTS, "net_dims: network not set");
   if (n_in) *n_in = ctx->net[net_id].n_in;
   if (n_out) *n_out = ctx->net[net_id].n_out;
+  return ADN_OK;
+}
+
+adn_status adn_net_shape(adn_ctx* ctx, int net_id, int* depth, int* width, int* skip) {
+  if (!ctx || (net_id != 0 && net_id != 1)) return fail(ctx, ADN_ERR_INVALID, "net_shape: bad arguments");
+  const Net& n = ctx->net[net_id];
+  if (!n.ready) return fail(ctx, ADN_ERR_NO_WEIGHTS, "net_shape: network not set");
+  if (depth) *depth = n.depth;
+  if (width) *width = n.width;
+  if (skip) *skip = n.skip;
   return ADN_OK;
 }
 

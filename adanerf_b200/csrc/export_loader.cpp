@@ -239,6 +239,36 @@ bool load_export_dir(const std::string& dir_in, ExportDir& out, std::string& err
   }
   for (int i = 0; i < 2; ++i)
     if (!read_onnx_initializers(dir + "model" + std::to_string(i) + ".onnx", out.nets[i], err)) return false;
+  // The networks' shapes come from the initialisers.  config.ini's layers / layerWidth (src/util/config.py:55-56), when
+  // present, must describe the same networks: depth = the number of layers.{i} / pts_linears.{i} weights, width = the
+  // input columns of layers.1 (the rows of layers.0 of a one-layer net) / of alpha_linear.
+  for (int i = 0; i < 2; ++i) {
+    const std::string prefix = i == 0 ? "layers." : "pts_linears.";
+    int depth = 0, width = 0, width0 = 0;
+    for (const NamedTensor& t : out.nets[i]) {
+      if (i == 1 && t.name == "alpha_linear.weight") width = int(t.cols);
+      if (t.name.compare(0, prefix.size(), prefix) != 0 || t.name.size() < 7 || t.name.compare(t.name.size() - 7, 7, ".weight") != 0)
+        continue;
+      const int idx = std::atoi(t.name.c_str() + prefix.size());
+      depth = std::max(depth, idx + 1);
+      if (i == 0 && idx == 0) width0 = int(t.rows);
+      if (i == 0 && idx == 1) width = int(t.cols);
+    }
+    if (i == 0 && depth == 1) width = width0;
+    const std::string onnx = "model" + std::to_string(i) + ".onnx";
+    for (const auto& [key, have] : {std::pair<const char*, int>{"layers", depth}, {"layerWidth", width}}) {
+      auto it = cfg.find(key);
+      if (it == cfg.end()) continue;
+      const auto items = list_items(it->second);
+      if (items.size() != 2) continue;
+      const int want = std::atoi(items[size_t(i)].c_str());
+      if (want != have) {
+        err = "config.ini: " + std::string(key) + " = " + strip(it->second) + " but " + onnx + " holds a network with " + key + " " +
+              std::to_string(have);
+        return false;
+      }
+    }
+  }
   return true;
 }
 

@@ -95,4 +95,8 @@ const char* ImageGenerator::last_error() const { return err_.c_str(); }
 
 bool ImageGenerator::stats(adn_stats* out) { return ctx_ && adn_get_stats(ctx_, out) == ADN_OK; }
 
+bool ImageGenerator::net_shape(int net_id, int* depth, int* width, int* skip) {
+  return ctx_ && adn_net_shape(ctx_, net_id, depth, width, skip) == ADN_OK;
+}
+
 }  // namespace adn_host

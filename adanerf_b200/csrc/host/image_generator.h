@@ -67,6 +67,8 @@ class ImageGenerator {
 
   const char* last_error() const;
   bool stats(adn_stats* out);
+  // The loaded network's shape (adn_net_shape): depth, width and skip layer (-1 = none).
+  bool net_shape(int net_id, int* depth, int* width, int* skip);
 
  private:
   adn_ctx* ctx_ = nullptr;

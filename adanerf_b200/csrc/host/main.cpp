@@ -88,6 +88,10 @@ int main(int argc, char** argv) {
   }
   adn_host::ImageGenerator gen;
   if (!gen.load(config, device)) { std::fprintf(stderr, "load failed: %s\n", gen.last_error()); return 1; }
+  for (int id = 0; id < 2; ++id) {
+    int d = 0, w = 0, sk = -1;
+    if (gen.net_shape(id, &d, &w, &sk)) std::printf("net %d: %s %d x %d, skip %d\n", id, id == 0 ? "sampling" : "shading", d, w, sk);
+  }
   if (budget > 0 && !gen.set_sample_budget(budget)) { std::fprintf(stderr, "sample budget: %s\n", gen.last_error()); return 1; }
   std::vector<int32_t> ns(budget > 0 ? size_t(W) * H : 0);   // per-ray sample counts, for M under a budget
   adn_host::Camera cam;

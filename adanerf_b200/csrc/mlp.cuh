@@ -25,7 +25,9 @@ namespace adn {
 
 constexpr int kMaxLayers = 12;
 constexpr int kMlpThreads = 384;  // three warpgroups: two consumers, one weight producer
-constexpr int kSideFloats = 3208; // fp32 side parameters (biases, alpha / rgb heads), copied to shared memory per CTA
+// fp32 side parameters (biases, alpha / rgb heads), copied to shared memory per CTA.  The largest supported net sets it: a
+// 10 x 256 shading net has 10 x 256 pts biases, 256 + 128 feature / view biases, 256 + 4 alpha and 384 + 4 rgb floats.
+constexpr int kSideFloats = 3592;
 
 enum : uint8_t {
   LF_RELU = 1,

@@ -138,11 +138,36 @@ def write_onnx_initializers(path, tensors):
         f.write(model)
 
 
+def net_shapes(sd0, sd1):
+    """The reference's `layers`, `layerWidth` and `skips` of the two networks, read from the tensor shapes as
+    adn_set_weights reads them: depth = the number of layers.{i} / pts_linears.{i} weights, width = the rows of the first,
+    and a shading-net skip after layer i when pts_linears.{i+1} reads W + 63 columns (-1: none).
+    Returns ((D0, W0, -1), (D1, W1, skip))."""
+    def depth(sd, prefix):
+        d = 0
+        while f"{prefix}{d}.weight" in sd:
+            d += 1
+        return d
+    d0, d1 = depth(sd0, "layers."), depth(sd1, "pts_linears.")
+    w0, w1 = int(sd0["layers.0.weight"].shape[0]), int(sd1["pts_linears.0.weight"].shape[0])
+    skips = [i - 1 for i in range(1, d1) if int(sd1[f"pts_linears.{i}.weight"].shape[1]) == w1 + 63]
+    return (d0, w0, -1), (d1, w1, skips[0] if skips else -1)
+
+
+def _skips_entry(depth, skip):
+    """The shading net's `skips` config entry that builds this net in the reference (models.py:210-213): "auto" is a skip
+    at 4 for D >= 6 and none for D <= 4; otherwise the skip layer, or for no skip a layer index the net never reaches."""
+    if skip == 4 or (skip < 0 and depth <= 4):
+        return "auto"
+    return str(skip if skip >= 0 else depth)
+
+
 def write_export_dir(path, scene, sd0, sd1, thr, K):
     """Writes {config.ini, dataset_info.txt, model0.onnx, model1.onnx} in the reference's export format
-    (src/export.py:28-93, src/train_data.py:180-195)."""
+    (src/export.py:28-93, src/train_data.py:180-195), config.ini with the networks' layers / layerWidth / skips."""
     import os
     os.makedirs(path, exist_ok=True)
+    (d0, w0, _), (d1, w1, skip) = net_shapes(sd0, sd1)
     as_np = lambda sd: {k: (v.detach().cpu().numpy() if hasattr(v, "detach") else np.asarray(v)) for k, v in sd.items()}
     write_onnx_initializers(os.path.join(path, "model0.onnx"), as_np(sd0))
     write_onnx_initializers(os.path.join(path, "model1.onnx"), as_np(sd1))
@@ -167,3 +192,4 @@ def write_export_dir(path, scene, sd0, sd1, thr, K):
                     "rayMarchNormalization = [InverseSqrtDistCentered, InverseSqrtDistCentered]\n"
                     f"numRaymarchSamples = [{K}, {K}]\ndepthTransform = log\nzNear = [0.001, 0.001]\nzFar = [1.0, 1.0]\n"
                     f"adaptiveSamplingThreshold = {thr}\nmultiDepthFeatures = [128, 128]\naccumulationMult = alpha\n")
+        f.write(f"activation = [relu, nerf]\nlayers = [{d0}, {d1}]\nlayerWidth = [{w0}, {w1}]\nskips = [, {_skips_entry(d1, skip)}]\n")

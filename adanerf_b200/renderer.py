@@ -112,6 +112,12 @@ class Renderer:
         self._check(self.lib.adn_net_dims(self.handle, int(net_id), C.byref(n_in), C.byref(n_out)))
         return n_in.value, n_out.value
 
+    def net_shape(self, net_id):
+        """(depth, width, skip) the library inferred from the weights of network net_id; skip = -1 when it has none."""
+        d, w, s = C.c_int(), C.c_int(), C.c_int()
+        self._check(self.lib.adn_net_shape(self.handle, int(net_id), C.byref(d), C.byref(w), C.byref(s)))
+        return d.value, w.value, s.value
+
     def register_host_buffer(self, array):
         """Page-locks a numpy array in place so render_rays_host / render_camera_host DMA straight from / to it.  The
         renderer keeps a reference (the memory must outlive the registration); unregister_host_buffer or close() ends it."""

@@ -90,8 +90,19 @@ const char* adn_version(void);
 
 /* net_id 0 = sampling net (BaseNet, src/models.py:18-195), 1 = shading net (NeRF, :199-277).
  * Packs the fp32 parameters into the kernels' layout (bf16 hi/lo split, swizzled K-major tiles).
- * Replaces load_state_dict / ImageGenerator::initEngine's ONNX->TensorRT build. */
+ * Replaces load_state_dict / ImageGenerator::initEngine's ONNX->TensorRT build.
+ * The network's shape (the reference's `layers`, `layerWidth`, `skips`) is read from the tensor shapes:
+ *   sampling net: layers.0 .. layers.{D-1}, D = 1-12, at most 128 inputs, hidden width W = 128 or 256 in every hidden
+ *     layer, 128 or 256 outputs (a render needs 128); no skips.
+ *   shading net: posEnc 10-4 (pts_linears.0 reads 63 columns, views_linears.0 reads W + 27), D = 1-10 pts_linears,
+ *     W = 128 or 256, view branch W/2; no skip, or one skip after layer i in [0, D-2], which shows as pts_linears.{i+1}
+ *     reading W + 63 columns (the reference's skips = auto is a skip at 4 for D >= 6 and none for D <= 4).
+ * Any other shape fails with ADN_ERR_INVALID and adn_last_error names the offending tensor. */
 adn_status adn_set_weights(adn_ctx* ctx, int net_id, const adn_tensor_desc* tensors, int n_tensors);
+
+/* The shape adn_set_weights inferred: depth D, width W (of a one-layer sampling net: its output width) and the skip layer
+ * (-1 = none; always -1 for the sampling net). */
+adn_status adn_net_shape(adn_ctx* ctx, int net_id, int* depth, int* width, int* skip);
 
 /* Loads {config.ini, dataset_info.txt, model0.onnx, model1.onnx} as written by src/export.py:28-93
  * (the directory the C++ viewer takes with -mp, adanerf_real_time_viewer/README.md:38-43).
