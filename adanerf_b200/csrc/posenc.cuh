@@ -10,10 +10,12 @@ namespace adn {
 // enc_L(v) = [v, sin(2^0 v), cos(2^0 v), ..., sin(2^(L-1) v), cos(2^(L-1) v)], each term a 3-vector
 // (src/util/feature_encoding.py:60-73).  Writes 3 + 6L floats.
 // The frequencies are powers of two, so sin / cos of 2^f v follow from those of 2^(f-1) v by the double-angle
-// identities (3 FMA-class ops instead of a ~40-instruction sincosf).  The rounding error doubles per step, so
-// an accurate sincosf re-anchors the recurrence every kAnchor octaves: the result stays within 2^(kAnchor-1)
-// ulp-class (<= ~2e-6 abs) of the directly evaluated value -- far inside the 2^f argument-rounding amplification
-// that the reference's own fp32 evaluation carries (SURVEY 8d: 5e-4 at 2^9).
+// identities (3 FMA-class ops instead of a ~40-instruction sincosf).  The error at least doubles per step, so an
+// accurate sincosf re-anchors the recurrence every kAnchor octaves.  Against float64 sin / cos the fourth step after an
+// anchor (bands 4 and 9) is off by up to ~4e-6 when the anchors are correctly rounded, and by up to 1.7e-5 when they
+// sit anywhere within sincosf's documented 2 ulp (per-band bounds: oracle/stage_emulation.py, recurrence_band_bounds)
+// -- still far inside the 2^f argument-rounding amplification that the reference's own fp32 evaluation carries
+// (SURVEY 8d: 5e-4 at 2^9).
 constexpr int kAnchor = 5;
 template <int L>
 __device__ __forceinline__ void posenc3(const float (&v)[3], float* out) {

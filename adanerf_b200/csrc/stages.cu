@@ -213,6 +213,14 @@ __device__ __forceinline__ int select_cells(const float4 v4, float thr, int K, i
   return need;
 }
 
+// Lane `lane`'s four cells of a 128-cell row: one 16-byte load when the rows are 16-byte aligned, else four 4-byte loads
+// (a float4 load from an address that is not a multiple of 16 faults).
+__device__ __forceinline__ float4 ld_row_quad(const float* __restrict__ row, int lane, bool aligned16) {
+  if (aligned16) return __ldg(reinterpret_cast<const float4*>(row) + lane);
+  const float* p = row + 4 * lane;
+  return make_float4(__ldg(p), __ldg(p + 1), __ldg(p + 2), __ldg(p + 3));
+}
+
 __device__ __forceinline__ unsigned long long ld_volatile_u64(const unsigned long long* p) {
   unsigned long long v;
   asm volatile("ld.volatile.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
@@ -309,7 +317,7 @@ stage2_kernel(const float* __restrict__ raw0, long long n_rays, float thr, const
               const float* __restrict__ zlut, int32_t* __restrict__ count, int32_t* __restrict__ offset,
               int32_t* __restrict__ cell_out, int32_t* __restrict__ ray_out, float* __restrict__ z_out,
               float* __restrict__ zp_out, long long* __restrict__ total, unsigned long long* __restrict__ tile_state,
-              unsigned int* __restrict__ ticket, int n_tiles, uint32_t epoch, uint32_t ticket_base) {
+              unsigned int* __restrict__ ticket, int n_tiles, uint32_t epoch, uint32_t ticket_base, bool aligned16) {
   __shared__ uint32_t s_sel[kS2Rays][4];
   __shared__ int s_cnt[kS2Rays];
   __shared__ int s_off[kS2Rays];
@@ -328,7 +336,7 @@ stage2_kernel(const float* __restrict__ raw0, long long n_rays, float thr, const
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
     const long long r = ray0 + warp * 8 + i;
-    rows8[i] = (r < n_rays) ? __ldg(reinterpret_cast<const float4*>(raw0 + r * 128) + lane) : make_float4(0.f, 0.f, 0.f, 0.f);
+    rows8[i] = (r < n_rays) ? ld_row_quad(raw0 + r * 128, lane, aligned16) : make_float4(0.f, 0.f, 0.f, 0.f);
   }
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
@@ -602,7 +610,7 @@ cudaError_t launch_stage2(const float* d_raw0, long long n_rays, float thr, int 
                                                                     d_ray, d_z, d_zp, d_total, state, ticket, n_tiles, epoch, base);
   else
     stage2_kernel<<<n_tiles, kS2Threads, 0, s>>>(d_raw0, n_rays, thr, d_thr, K, d_zlut, d_count, d_offset, d_cell, d_ray, d_z, d_zp,
-                                                 d_total, state, ticket, n_tiles, epoch, base);
+                                                 d_total, state, ticket, n_tiles, epoch, base, aligned);
   return cudaGetLastError();
 }
 

@@ -1,0 +1,331 @@
+"""fp32-FAITHFUL EMULATION OF THE SIMT STAGES -- TEST INFRASTRUCTURE, NOT PRODUCT CODE.
+
+`oracle/adanerf_oracle.py` restates the *reference* (torch fp32), which the kernels follow only up to the last ulp of a
+position (and so up to ~1e-4 on the 2^9 encoding band).  This module restates the *kernels* instead: stage 0
+(`stage0_kernel`), stage 3's per-sample inputs (`sample_inputs`), the positional encoding (`posenc3`) and both stage-5
+composites (`stage5_thread_kernel`, `stage5_warp_kernel`), operation for operation in numpy float32.  Every position
+operation of those kernels is an explicit round-to-nearest intrinsic or an fma in a fixed order, so the emulation gives
+the kernels' bits, and the GPU tests (`tests/test_stage_kernels_exact.py`) compare with `assert_array_equal`.
+
+What it cannot restate bit for bit is CUDA's `sincosf` and `expf`.  So `posenc3` either takes correctly rounded float64
+anchors or the kernel's own band-0 / band-5 outputs (then only the double-angle recurrence is emulated), and the
+composites take the sigmoid values as an input.
+
+numpy float32 ufuncs round every operation to nearest and never contract a multiply and an add, so `a * b + c` below is
+two roundings, exactly like `__fadd_rn(__fmul_rn(a, b), c)`.  Line numbers cite `adanerf_b200/csrc/`.
+"""
+import functools
+import math
+
+import numpy as np
+
+F32, F64 = np.float32, np.float64
+ANCHOR_EVERY = 5             # kAnchor (posenc.cuh:17)
+EPS_T = F32(1e-10)           # the 1e-10f of the transmittance factor (stages.cu:983,1035)
+
+
+def fma32(a, b, c):
+    """Correctly rounded fp32 fma(a, b, c).  The product of two fp32 values is exact in float64 (24 + 24 <= 53 bits); the
+    sum is rounded to odd in float64 (TwoSum gives the error term; an inexact sum is truncated toward zero and its last
+    bit set), then rounded to fp32.  Round-to-odd at 53 >= 24 + 2 bits followed by round-to-nearest equals one rounding
+    to nearest, so there is no double-rounding error."""
+    a64 = np.asarray(a, F32).astype(F64)
+    b64 = np.asarray(b, F32).astype(F64)
+    c64 = np.asarray(c, F32).astype(F64)
+    p = a64 * b64
+    s = p + c64
+    with np.errstate(invalid="ignore", over="ignore"):
+        bp = s - p
+        e = (p - (s - bp)) + (c64 - bp)
+        inexact = np.isfinite(s) & (e != 0)
+        away = inexact & ((e < 0) != (s < 0))          # s was rounded away from zero: truncate it
+    s = np.where(away, np.nextafter(s, 0.0), s)
+    s = (np.asarray(s, F64).view(np.uint64) | inexact.astype(np.uint64)).view(F64)
+    return s.astype(F32)
+
+
+def ulp32(y):
+    """fp32 ulp at |y| (the spacing of the fp32 value nearest to y)."""
+    return np.spacing(np.abs(np.asarray(y, F64)).astype(F32)).astype(F64)
+
+
+# ------------------------------------------------------------------------------------------------- scene constants
+def scene_constants(scene):
+    """The SceneDev values adn_create derives from a scene dict (api.cu:767-780, set_ndc_projection api.cu:420-424).  The
+    scene travels as fp32 fields (adn_scene), so every float is rounded to fp32 before the float64 work."""
+    size = [float(F32(v)) for v in scene["view_cell_size"]]
+    r2 = 0.0
+    for v in size:
+        r2 += (v / 2.0) * (v / 2.0)
+    r = math.sqrt(r2)
+    ndc = bool(scene.get("use_ndc"))
+    nfp0 = scene.get("n_freq_pos0") or (2 if ndc else scene.get("n_freq_pos", 10))
+    nfd0 = scene.get("n_freq_dir0") or (2 if ndc else scene.get("n_freq_dir", 4))
+    out = dict(c=np.asarray(scene["view_cell_center"], F32), r2=F32(r * r),
+               sqrt_max_depth=F32(math.sqrt(float(F32(scene["max_depth"])))), ndc=ndc, nfp0=int(nfp0), nfd0=int(nfd0),
+               ndc_cw=F32(0), ndc_ch=F32(0))
+    w, h = int(scene.get("w") or 0), int(scene.get("h") or 0)
+    if ndc and w > 0 and h > 0:
+        f_in = float(F32(scene.get("focal") or 0.0))
+        focal = f_in if f_in > 0 else 0.5 * float(w) / math.tan(0.5 * float(F32(scene["fov"])))
+        out["ndc_cw"] = F32(-1.0 / (float(w) / (2.0 * focal)))
+        out["ndc_ch"] = F32(-1.0 / (float(h) / (2.0 * focal)))
+    return out
+
+
+# ------------------------------------------------------------------------------------------------------- stage 0a
+def pixel_dir(W, H, fov, row0=0, rows=None):
+    """gen_dirs_kernel / pixel_dir (stages.cu:22-32) with camera_rays' float64 constants (api.cu:455-472): [rows*W, 3]."""
+    rows = H - row0 if rows is None else rows
+    fov = float(F32(fov))
+    focal = 0.5 * W / math.tan(0.5 * fov)
+    x_dist = math.tan(fov / 2) * focal
+    y_dist = x_dist * (float(H) / float(W))
+    x_pp, y_pp = x_dist / (W / 2.0), y_dist / (H / 2.0)
+    start_x, start_y = -(x_dist - x_pp / 2), -(y_dist - y_pp / 2)
+    rx = np.broadcast_to(start_x + x_pp * np.arange(W, dtype=F64), (rows, W))
+    ry = np.broadcast_to((start_y + y_pp * np.arange(row0, row0 + rows, dtype=F64))[:, None], (rows, W))
+    n = np.sqrt((rx * rx + ry * ry) + focal * focal)
+    d = np.stack([(rx / n).astype(F32), -(ry / n).astype(F32), -(focal / n).astype(F32)], -1)
+    return d.reshape(-1, 3)
+
+
+# ---------------------------------------------------------------------------------------------------- posenc3
+def posenc3(v, L, anchors=None, anchor_every=ANCHOR_EVERY):
+    """posenc3<L> (posenc.cuh:18-40): [..., 3] -> [..., 3 + 6L] = [v, sin 2^0 v, cos 2^0 v, ..., sin 2^(L-1) v, ...].
+    Bands f % 5 == 0 are anchors: with anchors=None the correctly rounded float64 sin / cos of the exact fp32 argument
+    v * 2^f; otherwise the columns of `anchors` (the kernel's own [..., 3 + 6L] block), so that only the recurrence is
+    emulated.  Every other band is the double-angle step from the band below: s' = (2s) c (2s is exact), c' = fma(-2s, s, 1).
+    anchor_every: the anchor spacing (a larger value removes the band-5 anchor; only the teeth tests change it)."""
+    v = np.asarray(v, F32)
+    out = np.empty(v.shape[:-1] + (3 + 6 * L,), F32)
+    out[..., :3] = v
+    s = c = None
+    for f in range(L):
+        lo = 3 + 6 * f
+        if f % anchor_every == 0:
+            if anchors is None:
+                x = (v * F32(2.0 ** f)).astype(F64)
+                s, c = np.sin(x).astype(F32), np.cos(x).astype(F32)
+            else:
+                s, c = np.asarray(anchors[..., lo:lo + 3], F32), np.asarray(anchors[..., lo + 3:lo + 6], F32)
+        else:
+            s, c = (F32(2) * s) * c, fma32(F32(-2) * s, s, F32(1))
+        out[..., lo:lo + 3] = s
+        out[..., lo + 3:lo + 6] = c
+    return out
+
+
+def posenc_f64(v, L):
+    """The encoding evaluated in float64 on the exact fp32 inputs (the reference every band's error is measured against)."""
+    v = np.asarray(v, F32).astype(F64)
+    out = np.empty(v.shape[:-1] + (3 + 6 * L,), F64)
+    out[..., :3] = v
+    for f in range(L):
+        out[..., 3 + 6 * f:6 + 6 * f] = np.sin(v * 2.0 ** f)
+        out[..., 6 + 6 * f:9 + 6 * f] = np.cos(v * 2.0 ** f)
+    return out
+
+
+@functools.lru_cache(maxsize=None)
+def recurrence_band_bounds(L=10, n_args=1 << 17, max_ulps=2, seed=0):
+    """Per band f: the largest |posenc3 - float64| over n_args fp32 arguments in [-4, 4] (more than a turn of every
+    anchor angle) when each anchor value, sin and cos independently, is any fp32 value within max_ulps ulp of the
+    correctly rounded one -- everything posenc3 can return while sincosf keeps its documented 2-ulp bound (CUDA C++
+    Programming Guide, single-precision mathematical functions).  Bands f and f +- 5 see the same recurrence, so each
+    takes the larger of the two.  Returns a float64 array [L]."""
+    rng = np.random.default_rng(seed)
+    x = rng.uniform(-4.0, 4.0, n_args).astype(F32)
+    steps = range(-max_ulps, max_ulps + 1)
+    worst = np.zeros(L, F64)
+    for f0 in range(0, L, ANCHOR_EVERY):
+        arg = x * F32(2.0 ** f0)
+        a64 = arg.astype(F64)
+        s0, c0 = np.sin(a64).astype(F32), np.cos(a64).astype(F32)
+        s_opts = [_nudge(s0, k) for k in steps]
+        c_opts = [_nudge(c0, k) for k in steps]
+        s = np.concatenate([so for so in s_opts for _ in c_opts])
+        c = np.concatenate([co for _ in s_opts for co in c_opts])
+        ref = np.tile(a64, len(s_opts) * len(c_opts))
+        for f in range(f0, min(L, f0 + ANCHOR_EVERY)):
+            if f > f0:
+                s, c = (F32(2) * s) * c, fma32(F32(-2) * s, s, F32(1))
+            r = ref * 2.0 ** (f - f0)
+            worst[f] = max(np.abs(s - np.sin(r)).max(), np.abs(c - np.cos(r)).max())
+    for f in range(L):
+        for g in (f - ANCHOR_EVERY, f + ANCHOR_EVERY):
+            if 0 <= g < L:
+                worst[f] = max(worst[f], worst[g])
+    return worst
+
+
+def _nudge(x, k):
+    """x moved by k fp32 ulps."""
+    x = np.asarray(x, F32)
+    for _ in range(abs(k)):
+        x = np.nextafter(x, F32(np.inf) if k > 0 else F32(-np.inf))
+    return x
+
+
+# ------------------------------------------------------------------------------------------------------- stage 0b
+def _dot3(a, b):
+    """((a0 b0 + a1 b1) + a2 b2), every operation rounded (stages.cu:80-81,87)."""
+    return (a[..., 0] * b[..., 0] + a[..., 1] * b[..., 1]) + a[..., 2] * b[..., 2]
+
+
+def rotate(rot, dirs):
+    """nds = R d as the FMA chain fma(R[r,2], d2, fma(R[r,1], d1, R[r,0] d0)) (stages.cu:73-75)."""
+    R = np.asarray(rot, F32).reshape(9)
+    d = np.asarray(dirs, F32).reshape(-1, 3)
+    return np.stack([fma32(R[3 * r + 2], d[:, 2], fma32(R[3 * r + 1], d[:, 1], R[3 * r] * d[:, 0])) for r in range(3)], -1)
+
+
+def sphere_delta(pose, nds, scene):
+    """compute_ray_offset's discriminant delta = udot^2 - (|o - c|^2 - r^2) (stages.cu:79-82); <= 0 is clamped to 0."""
+    k = scene_constants(scene)
+    omc = np.asarray(pose, F32).reshape(3) - k["c"]
+    udot = _dot3(omc[None, :], nds)
+    return udot, udot * udot - (_dot3(omc, omc) - k["r2"])
+
+
+def stage0(pose, rot, dirs, scene, nfd=None, nfp=None, contract=False):
+    """stage0_kernel<false, NFD, NFP> (stages.cu:52-111) -> (ray_o [N,3], ray_d [N,3], x0 [N, 6 + 6 (NFD + NFP)]) with the
+    direction block first.  nfd / nfp default to the scene's sampling-net encoding ("10-4", or "2-2" with NDC).
+    contract=True evaluates p = pose + nds t as one fma (a kernel the compiler was allowed to contract; teeth tests)."""
+    k = scene_constants(scene)
+    nfd = k["nfd0"] if nfd is None else nfd
+    nfp = k["nfp0"] if nfp is None else nfp
+    pose = np.asarray(pose, F32).reshape(3)
+    nds = rotate(rot, dirs)
+    udot, delta = sphere_delta(pose, nds, scene)
+    t = -udot + np.sqrt(np.fmax(delta, F32(0)))                                  # :83
+    if contract:
+        p = np.stack([fma32(nds[:, a], t, pose[a]) for a in range(3)], -1)
+    else:
+        p = pose[None, :] + nds * t[:, None]                                    # :86
+    nn = np.sqrt(_dot3(nds, nds))                                               # :87
+    dn = nds / nn[:, None]                                                      # :90
+    x0 = np.concatenate([posenc3(dn, nfd), posenc3(p, nfp)], -1)                 # :91-92
+    return p, nds, x0
+
+
+# -------------------------------------------------------------------------------------------------------- stage 3
+def sample_inputs(scene, ray_o, ray_d, ray_idx, z, contract=False):
+    """sample_inputs (posenc.cuh:45-84) for samples (ray_idx, z) -> (pos [M,3], dir [M,3]): the NDC branch (ndc_rays with
+    near = 1, un-normalised position, direction d' / |d'|) or pos - c over sqrt(max_depth) sqrt|pos - c| with the raw
+    direction.  contract=True fuses o + d z into one fma (teeth tests)."""
+    k = scene_constants(scene)
+    r = np.asarray(ray_idx, np.int64)
+    o = np.asarray(ray_o, F32).reshape(-1, 3)[r]
+    d = np.asarray(ray_d, F32).reshape(-1, 3)[r]
+    zw = np.asarray(z, F32)
+    if k["ndc"]:
+        cw, ch = k["ndc_cw"], k["ndc_ch"]
+        t = -(F32(1) + o[:, 2]) / d[:, 2]                                        # :57
+        on = o + t[:, None] * d                                                  # :60
+        q0, q1 = on[:, 0] / on[:, 2], on[:, 1] / on[:, 2]
+        o0, o1 = (cw * on[:, 0]) / on[:, 2], (ch * on[:, 1]) / on[:, 2]
+        o2 = F32(1) + F32(2) / on[:, 2]
+        d0 = cw * (d[:, 0] / d[:, 2] - q0)
+        d1 = ch * (d[:, 1] / d[:, 2] - q1)
+        d2 = F32(-2) / on[:, 2]
+        oo, dd = np.stack([o0, o1, o2], -1), np.stack([d0, d1, d2], -1)
+        pos = fma32(dd, zw[:, None], oo) if contract else oo + dd * zw[:, None]  # :68-70
+        dn = np.sqrt(_dot3(dd, dd))                                              # :71
+        return pos, dd / dn[:, None]                                             # :72-74
+    pos = (fma32(d, zw[:, None], o) if contract else o + d * zw[:, None]) - k["c"][None, :]   # :77
+    nrm = np.sqrt(_dot3(pos, pos))                                               # :79
+    den = k["sqrt_max_depth"] * np.sqrt(nrm)                                     # :80
+    with np.errstate(invalid="ignore", divide="ignore"):
+        return pos / den[:, None], d                                             # :82
+
+
+def stage3(scene, ray_o, ray_d, ray_idx, z):
+    """stage3_kernel's x1 [M, 90] (stages.cu:869-898) with float64 anchors: the position block (10 bands) first."""
+    pos, d = sample_inputs(scene, ray_o, ray_d, ray_idx, z)
+    with np.errstate(invalid="ignore"):
+        return np.concatenate([posenc3(pos, 10), posenc3(d, 4)], -1)
+
+
+# -------------------------------------------------------------------------------------------------------- stage 5
+def _gather(a, idx, live, fill=0):
+    a = np.asarray(a)
+    if a.shape[0] == 0:
+        return np.full(idx.shape + a.shape[1:], fill, a.dtype)
+    return a[np.where(live, idx, 0)]
+
+
+def stage5_thread(sig, zp, z, offset, count, K, eps=EPS_T):
+    """stage5_thread_kernel (stages.cu:954-1008) on sigmoid values sig [M,4] (rgb, alpha): per ray the sequential chain
+    alpha = s_a zp, w = alpha T, T = T ((1 - alpha) + 1e-10), c += w s, depth += w z.  -> dict(rgb [N,3], weights [N,K]
+    zero padded, depth_map [N]).  eps: the 1e-10 term (teeth tests drop it)."""
+    sig, zp, z = np.asarray(sig, F32), np.asarray(zp, F32), np.asarray(z, F32)
+    off, cnt = np.asarray(offset, np.int64), np.asarray(count, np.int64)
+    n = cnt.shape[0]
+    T = np.ones(n, F32)
+    acc = np.zeros((n, 4), F32)          # r, g, b, depth
+    w_out = np.zeros((n, K), F32)
+    with np.errstate(invalid="ignore", over="ignore"):
+        for j in range(K):
+            live = j < cnt
+            if not live.any():
+                break
+            idx = off + j
+            s = _gather(sig, idx, live)
+            a = s[:, 3] * _gather(zp, idx, live)
+            w = a * T
+            T = np.where(live, T * ((F32(1) - a) + eps), T)
+            terms = np.concatenate([w[:, None] * s[:, :3], (w * _gather(z, idx, live))[:, None]], -1)
+            acc = np.where(live[:, None], acc + terms, acc)
+            w_out[:, j] = np.where(live, w, F32(0))
+    return dict(rgb=acc[:, :3].copy(), weights=w_out, depth_map=acc[:, 3].copy())
+
+
+def stage5_warp(sig, zp, z, offset, count, K, eps=EPS_T, tree=True):
+    """stage5_warp_kernel, non-dense (stages.cu:1012-1082), as lane 0 ends it: per 32-sample block a Hillis-Steele
+    inclusive product scan of f = (1 - alpha) + 1e-10 (lane l multiplies in lane l - o's value, o = 1, 2, 4, 8, 16), T =
+    carry * (exclusive product), w = alpha T, carry *= the block's product; each lane sums its own w s / w z over the
+    blocks, then an xor butterfly (o = 16 ... 1) adds the lanes.  Lanes past the ray's count take alpha = s = z = 0.
+    tree=False takes T as the sequential product instead (teeth tests)."""
+    sig, zp, z = np.asarray(sig, F32), np.asarray(zp, F32), np.asarray(z, F32)
+    off, cnt = np.asarray(offset, np.int64), np.asarray(count, np.int64)
+    n = cnt.shape[0]
+    lanes = np.arange(32)
+    carry = np.ones(n, F32)
+    acc = np.zeros((n, 32, 5), F32)      # per lane: r, g, b, depth, acc
+    w_out = np.zeros((n, K), F32)
+    with np.errstate(invalid="ignore", over="ignore"):
+        for j0 in range(0, int(cnt.max(initial=0)), 32):
+            run = j0 < cnt                                               # rays whose loop reaches this block
+            j = j0 + lanes[None, :]
+            live = j < cnt[:, None]
+            idx = off[:, None] + j
+            s = np.where(live[..., None], _gather(sig, idx, live), F32(0))
+            alpha = np.where(live, s[..., 3] * _gather(zp, idx, live), F32(0))
+            zz = np.where(live, _gather(z, idx, live), F32(0))
+            f = (F32(1) - alpha) + eps
+            if tree:
+                p = f.copy()
+                for o in (1, 2, 4, 8, 16):
+                    p[:, o:] = p[:, o:] * p[:, :-o]
+            else:
+                p = np.empty_like(f)
+                p[:, 0] = f[:, 0]
+                for l in range(1, 32):
+                    p[:, l] = p[:, l - 1] * f[:, l]
+            excl = np.concatenate([np.ones((n, 1), F32), p[:, :31]], 1)
+            T = carry[:, None] * excl
+            w = alpha * T
+            terms = np.stack([w * s[..., 0], w * s[..., 1], w * s[..., 2], w * zz, w], -1)
+            acc = np.where(run[:, None, None], acc + terms, acc)
+            carry = np.where(run, carry * p[:, 31], carry)
+            inside = j0 + lanes < K
+            w_out[:, j0 + lanes[inside]] = np.where(live & run[:, None], w, F32(0))[:, inside]
+        for o in (16, 8, 4, 2, 1):
+            acc = acc + acc[:, lanes ^ o]
+    return dict(rgb=acc[:, 0, :3].copy(), weights=w_out, depth_map=acc[:, 0, 3].copy())
+
+
+def stage5(sig, zp, z, offset, count, K):
+    """The composite launch_stage5 picks for a packed (non-dense) call (stages.cu:1090): the warp kernel when K > 32."""
+    return (stage5_warp if K > 32 else stage5_thread)(sig, zp, z, offset, count, K)

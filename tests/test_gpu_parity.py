@@ -97,6 +97,17 @@ def test_generate_ray_directions_bit_exact(bare):
     np.testing.assert_array_equal(band, ref[300 * W:307 * W])
 
 
+@pytest.mark.parametrize("W,H,row0,rows", [(1, 1, 0, 1), (3, 801, 400, 1), (801, 799, 798, 1), (1920, 1080, 517, 64)])
+def test_generate_ray_directions_frame_sizes(bare, W, H, row0, rows):
+    """Other frame sizes (a single pixel, odd and non-square frames, 1080p): the whole frame and the band
+    [row0, row0 + rows) (what one tile of a multi-GPU frame generates), bit for bit."""
+    d = bare.generate_ray_directions(W, H, row0=0, rows=H).cpu().numpy()
+    ref = orc.generate_ray_directions(W, H, orc.SCENE_BARBERSHOP["fov"]).reshape(-1, 3).astype(np.float32)
+    np.testing.assert_array_equal(d, ref)
+    band = bare.generate_ray_directions(W, H, row0=row0, rows=rows).cpu().numpy()
+    np.testing.assert_array_equal(band, ref[row0 * W:(row0 + rows) * W])
+
+
 @pytest.mark.parametrize("case", CASES)
 def test_stage0_matches_reference(case):
     g = load_golden(case)
@@ -154,19 +165,50 @@ def test_stage2_bit_exact_on_reference_raw0(case, bare):
     r.close()
 
 
+def _stage2_adversarial(n=64 * 5 + 37):
+    """Rows built from the values selection can get wrong: -0.0 against +0.0 ties, denormals, +-inf, values equal to a
+    threshold and one ulp either side of it; some rows are nothing but one such value.  n is not a multiple of the 64-ray
+    tile."""
+    rng = np.random.default_rng(12)
+    f = np.float32
+    t2, t5 = f(0.2), f(0.5)
+    special = np.array([0.0, -0.0, 2.0 ** -149, -(2.0 ** -149), 3 * 2.0 ** -149, 2.0 ** -126, 1e-40, np.inf, -np.inf,
+                        t2, np.nextafter(t2, f(1)), np.nextafter(t2, f(0)), t5, np.nextafter(t5, f(1)), np.nextafter(t5, f(0)),
+                        -t2, 1.0, -1.0], f)
+    raw = rng.choice(special, (n, 128))
+    mixed = rng.random((n, 128)) < 0.5
+    raw[mixed] = rng.uniform(-0.5, 0.7, int(mixed.sum())).astype(f)
+    for i, v in enumerate(special):                      # single-valued rows (every cell ties)
+        raw[i] = v
+    raw[len(special)] = np.where(np.arange(128) % 2 == 0, f(-0.0), f(0.0))
+    raw[len(special) + 1] = np.where(np.arange(128) % 3 == 0, f(np.inf), f(-np.inf))
+    return torch.from_numpy(raw)
+
+
 def test_stage2_stress_vectors(bare):
-    """Ties, all-equal rows, value == thr, nothing above thr ... against the oracle (ties lower-cell-first)."""
+    """Ties, all-equal rows, value == thr, nothing above thr, signed zeros, denormals, infinities ... against the oracle
+    (ties lower-cell-first) at every K: <= 8 / <= 16 the two thread-per-ray kernels, above the warp-per-ray kernel.  At
+    K <= 16 a raw0 that is only 4-byte aligned (the warp kernel's fallback) gives the same result as the aligned one."""
     g = load_golden("stage2_stress")
-    raw0 = torch.from_numpy(g["raw0"])
     dr = g["meta"]["depth_range"]
-    for K in (1, 4, 8, 16, 32, 64, 128):   # <= 16: thread-per-ray kernel, above: warp-per-ray kernel, 128: dense
-        for thr in (0.2, 0.5):
-            s2 = bare.stage2(raw0.cuda(), thr, K)
-            o2 = orc.stage2_sample(raw0, thr, K, dr)
-            mask = torch.isfinite(o2["z"]).numpy()
-            np.testing.assert_array_equal(s2["count"].cpu().numpy(), o2["count"].numpy())
-            np.testing.assert_array_equal(s2["cell"].cpu().numpy(), o2["cell"].numpy()[mask])
-            np.testing.assert_array_equal(s2["zp"].cpu().numpy(), o2["zp"].numpy()[mask])
+    sets = [(torch.from_numpy(g["raw0"]), (0.2, 0.5)), (_stage2_adversarial(), (0.2, 0.5, 3 * 2.0 ** -149))]
+    for raw0, thrs in sets:
+        n = raw0.shape[0]
+        shifted = torch.empty(n * 128 + 1, dtype=torch.float32, device="cuda")[1:].view(n, 128)
+        shifted.copy_(raw0)
+        assert shifted.data_ptr() % 16 == 4
+        for K in range(1, 129):
+            for thr in thrs:
+                s2 = bare.stage2(raw0.cuda(), thr, K)
+                o2 = orc.stage2_sample(raw0, thr, K, dr)
+                mask = torch.isfinite(o2["z"]).numpy()
+                np.testing.assert_array_equal(s2["count"].cpu().numpy(), o2["count"].numpy(), err_msg=f"K={K} thr={thr}")
+                np.testing.assert_array_equal(s2["cell"].cpu().numpy(), o2["cell"].numpy()[mask], err_msg=f"K={K} thr={thr}")
+                np.testing.assert_array_equal(s2["zp"].cpu().numpy(), o2["zp"].numpy()[mask], err_msg=f"K={K} thr={thr}")
+                if K <= 16:
+                    s2m = bare.stage2(shifted, thr, K)
+                    for k in ("count", "offset", "cell", "ray", "z", "zp"):
+                        assert torch.equal(s2m[k], s2[k]), (K, thr, k)
 
 
 def test_stage2_large_properties(bare):
