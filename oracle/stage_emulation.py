@@ -7,6 +7,10 @@ composites (`stage5_thread_kernel`, `stage5_warp_kernel`), operation for operati
 operation of those kernels is an explicit round-to-nearest intrinsic or an fma in a fixed order, so the emulation gives
 the kernels' bits, and the GPU tests (`tests/test_stage_kernels_exact.py`) compare with `assert_array_equal`.
 
+For stage 2 it restates the host side bit for bit: the 128-entry adaptive depth table `adn_create` uploads (`zlut`) and
+the dense table of `ensure_dense_lut` (`zlut_dense`); `stage2_packed` turns the oracle's selection into the kernels'
+packed buffers.
+
 What it cannot restate bit for bit is CUDA's `sincosf` and `expf`.  So `posenc3` either takes correctly rounded float64
 anchors or the kernel's own band-0 / band-5 outputs (then only the double-angle recurrence is emulated), and the
 composites take the sigmoid values as an input.
@@ -71,6 +75,57 @@ def scene_constants(scene):
         out["ndc_cw"] = F32(-1.0 / (float(w) / (2.0 * focal)))
         out["ndc_ch"] = F32(-1.0 / (float(h) / (2.0 * focal)))
     return out
+
+
+# ------------------------------------------------------------------------------------------------- depth tables
+def _to_world(z, scene):
+    """LogTransform.to_world as adn_create / ensure_dense_lut evaluate it: pow in float64 on max_v = dr1 - dr0 (the fp32
+    scene fields widened), rounded to fp32, then (w - 1) + dr0 in fp32.  NDC scenes (FromClassifiedDepthAdaptiveNoDepthRange)
+    keep z itself."""
+    z = np.asarray(z, F32)
+    if scene.get("use_ndc"):
+        return z.copy()
+    dr0, dr1 = F32(scene["depth_range"][0]), F32(scene["depth_range"][1])
+    base = (float(dr1) - float(dr0)) + 1.0
+    w = np.array([math.pow(base, float(v)) for v in z], F64).astype(F32)
+    return (w - F32(1)) + dr0
+
+
+def zlut(scene):
+    """The adaptive depth table (api.cu:781-789): cell centres (i + 0.5) * (1 / 128) in fp32, then _to_world.  [128] fp32."""
+    return _to_world((np.arange(128, dtype=F32) + F32(0.5)) * F32(1.0 / 128.0), scene)
+
+
+def linspace01(K):
+    """torch.linspace(0, 1, K + 1) in fp32 as ATen evaluates it (symmetric: k * step below the half-way index, 1 - (K - k)
+    * step from it on, step = 1 / K) -- the lin of api.cu:433-434.  [K + 1] fp32."""
+    step = F32(1) / F32(K)
+    k = np.arange(K + 1)
+    return np.where(k < (K + 1) // 2, k.astype(F32) * step, F32(1) - (K - k).astype(F32) * step).astype(F32)
+
+
+def zlut_dense(scene, K):
+    """The dense table of ensure_dense_lut (api.cu:426-439): t = linspace01(K)[:K] + fp32(0.5 / K), z = z_near (1 - t) +
+    z_far t in fp32, then _to_world.  [K] fp32."""
+    t = linspace01(K)[:K] + F32(0.5 / K)
+    near, far = F32(scene.get("z_near", 0.001)), F32(scene.get("z_far", 1.0))
+    return _to_world(near * (F32(1) - t) + far * t, scene)
+
+
+# ------------------------------------------------------------------------------------------------------- stage 2
+def stage2_packed(sel, lut):
+    """The packed buffers of stage 2 (stage2_kernel / stage2_thread_kernel, stages.cu) from the selection of
+    orc.stage2_sample (`sel`: count [N], cell [N,K] ascending, -1 padded, zp [N,K]): ray-major, cells ascending inside a ray.
+    -> dict(count [N], offset [N], total, ray [M], cell [M], zp [M], z [M] = lut[cell]); int32 / fp32 like the kernels'."""
+    cell = np.asarray(sel["cell"])
+    live = cell >= 0
+    count = live.sum(1).astype(np.int32)
+    assert np.array_equal(count, np.asarray(sel["count"])), "stage2_packed: counts disagree with the selection"
+    offset = (np.cumsum(count, dtype=np.int64) - count).astype(np.int32)
+    c = cell[live].astype(np.int32)
+    return dict(count=count, offset=offset, total=int(count.sum()),
+                ray=np.repeat(np.arange(cell.shape[0], dtype=np.int32), count), cell=c,
+                zp=np.asarray(sel["zp"], F32)[live], z=np.asarray(lut, F32)[c])
 
 
 # ------------------------------------------------------------------------------------------------------- stage 0a

@@ -176,6 +176,110 @@ def test_stage5_emulation_matches_the_oracle_at_k128():
     np.testing.assert_allclose(out["depth_map"], ref["depth_map"].numpy(), rtol=0, atol=2e-5)
 
 
+# ------------------------------------------------------------------------------------------------- depth tables
+LOG_SCENES = {"barbershop": orc.SCENE_BARBERSHOP, "pavillon": orc.SCENE_PAVILLON}
+
+
+def _world64(z, scene):
+    """LogTransform.to_world in float64 on the fp32 scene fields and the exact fp32 z; also returns w = the power."""
+    dr0, dr1 = float(F32(scene["depth_range"][0])), float(F32(scene["depth_range"][1]))
+    w = (dr1 - dr0 + 1.0) ** np.asarray(z, F32).astype(np.float64)
+    return (w - 1.0) + dr0, w
+
+
+def _dense_z(K):
+    t = se.linspace01(K)[:K] + F32(0.5 / K)
+    return F32(0.001) * (F32(1) - t) + F32(1.0) * t
+
+
+@pytest.mark.parametrize("name", sorted(LOG_SCENES))
+def test_depth_tables_within_an_ulp_of_float64(name):
+    """Both tables are within 1 ulp of the power w = (max_v + 1)^z of the float64 formula: pow is correctly rounded (up to
+    glibc's < 1 ulp), (w - 1) and + dr0 add one rounding each.  Relative to the table value itself the error is larger where
+    (w - 1) + dr0 cancels: Barbershop's dr0 = -0.43 puts a zero crossing inside the table."""
+    scene = LOG_SCENES[name]
+    cells = (np.arange(128, dtype=F32) + F32(0.5)) * F32(1.0 / 128.0)
+    for lut, z in ((se.zlut(scene), cells), (se.zlut_dense(scene, 128), _dense_z(128))):
+        ref, w = _world64(z, scene)
+        err = np.abs(lut.astype(np.float64) - ref)
+        assert (err <= se.ulp32(w)).all(), (err / se.ulp32(w)).max()
+        print(f"{name}: max {float((err / se.ulp32(w)).max()):.3f} ulp of w, {float((err / se.ulp32(ref)).max()):.1f} ulp of the value")
+
+
+@pytest.mark.parametrize("name", sorted(LOG_SCENES))
+def test_depth_tables_against_the_oracle(name):
+    """The oracle evaluates to_world in fp32 torch (pow included), so it is not the kernels' table: both are within 4 ulp of
+    w of each other (absolute <= 4.8e-7 on Barbershop, 1.9e-6 on Pavillon).  Near Barbershop's zero crossing that is up to
+    64 ulp of the value (fp32 cancellation in (w - 1) + dr0), so the bound is absolute, in units of w."""
+    scene = LOG_SCENES[name]
+    cells = (np.arange(128, dtype=F32) + F32(0.5)) * F32(1.0 / 128.0)
+    oracle_dense = orc.stage2_sample(torch.zeros(1, 128), 0.0, 128, scene["depth_range"])["z"].numpy()[0]
+    for lut, z, o in ((se.zlut(scene), cells, orc.log_to_world(torch.from_numpy(cells), scene["depth_range"]).numpy()),
+                      (se.zlut_dense(scene, 128), _dense_z(128), oracle_dense)):
+        _, w = _world64(z, scene)
+        err = np.abs(lut.astype(np.float64) - o)
+        assert (err <= 4 * se.ulp32(w)).all(), (err / se.ulp32(w)).max()
+        assert err.max() <= 2e-6
+
+
+def test_ndc_depth_tables_are_the_cell_centres():
+    """FromClassifiedDepthAdaptiveNoDepthRange: the adaptive table is the cell centre itself, the dense one the lerp."""
+    z = se.zlut(orc.SCENE_PAVILLON_NDC)
+    np.testing.assert_array_equal(z, (np.arange(128, dtype=F32) + F32(0.5)) * F32(1.0 / 128.0))
+    assert np.array_equal(z, orc.stage2_sample(torch.ones(1, 128), 0.5, 128, None, no_depth_range=True)["z"].numpy()[0])
+    dense = orc.stage2_sample(torch.zeros(1, 128), 0.0, 128, None, no_depth_range=True)["z"].numpy()[0]
+    np.testing.assert_array_equal(se.zlut_dense(orc.SCENE_PAVILLON_NDC, 128).view(np.uint32), dense.view(np.uint32))
+
+
+def test_linspace_is_atens_rule():
+    """linspace01 is ATen's per-element linspace rule (k * step below the half-way index, 1 - (K - k) * step from it).
+    torch's vectorised CPU kernel continues a lane chunk that starts below the half-way index with k * step past it, so
+    where 1 / K is inexact it can differ by 1 ulp; where 1 / K is a power of two every term is exact and the two agree bit
+    for bit -- K = 128 among them, the only K dense mode takes."""
+    for K in range(1, 257):
+        ours = se.linspace01(K)
+        ref = torch.linspace(0, 1, K + 1).numpy()
+        diff = np.abs(ours.view(np.int32).astype(np.int64) - ref.view(np.int32))
+        assert diff.max() <= 1, K
+        if K & (K - 1) == 0:
+            np.testing.assert_array_equal(ours.view(np.uint32), ref.view(np.uint32), err_msg=f"K={K}")
+        assert ours[0] == 0 and ours[-1] == 1 and (np.diff(ours) > 0).all(), K
+    K = 9                                       # the rule itself, written out once: ATen's symmetric evaluation
+    step = F32(1) / F32(K)
+    want = [F32(k) * step if k < 5 else F32(1) - F32(K - k) * step for k in range(K + 1)]
+    np.testing.assert_array_equal(se.linspace01(K), np.array(want, F32))
+
+
+def test_teeth_powf_depth_table():
+    """A table built with powf on the fp32 base (instead of pow in double) differs from zlut in at least one cell of each
+    shipped scene, so the GPU tests that compare z with zlut bit for bit catch it."""
+    cells = (np.arange(128, dtype=F32) + F32(0.5)) * F32(1.0 / 128.0)
+    for scene in LOG_SCENES.values():
+        dr0, dr1 = F32(scene["depth_range"][0]), F32(scene["depth_range"][1])
+        base = F32((float(dr1) - float(dr0)) + 1.0)
+        bad = (np.power(base, cells, dtype=F32) - F32(1)) + dr0
+        n = int((bad != se.zlut(scene)).sum())
+        print(f"powf table: {n} of 128 cells differ")
+        assert n >= 1
+
+
+def test_stage2_packed_view_of_the_golden_cases():
+    """stage2_packed on the oracle's selection is the golden cases' packed samples, and its z the golden z up to the
+    to_world difference above."""
+    for case in ("pav_k8_t0.2", "pav_k16_t0.15", "rand_k8_t0.2"):
+        g = load_golden(case)
+        m = g["meta"]
+        scene = m["scene_params"]
+        p = se.stage2_packed(orc.stage2_sample(torch.from_numpy(g["raw0"]), m["thr"], m["K"], scene["depth_range"]),
+                             se.zlut(scene))
+        mask = np.isfinite(g["z_nan"])
+        np.testing.assert_array_equal(p["count"], mask.sum(1))
+        np.testing.assert_array_equal(p["offset"], np.cumsum(mask.sum(1)) - mask.sum(1))
+        np.testing.assert_array_equal(p["ray"], np.nonzero(mask)[0])
+        np.testing.assert_allclose(p["z"], g["z_nan"][mask], rtol=0, atol=2e-6)
+        assert p["total"] == mask.sum() and p["ray"].dtype == np.int32 and p["z"].dtype == F32
+
+
 # -------------------------------------------------------------------------------------------- posenc band bounds
 def test_posenc_from_exact_anchors_is_within_the_band_bounds():
     """posenc3 from correctly rounded anchors stays inside the per-band bounds the kernel tests apply; the bound table is
