@@ -1103,19 +1103,32 @@ adn_status adn_mlp1_forward(adn_ctx* ctx, const float* d_x1, int64_t n_samples, 
   return run_mlp(ctx, 1, static_cast<uint8_t*>(ctx->tiles1.p), d_raw1, nullptr, n_samples, st);
 }
 
+adn_status adn_stage5_composite_aux(adn_ctx* ctx, const float* d_raw1, const float* d_zp, const float* d_z,
+                                    const int32_t* d_offset, const int32_t* d_count, int64_t n_rays, int K, int dense,
+                                    float* d_rgb, uint8_t* d_rgba8, const adn_aux_outputs* aux, void* stream) {
+  const adn_aux_outputs a = aux ? *aux : adn_aux_outputs{};
+  const bool reads_z = a.d_z_vals || a.d_depth_map || a.d_disp_map || a.d_depth_est;
+  if (!ctx || n_rays < 0 || K < 1 || K > 128 || (dense && K != 128))
+    return fail(ctx, ADN_ERR_INVALID, "stage5: bad arguments (dense mode needs K == 128)");
+  if (n_rays > 0 && (!d_raw1 || !d_zp || (!dense && (!d_offset || !d_count || (reads_z && !d_z)))))
+    return fail(ctx, ADN_ERR_INVALID, "stage5: bad arguments");
+  ADN_CUDA(ctx, cudaSetDevice(ctx->device));
+  adn_status s;
+  if (dense && (s = ensure_dense_lut(ctx, K)) != ADN_OK) return s;
+  ADN_CUDA(ctx, launch_stage5(d_raw1, d_zp, dense ? nullptr : d_z, ctx->zlut_dense.as<float>(), dense ? nullptr : d_offset,
+                              d_count, n_rays, K, dense, d_rgb, d_rgba8, stage5_aux(ctx, a), static_cast<cudaStream_t>(stream)));
+  ctx->stats.kernel_launches++;
+  return ADN_OK;
+}
+
 adn_status adn_stage5_composite(adn_ctx* ctx, const float* d_raw1, const float* d_zp, const float* d_z, const int32_t* d_offset,
                                 const int32_t* d_count, int64_t n_rays, int K, float* d_rgb, float* d_weights,
                                 float* d_depth_map, void* stream) {
-  if (!ctx || !d_raw1 || !d_zp || !d_offset || !d_count || !d_rgb || n_rays < 0 || K < 1 || K > 128 || (d_depth_map && !d_z))
-    return fail(ctx, ADN_ERR_INVALID, "stage5: bad arguments");
-  ADN_CUDA(ctx, cudaSetDevice(ctx->device));
-  Stage5Aux aux;
-  aux.weights = d_weights;
-  aux.depth_map = d_depth_map;
-  ADN_CUDA(ctx, launch_stage5(d_raw1, d_zp, d_z, nullptr, d_offset, d_count, n_rays, K, 0, d_rgb, nullptr, aux,
-                              static_cast<cudaStream_t>(stream)));
-  ctx->stats.kernel_launches++;
-  return ADN_OK;
+  if (!d_rgb) return fail(ctx, ADN_ERR_INVALID, "stage5: bad arguments");
+  adn_aux_outputs aux{};
+  aux.d_weights = d_weights;
+  aux.d_depth_map = d_depth_map;
+  return adn_stage5_composite_aux(ctx, d_raw1, d_zp, d_z, d_offset, d_count, n_rays, K, 0, d_rgb, nullptr, &aux, stream);
 }
 
 adn_status adn_image_metrics(adn_ctx* ctx, const float* d_image, const float* d_reference, int64_t n_values, int clamp01,

@@ -137,10 +137,12 @@ int main(int argc, char** argv) {
     cudaDeviceSynchronize();
     std::vector<unsigned char> px(size_t(W) * H * 4);
     if (cudaMemcpy2DFromArray(px.data(), size_t(W) * 4, arr, 0, 0, size_t(W) * 4, size_t(H), cudaMemcpyDeviceToHost) != cudaSuccess) { std::fprintf(stderr, "readback failed\n"); return 1; }
-    size_t bad = 0;   // rgb holds the same camera's fp32 frame (last loop iteration): clamp * 255, alpha 255
+    // rgb holds the same camera's fp32 frame (last loop iteration): saturate(x) * 255 truncated, alpha 255 -- the
+    // viewer's clamp as nvcc compiles it (FADD.SAT: NaN -> 0)
+    size_t bad = 0;
     for (size_t i = 0; i < size_t(W) * H; ++i) {
       for (int c = 0; c < 3; ++c) {
-        const float v = rgb[3 * i + c] < 0.f ? 0.f : (rgb[3 * i + c] > 1.f ? 1.f : rgb[3 * i + c]);
+        const float v = rgb[3 * i + c] > 0.f ? std::fmin(rgb[3 * i + c], 1.f) : 0.f;
         if (px[4 * i + c] != (unsigned char)(v * 255.0f)) ++bad;
       }
       if (px[4 * i + 3] != 255) ++bad;
@@ -161,7 +163,7 @@ int main(int argc, char** argv) {
     if (!fp) { std::fprintf(stderr, "cannot write %s\n", out.c_str()); return 1; }
     std::fprintf(fp, "P6\n%d %d\n255\n", W, H);
     for (size_t i = 0; i < rgb.size(); ++i) {
-      const float v = rgb[i] < 0.f ? 0.f : (rgb[i] > 1.f ? 1.f : rgb[i]);
+      const float v = rgb[i] > 0.f ? std::fmin(rgb[i], 1.f) : 0.f;
       std::fputc(int(v * 255.0f), fp);
     }
     std::fclose(fp);

@@ -70,10 +70,10 @@ cudaError_t launch_stage3(const SceneDev& sc, const float* d_ray_o, const float*
 struct Stage5Aux {
   float* weights = nullptr;     // [N,K] zero padded (NeRFWeightsOutput)
   float* alpha = nullptr;       // [N,K] zero padded, sigmoid(a) * zp (NeRFAlphaOutput)
-  float* z_vals = nullptr;      // [N,K] world depth, NaN padded (NeRFInputFeatureZVals)
+  float* z_vals = nullptr;      // [N,K] world depth, NaN padded and NaN at z == +-0 unless dense (NeRFInputFeatureZVals)
   float* depth_map = nullptr;   // [N] sum w z
   float* acc_map = nullptr;     // [N] sum w
-  float* disp_map = nullptr;    // [N] 1 / max(1e-10, depth_map / acc_map)
+  float* disp_map = nullptr;    // [N] 1 / torch.max(1e-10, depth_map / acc_map), NaN when the quotient is
   float* depth_est = nullptr;   // [N] LogTransform.from_world(depth_map, depth_range) (NeRFOutputDepth)
   int linear_depth = 0;         // NDC: depth_est = depth_map (features.py:573-574)
   float dr_min = 0.0f;          // depth_range[0]

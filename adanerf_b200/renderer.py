@@ -163,11 +163,13 @@ class Renderer:
     # ---- the hot path --------------------------------------------------------------------
     AUX_KEYS = ("weights", "alpha", "z_vals", "depth_map", "acc_map", "disp_map", "depth_est")
 
-    def render_rays(self, pose, rot, dirs, thr, K, want_nsamples=True, want_oracle_weights=False, want_aux=False, out=None):
+    def render_rays(self, pose, rot, dirs, thr, K, want_nsamples=True, want_oracle_weights=False, want_aux=False, out=None,
+                    aux_out=None):
         """dirs [N,3] (cuda tensor) -> dict(rgb [N,3], n_samples [N] int32, oracle_weights [N,128]).
         want_aux: True or an iterable of AUX_KEYS -> additionally weights / alpha / z_vals [N,K] and depth_map /
         acc_map / disp_map / depth_est [N] (adaptive_raw2outputs' other outputs, src/nerf_raymarch_common.py:137-144;
-        depth_est = "NeRFOutputDepth", src/features.py:574-577)."""
+        depth_est = "NeRFOutputDepth", src/features.py:574-577).  aux_out: dict of contiguous float32 tensors on the
+        renderer's device to write requested aux outputs into instead of new ones."""
         p, r = self._pose_rot(pose, rot)
         d = self._f32(dirs).reshape(-1, 3)
         n = d.shape[0]
@@ -183,7 +185,12 @@ class Renderer:
             for k in self.AUX_KEYS if want_aux is True else tuple(want_aux):
                 if k not in self.AUX_KEYS:
                     raise KeyError(f"unknown auxiliary output {k!r}")
-                t = torch.empty((n, int(K)) if k in ("weights", "alpha", "z_vals") else (n,), dtype=torch.float32, device=self._dev())
+                shape = (n, int(K)) if k in ("weights", "alpha", "z_vals") else (n,)
+                t = (aux_out or {}).get(k)
+                if t is None:
+                    t = torch.empty(shape, dtype=torch.float32, device=self._dev())
+                elif t.dtype != torch.float32 or tuple(t.shape) != shape or not t.is_contiguous() or t.device != self._dev():
+                    raise ValueError(f"render_rays: aux_out[{k!r}] must be a contiguous float32 {list(shape)} tensor on the renderer's device")
                 out[k] = t
                 setattr(aux, "d_" + k, t.data_ptr())
         with torch.cuda.device(self.device):
@@ -205,10 +212,14 @@ class Renderer:
                                                    rgb.data_ptr(), ns.data_ptr() if ns is not None else None, self._stream()))
         return dict(rgb=rgb, n_samples=ns)
 
-    def render_camera_rgba8(self, pose, rot, W, H, thr, K, row0=0, rows=None):
+    def render_camera_rgba8(self, pose, rot, W, H, thr, K, row0=0, rows=None, out=None):
+        """The viewer's pixels of image rows [row0, row0+rows) -> [rows*W, 4] uint8 (into `out` when given)."""
         rows = H - row0 if rows is None else rows
         p, r = self._pose_rot(pose, rot)
-        out = torch.empty((rows * W, 4), dtype=torch.uint8, device=self._dev())
+        if out is not None and (out.dtype != torch.uint8 or tuple(out.shape) != (rows * W, 4) or not out.is_contiguous()
+                                or out.device != self._dev()):
+            raise ValueError("render_camera_rgba8: out must be a contiguous uint8 [rows*W, 4] tensor on the renderer's device")
+        out = out if out is not None else torch.empty((rows * W, 4), dtype=torch.uint8, device=self._dev())
         with torch.cuda.device(self.device):
             self._check(self.lib.adn_render_camera_rgba8(self.handle, _fptr(p), _fptr(r), W, H, row0, rows, float(thr), int(K),
                                                          out.data_ptr(), self._stream()))
@@ -317,19 +328,45 @@ class Renderer:
         self._check(self.lib.adn_mlp1_forward(self.handle, x.data_ptr(), x.shape[0], out.data_ptr(), self._stream()))
         return out
 
-    def stage5(self, raw1, zp, z, offset, count, K, want_aux=True):
-        r1, zpp, zz = self._f32(raw1), self._f32(zp), self._f32(z)
-        off = offset.to(device=self._dev(), dtype=torch.int32).contiguous()
-        cnt = count.to(device=self._dev(), dtype=torch.int32).contiguous()
-        n = cnt.shape[0]
-        rgb = torch.empty((n, 3), dtype=torch.float32, device=self._dev())
-        w = torch.empty((n, K), dtype=torch.float32, device=self._dev()) if want_aux else None
-        dm = torch.empty((n,), dtype=torch.float32, device=self._dev()) if want_aux else None
-        self._check(self.lib.adn_stage5_composite(self.handle, r1.data_ptr(), zpp.data_ptr(), zz.data_ptr(), off.data_ptr(),
-                                                  cnt.data_ptr(), n, int(K), rgb.data_ptr(),
-                                                  w.data_ptr() if w is not None else None,
-                                                  dm.data_ptr() if dm is not None else None, self._stream()))
-        return dict(rgb=rgb, weights=w, depth_map=dm)
+    def stage5(self, raw1, zp, z, offset, count, K, want_aux=True, aux=None, dense=False, rgba8=False, out=None):
+        """Stage 5 alone (adn_stage5_composite_aux) -> dict(rgb [N,3], rgba8 [N,4] uint8, and each requested aux output).
+        want_aux: weights and depth_map (aux=None only).  aux: True or an iterable of AUX_KEYS.  dense: zp is raw0 [N,128]
+        and z / offset / count may be None (K must be 128).  out: dict of tensors to write into instead of new ones (keys
+        "rgb", "rgba8" and AUX_KEYS; each one given is also requested) -- slots the kernel does not write keep their
+        contents."""
+        dev = self._dev()
+        out = dict(out or {})
+        r1, zpp = self._f32(raw1), self._f32(zp)
+        n = zpp.shape[0] if dense else count.shape[0]
+        zz = self._f32(z) if z is not None else None
+        off = offset.to(device=dev, dtype=torch.int32).contiguous() if offset is not None else None
+        cnt = count.to(device=dev, dtype=torch.int32).contiguous() if count is not None else None
+        keys = (("weights", "depth_map") if want_aux else ()) if aux is None else self.AUX_KEYS if aux is True else tuple(aux)
+        keys = tuple(k for k in self.AUX_KEYS if k in keys or k in out)
+        shapes = dict(rgb=((n, 3), torch.float32), rgba8=((n, 4), torch.uint8))
+        shapes.update({k: ((n, int(K)) if k in ("weights", "alpha", "z_vals") else (n,), torch.float32) for k in self.AUX_KEYS})
+        for k in ("rgb",) + (("rgba8",) if rgba8 or "rgba8" in out else ()) + keys:
+            if k not in shapes:
+                raise KeyError(f"unknown stage-5 output {k!r}")
+            shape, dt = shapes[k]
+            if k in out:
+                t = out[k]
+                if t.dtype != dt or tuple(t.shape) != shape or not t.is_contiguous() or t.device != dev:
+                    raise ValueError(f"stage5: out[{k!r}] must be a contiguous {dt} {list(shape)} tensor on the renderer's device")
+            else:
+                out[k] = torch.empty(shape, dtype=dt, device=dev)
+        a = AuxOutputs()
+        for k in keys:
+            setattr(a, "d_" + k, out[k].data_ptr())
+        ptr = lambda t: t.data_ptr() if t is not None else None
+        with torch.cuda.device(self.device):
+            self._check(self.lib.adn_stage5_composite_aux(self.handle, r1.data_ptr(), zpp.data_ptr(), ptr(zz), ptr(off), ptr(cnt),
+                                                          n, int(K), int(bool(dense)), out["rgb"].data_ptr(),
+                                                          ptr(out.get("rgba8")), C.byref(a), self._stream()))
+        if aux is None:
+            for k in ("weights", "depth_map"):
+                out.setdefault(k, None)
+        return out
 
 
 _RENDERERS = {}

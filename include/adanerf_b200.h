@@ -151,10 +151,11 @@ adn_status adn_render_rays(adn_ctx* ctx, const float* pose, const float* rot, co
 typedef struct adn_aux_outputs {
   float* d_weights;    /* [N,K] "NeRFWeightsOutput": alpha * transmittance, 0 in unused slots */
   float* d_alpha;      /* [N,K] "NeRFAlphaOutput": sigmoid(raw alpha) * sampling-net value, 0 in unused slots */
-  float* d_z_vals;     /* [N,K] "NeRFInputFeatureZVals": world depth of the samples, NaN in unused slots */
+  float* d_z_vals;     /* [N,K] "NeRFInputFeatureZVals": world depth of the samples, NaN in unused slots and, as in the
+                          reference's adaptive path, at samples with z == +-0 (dense mode keeps 0) */
   float* d_depth_map;  /* [N] sum_k w z (world depth) */
   float* d_acc_map;    /* [N] sum_k w */
-  float* d_disp_map;   /* [N] 1 / max(1e-10, depth_map / acc_map) */
+  float* d_disp_map;   /* [N] 1 / torch.max(1e-10, depth_map / acc_map): NaN when the quotient is (0 / 0 at acc == 0) */
   float* d_depth_est;  /* [N] "NeRFOutputDepth": LogTransform.from_world(depth_map, depth_range) */
 } adn_aux_outputs;
 adn_status adn_render_rays_aux(adn_ctx* ctx, const float* pose, const float* rot, const float* d_dirs, int64_t n_rays,
@@ -231,6 +232,14 @@ adn_status adn_mlp1_forward(adn_ctx* ctx, const float* d_x1, int64_t n_samples, 
 adn_status adn_stage5_composite(adn_ctx* ctx, const float* d_raw1, const float* d_zp, const float* d_z,
                                 const int32_t* d_offset, const int32_t* d_count, int64_t n_rays, int K,
                                 float* d_rgb, float* d_weights, float* d_depth_map, void* stream);
+/* stage 5 with every output a render can ask for: d_rgb [N,3] and d_rgba8 [N] uchar4 (the viewer's pixels) may each be
+ * NULL, and so may every pointer of *aux (aux itself may be NULL).  depth_est uses the context's scene (depth_range, NDC)
+ * exactly as a render does.  dense = 0: the packed layout of adn_stage2_sample (d_zp, d_z [M], d_offset / d_count [N]).
+ * dense = 1: RayMarchFromPoses without remapping -- K must be 128, d_zp is the sampling net's raw0 [N,128], z comes from
+ * the context's dense depth table (what a thr == 0 render uses), and d_z / d_offset / d_count are ignored. */
+adn_status adn_stage5_composite_aux(adn_ctx* ctx, const float* d_raw1, const float* d_zp, const float* d_z,
+                                    const int32_t* d_offset, const int32_t* d_count, int64_t n_rays, int K, int dense,
+                                    float* d_rgb, uint8_t* d_rgba8, const adn_aux_outputs* aux, void* stream);
 
 /* ---- evaluation metric on the device ------------------------------------------------------ */
 /* calculate_mse / calculate_psnr (src/evaluate.py:49-54) of two device images of n_values floats each:

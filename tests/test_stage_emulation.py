@@ -355,3 +355,114 @@ def test_teeth_sequential_product_in_the_warp_composite():
     assert not np.array_equal(good["weights"], bad["weights"])
     # the thread kernel's chain is not the warp kernel's either: the two emulations are not interchangeable
     assert not np.array_equal(good["weights"], se.stage5_thread(sig, zp, z, off, cnt, 100)["weights"])
+
+
+# ------------------------------------------------------------------------------------- stage-5 per-ray and padded outputs
+@pytest.mark.parametrize("case", ["pav_k8_t0.2", "pav_k8_t0.5", "pav_k16_t0.15", "shaped_k8_t0.2", "rand_k8_t0.2",
+                                  "ndc_k16_t0.15"])
+def test_stage5_aux_emulation_matches_the_oracle(case):
+    """alpha, z_vals, acc_map, disp_map and depth_est of both composites against the reference's tensors (golden alpha,
+    z_vals, depth_est) and the oracle's composite (acc, disp) on the same inputs."""
+    g = load_golden(case)
+    m = g["meta"]
+    K, scene = m["K"], m["scene_params"]
+    mask, _, z = _packed(g, K)
+    cnt = mask.sum(1)
+    off = np.concatenate([[0], np.cumsum(cnt)[:-1]])
+    o2 = orc.stage2_sample(torch.from_numpy(g["raw0"]), m["thr"], K, scene["depth_range"], no_depth_range=bool(scene.get("use_ndc")))
+    zp = o2["zp"].numpy()[mask]
+    raw1 = g["raw1_pad"].reshape(-1, 4)[mask.flatten()]
+    comp = orc.stage5_composite(torch.from_numpy(raw1), torch.from_numpy(z), o2["zp"].float(), torch.from_numpy(mask.flatten()),
+                                mask.shape[0], K)
+    for fn in (se.stage5_thread, se.stage5_warp):
+        out = fn(_sig32(raw1), zp, z, off, cnt, K)
+        np.testing.assert_allclose(out["alpha"], g["alpha"], rtol=0, atol=1e-6)
+        np.testing.assert_array_equal(out["z_vals"], g["z_nan"])          # NaN at the same places
+        np.testing.assert_allclose(out["acc_map"], comp["acc"].numpy(), rtol=0, atol=2e-6)
+        # disparity is ill-conditioned where depth_map / acc is tiny, so the rule is checked on the oracle's own inputs
+        _assert_bits_equal(se.disp_map(comp["depth_map"].numpy(), comp["acc"].numpy()), comp["disp"].numpy())
+        v, bound = se.depth_est_f64(out["depth_map"], scene)
+        np.testing.assert_allclose(v, g["depth_est"][:, 0], rtol=0, atol=2e-6)
+        ref = out["depth_map"] if scene.get("use_ndc") else orc.log_from_world(torch.from_numpy(out["depth_map"]), scene["depth_range"]).numpy()
+        assert (np.abs(v - ref) <= bound + 4 * se.ulp32(ref)).all()
+
+
+def test_stage5_dense_emulation_matches_the_oracle():
+    """The dense variant against the oracle's dense composite (mapping None, zp = raw0, z = the dense table)."""
+    rng = np.random.default_rng(12)
+    n, scene = 200, orc.SCENE_BARBERSHOP
+    raw0 = rng.uniform(-0.2, 1.2, (n, 128)).astype(F32)
+    raw1 = rng.standard_normal((n * 128, 4)).astype(F32)
+    lut = se.zlut_dense(scene, 128)
+    out = se.stage5_dense(_sig32(raw1), raw0, lut)
+    ref = orc.stage5_composite(torch.from_numpy(raw1), torch.from_numpy(np.tile(lut, n)), torch.from_numpy(raw0), None, n, 128)
+    for k, rk in (("rgb", "rgb"), ("weights", "weights"), ("alpha", "alpha"), ("acc_map", "acc")):
+        np.testing.assert_allclose(out[k], ref[rk].numpy(), rtol=0, atol=2e-6, err_msg=k)
+    np.testing.assert_allclose(out["depth_map"], ref["depth_map"].numpy(), rtol=0, atol=2e-5)
+    np.testing.assert_array_equal(out["z_vals"], np.tile(lut, (n, 1)))
+
+
+def test_z_vals_of_a_live_sample_at_zero_is_nan_except_in_dense_mode():
+    """features.py:546-547 sets every slot of the restored z == 0 to NaN, live samples at z = +-0 included; the dense path
+    stores its z unchanged.  depth_map still uses z = 0 (adaptive_raw2outputs reads its own restored_z)."""
+    sig = np.full((4, 4), 0.5, F32)
+    zp = np.ones(4, F32)
+    z = np.array([0.0, -0.0, 1.5, 0.0], F32)
+    for fn in (se.stage5_thread, se.stage5_warp):
+        out = fn(sig, zp, z, [0, 3], [3, 1], 4)
+        assert np.isnan(out["z_vals"][0, [0, 1, 3]]).all() and out["z_vals"][0, 2] == F32(1.5)
+        assert np.isnan(out["z_vals"][1]).all()
+        assert out["z_vals"].view(np.uint32)[np.isnan(out["z_vals"])].tolist() == [0x7fc00000] * 7
+    lut = np.zeros(128, F32)
+    assert (se.stage5_dense(np.full((128, 4), 0.5, F32), np.ones((1, 128), F32), lut)["z_vals"] == 0).all()
+
+
+def _torch_disp(dm, acc):
+    dm, acc = torch.from_numpy(np.asarray(dm, F32)), torch.from_numpy(np.asarray(acc, F32))
+    return (1.0 / torch.max(1e-10 * torch.ones_like(dm), dm / acc)).numpy()
+
+
+def _assert_bits_equal(a, b):
+    a, b = np.asarray(a, F32), np.asarray(b, F32)
+    np.testing.assert_array_equal(np.isnan(a), np.isnan(b))
+    fin = ~np.isnan(a)
+    np.testing.assert_array_equal(a[fin].view(np.uint32), b[fin].view(np.uint32))
+
+
+def test_disp_map_is_torch_max():
+    """disp_map equals 1 / torch.max(1e-10, dm / acc) bit for bit: 0 / 0, x / 0, +-inf quotients, negative acc, quotients
+    around 1e-10, denormals, and NaN inputs.  The fmaxf form differs exactly where the quotient is NaN."""
+    tiny, den = F32(1e-10), F32(2.0 ** -140)
+    vals = np.array([0.0, -0.0, 1.0, -1.0, 0.5, 3.0, np.inf, -np.inf, np.nan, tiny, np.nextafter(tiny, F32(0)),
+                     np.nextafter(tiny, F32(1)), den, -den, 1e30, 7.25], F32)
+    dm, acc = (a.ravel() for a in np.meshgrid(vals, vals))
+    rng = np.random.default_rng(5)
+    dm = np.concatenate([dm, rng.standard_normal(5000).astype(F32) * 10])
+    acc = np.concatenate([acc, rng.uniform(-0.5, 1.5, 5000).astype(F32)])
+    ours, want = se.disp_map(dm, acc), _torch_disp(dm, acc)
+    _assert_bits_equal(ours, want)
+    assert np.isnan(se.disp_map(F32(0), F32(0)))
+    with np.errstate(invalid="ignore", divide="ignore", over="ignore"):
+        old = F32(1) / np.fmax(F32(1e-10), dm / acc)
+    assert not np.array_equal(np.isnan(old), np.isnan(want))          # the fmaxf form gives 1e10 at 0 / 0
+
+
+def _saturatef(x):
+    """__saturatef (CUDA Math API): x clamped to [+0, 1], NaN -> +0."""
+    return F32(0) if np.isnan(x) or x <= 0 else min(F32(x), F32(1))
+
+
+def test_rgba8_is_the_viewers_compiled_clamp():
+    """rgba8 on NaN, +-inf, +-0, every k / 255 and its fp32 neighbours, 1 - ulp, and values outside [0, 1], against a
+    per-value trunc(__saturatef(x) * 255).  nvcc compiles helper_math.h's clamp fmaxf(0, fminf(x, 1)) -- and the other
+    order too -- to one FADD.SAT, so the viewer's NaN pixel is 0, not the 255 the C semantics of the source would give."""
+    ks = (np.arange(256, dtype=np.float64) / 255.0).astype(F32)
+    x = np.concatenate([np.array([np.nan, -np.nan, np.inf, -np.inf, 0.0, -0.0, 1.0, np.nextafter(F32(1), F32(0)), 1.5, -0.25,
+                                  2.0 ** -149, -2.0 ** -149, 1e30], F32),
+                        ks, np.nextafter(ks, F32(2)), np.nextafter(ks, F32(-1))]).astype(F32)
+    x = np.concatenate([x, np.zeros((-len(x)) % 3, F32)]).reshape(-1, 3)
+    got = se.rgba8(x)
+    want = np.array([[int(np.trunc(_saturatef(v) * F32(255))) for v in row] + [255] for row in x], np.uint8)
+    np.testing.assert_array_equal(got, want)
+    assert got[0, 0] == 0 and got[0, 1] == 0 and got[0, 2] == 255 and got[1, 0] == 0         # NaN, NaN, inf, -inf
+    assert set(np.unique(se.rgba8(ks.reshape(-1, 1).repeat(3, 1))[:, 0])) == set(range(256))

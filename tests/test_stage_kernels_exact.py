@@ -215,13 +215,16 @@ def _composite_f64(logits, zp, z, off, cnt, K):
       factors (<= 1) multiply it, and T_j's tree has at most j + 1 multiplies -> e_T = sum_{i<j} e_f(i) T_i + (j + 1) u T_j;
       w = alpha T: e_w = e_a T + alpha e_T + u w;  term = w s: e_w s + w e_s + u term;
       sum of n terms in any order of depth <= n + 9 (thread: n sequential adds; warp: <= 4 per lane + 5 butterfly levels):
-      (n + 9) u sum(term).  Returns (rgb, weights, depth) and their bounds."""
+      (n + 9) u sum(term); acc_map = sum w the same way.  Returns (rgb, weights, alpha, depth_map, acc_map) and their
+      bounds."""
     n = cnt.shape[0]
     eps = float(se.EPS_T)
     T, S = np.ones(n), np.zeros(n)
     rgb, e_rgb = np.zeros((n, 3)), np.zeros((n, 3))
     dm, e_dm, sum_rgb, sum_dm = np.zeros(n), np.zeros(n), np.zeros((n, 3)), np.zeros(n)
     w_out, e_w_out = np.zeros((n, K)), np.zeros((n, K))
+    a_out, e_a_out = np.zeros((n, K)), np.zeros((n, K))
+    acc, e_acc = np.zeros(n), np.zeros(n)
     for j in range(K):
         live = j < cnt
         idx = np.where(live, off + j, 0)
@@ -240,12 +243,15 @@ def _composite_f64(logits, zp, z, off, cnt, K):
         e_rgb = upd(e_rgb, e_w[:, None] * s[:, :3] + w[:, None] * e_s[:, :3] + U * term)
         dm, sum_dm = upd(dm, zt), upd(sum_dm, zt)
         e_dm = upd(e_dm, e_w * z[idx] + U * zt)
+        acc, e_acc = upd(acc, w), upd(e_acc, e_w)
         w_out[:, j], e_w_out[:, j] = np.where(live, w, 0), np.where(live, e_w, 0)
+        a_out[:, j], e_a_out[:, j] = np.where(live, a, 0), np.where(live, e_a, 0)
         S = np.where(live, S + e_f * T, S)
         T = np.where(live, T * f, T)
     depth = (cnt + 9) * U
-    return dict(rgb=rgb, weights=w_out, depth_map=dm), dict(rgb=1.01 * (e_rgb + depth[:, None] * sum_rgb),
-                                                             weights=1.01 * e_w_out, depth_map=1.01 * (e_dm + depth * sum_dm))
+    return (dict(rgb=rgb, weights=w_out, alpha=a_out, depth_map=dm, acc_map=acc),
+            dict(rgb=1.01 * (e_rgb + depth[:, None] * sum_rgb), weights=1.01 * e_w_out, alpha=1.01 * e_a_out,
+                 depth_map=1.01 * (e_dm + depth * sum_dm), acc_map=1.01 * (e_acc + depth * acc)))
 
 
 @pytest.mark.parametrize("K", [8, 17, 32, 33, 64, 128])
