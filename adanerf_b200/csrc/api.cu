@@ -211,8 +211,9 @@ adn_status upload(adn_ctx* ctx, Net& net, const std::vector<uint8_t>& wblob, con
 // The layer programs of the two networks are derived here, from the tensor shapes, and nowhere else in the library.
 //
 // Sampling net: BaseNet without skips (src/models.py:71-76,183-195): layers.{i}.weight/bias, D = 1-12 layers, n_in <= 128
-// inputs, every hidden layer W = 128 or 256 wide, 128 or 256 outputs.  Layer 0 reads the input blocks, every other layer
-// the W/64 activation blocks, which its epilogue overwrites in place.
+// inputs, every hidden layer W = 128 or 256 wide, 128 or 256 outputs.  Layer 0 reads the two input blocks, every other
+// layer the W/64 hidden blocks (split precision: in shared memory, overwritten in place by its epilogue; plain bf16: in
+// registers).
 adn_status build_net0(adn_ctx* ctx) {
   Net& net = ctx->net[0];
   auto bad = [&](const std::string& msg) { return fail(ctx, ADN_ERR_INVALID, "sampling net: " + msg); };
@@ -256,14 +257,13 @@ adn_status build_net0(adn_ctx* ctx) {
       for (int c = 0; c < k_in; c += 64) segs.push_back({c, 64});
     }
     L.n_kb = uint8_t(segs.size());
+    (l == 0 ? L.in_first : L.n_hid) = L.n_kb;
     for (size_t i = 0; i < segs.size(); ++i) {
-      L.a_blk[i] = uint8_t(i);
       // 16-wide K steps that hold data; block 0 keeps at least one (it initialises the accumulator)
       L.k_cnt[i] = uint8_t(std::max(i == 0 ? 1 : 0, (segs[i].valid + 15) / 16));
     }
     L.n_half = uint8_t(n_out / 128);
     L.flags = last ? uint8_t(LF_FINAL_RAW) : uint8_t(LF_RELU | LF_OUT_ACT);
-    L.out_blk0 = 0;
     L.w_off = uint32_t(wblob.size());
     pack_layer(W->data.data(), n_out, k_in, segs, nsplit, wblob);
     L.bias_off = uint32_t(push_floats(fblob, B->data.data(), B->data.size()));
@@ -287,10 +287,11 @@ adn_status build_net0(adn_ctx* ctx) {
 // Shading net: NeRF(D, W, skips, use_viewdirs=True) (src/models.py:199-277) with posEnc 10-4 (63 position + 27 direction
 // features).  D = 1-10 pts_linears (D + feature + view layer <= kMaxLayers), W = 128 or 256, the view branch W/2.  A skip
 // after pts layer i shows as pts_linears.{i+1} reading W + 63 columns, cat[pts, h] (models.py:226-228, 260-261); at most
-// one.  The program, activation block 0 holding the input block P (then V) and blocks 1.. the W/64 hidden blocks:
-//   pts layer 0 reads P; the skip consumer reads P and the hidden blocks; the other pts layers read the hidden blocks; the
+// one.  The program, the input block P (then V) in shared memory and the W/64 hidden blocks in the consumers' registers:
+//   pts layer 0 reads P; the skip consumer reads P, then the hidden blocks; the other pts layers read the hidden blocks; the
 //   last pts layer also forms alpha (LF_ALPHA_DOT); V replaces P after the skip consumer, or after layer 0 without a skip;
-//   feature_linear: W -> W without activation; views_linears.0 on cat[feature, V] -> W/2, with rgb_linear in its epilogue.
+//   feature_linear: W -> W without activation; views_linears.0 on cat[feature, V] -> W/2 reads the hidden blocks, then V,
+//   with rgb_linear in its epilogue.
 // At W = 128 the view layer's 64 outputs are padded to the kernel's 128 rows with zero weights, zero biases and zero
 // rgb_linear columns: ReLU(0) = 0 adds nothing to the rgb dot products, so the result is exact.
 adn_status build_net1(adn_ctx* ctx) {
@@ -350,13 +351,12 @@ adn_status build_net1(adn_ctx* ctx) {
   for (int l = 0; l < D + 2; ++l) {
     MlpLayer& L = P.layers[l];
     std::vector<Seg> segs;
-    std::vector<uint8_t> blk;
-    auto read_p = [&] { segs.push_back({0, kP}), blk.push_back(0); };
+    auto read_p = [&] { segs.push_back({0, kP}), L.in_first = 1; };
     auto read_hidden = [&](int col0) {
-      for (int b = 0; b < nh; ++b) segs.push_back({col0 + 64 * b, 64}), blk.push_back(uint8_t(1 + b));
+      for (int b = 0; b < nh; ++b) segs.push_back({col0 + 64 * b, 64});
+      L.n_hid = uint8_t(nh);
     };
     const HostTensor *Wt, *B;
-    L.out_blk0 = 1;
     L.n_half = uint8_t(W / 128);
     if (l < D) {
       if (l == 0) {
@@ -378,17 +378,14 @@ adn_status build_net1(adn_ctx* ctx) {
     } else {  // views_linears.0 on cat[feature, views] (models.py:266-269) + rgb_linear in the epilogue
       read_hidden(0);
       segs.push_back({W, kV});
-      blk.push_back(0);
-      L.flags = LF_RELU | LF_FINAL_RGB | LF_WAIT_IN;
+      L.in_last = 1;
+      L.flags = LF_RELU | LF_FINAL_RGB;
       L.n_half = 1;
       Wt = vw;
       B = vb;
     }
     L.n_kb = uint8_t(segs.size());
-    for (size_t i = 0; i < segs.size(); ++i) {
-      L.a_blk[i] = blk[i];
-      L.k_cnt[i] = uint8_t((segs[i].valid + 15) / 16);
-    }
+    for (size_t i = 0; i < segs.size(); ++i) L.k_cnt[i] = uint8_t((segs[i].valid + 15) / 16);
     L.w_off = uint32_t(wblob.size());
     pack_layer(Wt->data.data(), int(Wt->rows), int(Wt->cols), segs, 1, wblob);
     std::vector<float> bias(size_t(L.n_half) * 128, 0.0f);   // zero rows past the view layer's W/2 outputs

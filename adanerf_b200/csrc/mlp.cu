@@ -17,7 +17,9 @@ struct ConstFlags {
 
 template <int NSPLIT>
 struct MlpCfg {
-  static constexpr int kNB = (NSPLIT == 2) ? 4 : 5;                  // activation blocks per term
+  // activation blocks per term: the split net's input / hidden blocks; with NSPLIT == 1 the input blocks only (the
+  // sampling net's two, the shading net's P, then V), the hidden activations stay in registers
+  static constexpr int kNB = (NSPLIT == 2) ? 4 : 2;
   static constexpr int kStageBytes = NSPLIT * kBlkBytes;              // one [128 x 64] weight block (+ its lo part)
   // as many ring stages as fit next to the activations and the side parameters (227 KB per block)
   static constexpr int kStages = (NSPLIT == 2) ? 2 : 8;
@@ -106,7 +108,7 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
 
   if (warp >= kProducerWarp) {
     // ===================================================================== weight producer
-    setmaxnreg_dec<40>();
+    setmaxnreg_dec<24>();
     // Stage i of a layer is [128 N rows x 64 K] (hi, then lo when NSPLIT == 2), N half outermost: the order the
     // consumers walk them in.
     if (warp == kProducerWarp && lane == 0) {
@@ -132,7 +134,9 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
   }
 
   // ============================================================================ consumer warpgroups
-  setmaxnreg_inc<232>();
+  // 2 x 128 x 240 + 128 x 24 <= 64 K registers.  The shading net's consumers keep 128 accumulator and 64 A-fragment
+  // registers live through the MMAs; at 232 the fused encoder, which runs while a layer's fragments are live, spills.
+  setmaxnreg_inc<240>();
   const int wg = warp >> 2;                               // rows [64 wg, 64 wg + 64) of every tile
   const int tw = threadIdx.x & 127;
   const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2); // accumulator rows r0 and r0 + 8 of this thread
@@ -145,8 +149,45 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
   const uint64_t desc_hi = make_desc_sw128(0) & ~uint64_t(0x3FFF);
   auto desc = [&](uint32_t addr) -> uint64_t { return desc_hi | uint64_t((addr & 0x3FFFF) >> 4); };
 
+  // Shading net: the bf16 output of the last LF_OUT_ACT layer as register-A fragments, [K block][K step][register]
+  // (hidden column 64 kb + 16 k + ...).  Indexed with compile-time constants only, so it stays in registers.
+  uint32_t afrag[4][4][4];
+  // The compiler cannot see which layers read afrag (the layer program is read at run time), so every epilogue and every
+  // tile start define all of it; the registers a layer does not write are never read.  Otherwise the previous values
+  // stay alive through MMAs, epilogues and the fused encoder, and spill.
+  auto clear_afrag = [&](int kb0, int kb1) {
+#pragma unroll
+    for (int kb = 0; kb < 4; ++kb)
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+          if (kb >= kb0 && kb < kb1) afrag[kb][k][j] = 0u;
+  };
+
   int stage = 0;
   uint32_t phase = 0;
+  int prev = -1;   // ring stage whose MMAs may still be running
+  // One K block = one ring stage: wait for it, issue up to 4 K steps through mma(k, B stage address, accumulate), and hand
+  // the previous stage back to the producer once its MMAs have retired.
+  auto k_block = [&](bool first, int nk, auto mma) {
+    mbar_wait(&w_full[stage], phase, err_flag, 2);
+    wgmma_fence();
+    const uint32_t b = ring_s + uint32_t(stage) * STAGE_BYTES;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      if (k < nk) mma(k, b, (first && k == 0) ? 0u : 1u);   // zero-padded tail columns of an input block are not multiplied
+    }
+    wgmma_commit();
+    wgmma_wait<1>();   // the previous stage's MMAs have retired: hand it back to the producer
+    if (prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);
+    prev = stage;
+    if (++stage == STAGES) {
+      stage = 0;
+      phase ^= 1;
+    }
+  };
+
   for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) {
     // tile input (the previous tile's last MMAs retired before its epilogue: the blocks are free)
     if (ENC) {
@@ -158,54 +199,67 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
     }
     fence_proxy_async_smem();
     named_bar_sync(bar_id, 128);
+    if (NSPLIT == 1) clear_afrag(0, 4);
     float alpha[2] = {0.0f, 0.0f};
     for (int l = 0; l < prog.n_layers; ++l) {
       const MlpLayer& L = prog.layers[l];
       float acc[2][64];   // written by the first MMA of each half (accumulate = 0): K block 0 has at least one K step
-      int prev = -1;   // ring stage whose MMAs may still be running
 #pragma unroll
       for (int nh = 0; nh < 2; ++nh) {
         if (nh >= L.n_half) break;
-        for (int kb = 0; kb < L.n_kb; ++kb) {
-          const uint32_t a_hi = blk_addr(0, L.a_blk[kb]) + wg_off;
-          const uint32_t a_lo = a_hi + uint32_t(NSPLIT - 1) * NB * kBlkBytes;
-          const uint32_t b_hi = ring_s + uint32_t(stage) * STAGE_BYTES;
-          const uint32_t b_lo = b_hi + uint32_t(NSPLIT - 1) * kBlkBytes;
-          const int nk = L.k_cnt[kb];   // zero-padded tail columns of an input block are not multiplied
-          mbar_wait(&w_full[stage], phase, err_flag, 2);
-          wgmma_fence();
+        if (NSPLIT == 2) {
+          for (int kb = 0; kb < L.n_kb; ++kb) {
+            const uint32_t a_hi = blk_addr(0, kb) + wg_off;
+            const uint32_t a_lo = a_hi + uint32_t(NB) * kBlkBytes;
+            k_block(kb == 0, L.k_cnt[kb], [&](int k, uint32_t b_hi, uint32_t accumulate) {
+              const uint32_t b_lo = b_hi + uint32_t(kBlkBytes);
+              wgmma_m64n128_bf16(acc[nh], desc(a_hi + 32 * k), desc(b_hi + 32 * k), accumulate);
+              wgmma_m64n128_bf16(acc[nh], desc(a_lo + 32 * k), desc(b_hi + 32 * k), 1u);
+              wgmma_m64n128_bf16(acc[nh], desc(a_hi + 32 * k), desc(b_lo + 32 * k), 1u);
+            });
+          }
+        } else {
+          auto from_smem = [&](int blk) {
+            const uint32_t a = blk_addr(0, blk) + wg_off;
+            return [&, a](int k, uint32_t b, uint32_t accumulate) {
+              wgmma_m64n128_bf16(acc[nh], desc(a + 32 * k), desc(b + 32 * k), accumulate);
+            };
+          };
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            if (k < nk) {
-              wgmma_m64n128_bf16(acc[nh], desc(a_hi + 32 * k), desc(b_hi + 32 * k), (kb > 0 || k > 0) ? 1u : 0u);
-              if (NSPLIT == 2) {
-                wgmma_m64n128_bf16(acc[nh], desc(a_lo + 32 * k), desc(b_hi + 32 * k), 1u);
-                wgmma_m64n128_bf16(acc[nh], desc(a_hi + 32 * k), desc(b_lo + 32 * k), 1u);
-              }
-            }
+          for (int ib = 0; ib < NB; ++ib) {
+            if (ib >= L.in_first) break;
+            k_block(ib == 0, L.k_cnt[ib], from_smem(ib));
           }
-          wgmma_commit();
-          wgmma_wait<1>();   // the previous stage's MMAs have retired: hand it back to the producer
-          if (prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);
-          prev = stage;
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1;
+#pragma unroll
+          for (int hb = 0; hb < 4; ++hb) {
+            if (hb >= L.n_hid) break;
+            k_block(hb == 0 && L.in_first == 0, 4, [&](int k, uint32_t b, uint32_t accumulate) {
+              wgmma_m64n128_bf16_rs(acc[nh], afrag[hb][k], desc(b + 32 * k), accumulate);
+            });
           }
+          if (L.in_last) k_block(L.n_kb == 1, L.k_cnt[L.n_kb - 1], from_smem(0));
         }
       }
       wgmma_wait<0>();
       if (lane == 0) mbar_arrive(&w_empty[prev]);
-      named_bar_sync(bar_id, 128);   // all of the warpgroup's MMAs retired: the A blocks may be overwritten in place
+      prev = -1;
+      // All of the warpgroup's MMAs retired: the A blocks in shared memory may be overwritten in place.  The shading net
+      // overwrites its input block only after the LF_LOAD_IN1_AFTER layer and at the next tile's start.
+      const bool input_next = (L.flags & LF_LOAD_IN1_AFTER) || l + 1 == prog.n_layers;
+      if (NSPLIT == 2 || input_next) named_bar_sync(bar_id, 128);
 
       // ------------------------------------------------------------------ epilogue
       // Instantiated per set of layer flags (a compile-time constant for the sets the networks use): with no branches in
       // the unrolled column loop the compiler batches the bias / head loads ahead of the dependent adds and stores.
       auto epilogue = [&](auto flags) {
         float rgb[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+        if (NSPLIT == 1 && !(flags & LF_OUT_ACT)) clear_afrag(0, 4);
 #pragma unroll
         for (int nh = 0; nh < 2; ++nh) {
-          if (nh >= L.n_half) break;
+          if (nh >= L.n_half) {
+            if (NSPLIT == 1 && (flags & LF_OUT_ACT)) clear_afrag(2 * nh, 4);
+            break;
+          }
 #pragma unroll
           for (int i = 0; i < 16; ++i) {
             const int col = nh * 128 + 8 * i + cq;
@@ -229,10 +283,14 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
                 alpha[rr] = fmaf(v1, w.y, fmaf(v0, w.x, alpha[rr]));
               }
               if (flags & LF_OUT_ACT) {
-                const uint32_t off = uint32_t(L.out_blk0 + (col >> 6)) * kBlkBytes + sw128_offset(uint32_t(row), uint32_t(col & 63));
                 const uint32_t hi = bf16x2(v0, v1);
-                *reinterpret_cast<uint32_t*>(act + off) = hi;
-                if (NSPLIT == 2) *reinterpret_cast<uint32_t*>(act + NB * kBlkBytes + off) = bf16x2_lo(v0, v1, hi);
+                if (NSPLIT == 1) {
+                  afrag[2 * nh + (i >> 3)][(i >> 1) & 3][2 * (i & 1) + rr] = hi;   // ptx.cuh: wgmma_m64n128_bf16_rs
+                } else {
+                  const uint32_t off = uint32_t(col >> 6) * kBlkBytes + sw128_offset(uint32_t(row), uint32_t(col & 63));
+                  *reinterpret_cast<uint32_t*>(act + off) = hi;
+                  *reinterpret_cast<uint32_t*>(act + NB * kBlkBytes + off) = bf16x2_lo(v0, v1, hi);
+                }
               }
               if (flags & LF_FINAL_RGB) {
 #pragma unroll
@@ -280,8 +338,10 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
           copy_rows(in_tiles + size_t(t) * prog.in.tile_bytes() + prog.in.blk_off(0, prog.in_nblk0), blk_addr(0, 0), 1, wg, tw);
         }
       }
-      fence_proxy_async_smem();        // generic-proxy stores -> visible to the next layer's wgmma reads
-      named_bar_sync(bar_id, 128);
+      if (NSPLIT == 2 || (L.flags & LF_LOAD_IN1_AFTER)) {
+        fence_proxy_async_smem();        // generic-proxy stores -> visible to the next layer's wgmma reads
+        named_bar_sync(bar_id, 128);
+      }
     }
   }
 }

@@ -5,9 +5,10 @@
 //     (TMA engine), pre-packed on the host as K-major SWIZZLE_128B tiles in consumption order,
 //   * activations never leave the SM: two consumer warpgroups each own 64 rows of the tile, accumulate
 //     a layer in registers (wgmma m64n128k16, one 64-register accumulator per 128-column N half), add
-//     bias / ReLU, round to bf16 (optionally a hi+lo split) and write the next layer's A operand
-//     straight into swizzled shared memory; a warpgroup only ever touches its own rows, so the layers
-//     of one warpgroup need no synchronisation with the other beyond the shared weight ring,
+//     bias / ReLU, round to bf16 and keep the result as the next layer's A operand: in registers for plain
+//     bf16 nets (the accumulator fragment is the register-A fragment, 64 registers at W = 256), in
+//     swizzled shared memory as a hi+lo split for the split-precision net; a warpgroup only ever touches its own
+//     rows, so the layers of one warpgroup need no synchronisation with the other beyond the shared weight ring,
 //   * warp roles: warpgroups 0, 1 = consumers, warpgroup 2 = weight producer (one thread issues the copies); the
 //     producer hands most of its registers to the consumers (setmaxnreg), whose accumulators take 128 per thread.
 //
@@ -35,18 +36,21 @@ enum : uint8_t {
   LF_OUT_ACT = 4,        // write bf16 activations for the next layer
   LF_FINAL_RAW = 8,      // write fp32 rows to global (sampling net output / test programs)
   LF_FINAL_RGB = 16,     // rgb_linear on CUDA cores + write float4 (rgb, alpha)
-  LF_LOAD_IN1_AFTER = 32,  // once this layer's MMAs are done, fetch the input block after the tile-start ones (view dirs)
-  LF_WAIT_IN = 64          // this layer reads that 2nd input block
+  LF_LOAD_IN1_AFTER = 32   // once this layer's MMAs are done, fetch the input block after the tile-start ones (view dirs)
 };
 
+// Where a layer's A operand comes from, in K order: in_first input blocks (activation blocks 0, 1) in shared memory, then
+// n_hid hidden blocks, then input block 0 when in_last; n_kb = in_first + n_hid + in_last.  With NSPLIT == 1 (the shading
+// net, and the plain bf16 sampling net) the hidden blocks are in the registers the previous layer's epilogue wrote; the
+// split-precision sampling net (NSPLIT == 2) keeps them as activation blocks 0 .. n_hid - 1, which each epilogue
+// overwrites in place, so there K block kb reads activation block kb.
 struct MlpLayer {
   uint32_t w_off;     // byte offset of this layer's packed weight stages (N half outermost, then K block)
   uint32_t bias_off;  // float offset of the fp32 bias vector in MlpProgram::side
   uint8_t n_kb;       // number of 64-wide K blocks
-  uint8_t a_blk[6];   // activation block index per K block
+  uint8_t in_first, n_hid, in_last;   // 0-2, 0 or W / 64, 0 / 1
   uint8_t n_half;     // N / 128  (1 or 2)
   uint8_t flags;
-  uint8_t out_blk0;   // first activation block the epilogue writes
   // 16-wide K steps issued per K block (4 = the whole 64-wide block; fewer when the tail columns of the block are zero
   // padding, e.g. 90 input features -> blocks of 4 and 2 steps; 30 features -> 2 and 0).
   uint8_t k_cnt[6];

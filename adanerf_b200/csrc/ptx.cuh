@@ -114,8 +114,8 @@ template <int N>
 __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // ------------------------------------------------------------------------------------ wgmma
-// Warpgroup MMA (sm_90a): D[64 x 128] (fp32, registers) += A[64 x 16] * B[128 x 16]^T, A and B bf16 K-major in shared
-// memory, issued by all 128 threads of a warpgroup.  Accumulator fragment of thread t (warp w = t / 32, lane l):
+// Warpgroup MMA (sm_90a): D[64 x 128] (fp32, registers) += A[64 x 16] * B[128 x 16]^T, B (and, in the first form, A) bf16
+// K-major in shared memory, issued by all 128 threads of a warpgroup.  Accumulator fragment of thread t (warp w = t / 32, lane l):
 // d[4 i + j] is row 16 w + l / 4 + 8 (j >> 1), column 8 i + 2 (l % 4) + (j & 1).
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -141,6 +141,32 @@ __device__ __forceinline__ void wgmma_m64n128_bf16(float (&d)[64], uint64_t a_de
         "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
         "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "l"(a_desc), "l"(b_desc), "r"(accumulate)
+      : "memory");
+}
+
+// The same MMA with A from registers (SASS: HGMMA with a register A operand).  Fragment of thread t (warp w, lane l):
+// a[0] = A[16 w + l / 4][2 (l % 4) + {0, 1}], a[1] = the same columns of row + 8, a[2] / a[3] = columns + 8 of those rows,
+// bf16 pairs, lower column in the low half.  For columns 16 j .. 16 j + 15 of a finished accumulator d that is
+// a = {bf16x2(d[8j], d[8j+1]), bf16x2(d[8j+2], d[8j+3]), bf16x2(d[8j+4], d[8j+5]), bf16x2(d[8j+6], d[8j+7])}: a layer's
+// output feeds the next layer's MMAs without leaving the registers.
+__device__ __forceinline__ void wgmma_m64n128_bf16_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "{%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+        "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+        "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+        "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+        "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate)
       : "memory");
 }
 
