@@ -47,6 +47,13 @@ class B200Inference:
                      z_near=f1.z_near, z_far=f1.z_far)
         if getattr(f1, "useNDC", False):    # configs/*_ndc.ini: ndc_rays(self.h, self.w, self.view.focal, 1., ...) (features.py:430)
             scene.update(use_ndc=True, w=int(f1.w), h=int(f1.h), focal=float(info.view.focal))
+        # posEnc / posEncArgs of each net, as its FeatureSet holds them (enc_type, n_freq_pos, n_freq_dir; features.py:326-339):
+        # posEnc none ignores the band counts (-1 / -1).  The sampling net's fields take -1 for zero bands, since 0 there
+        # means "the shading net's count".
+        for f, (kp, kd), zero in ((f1, ("n_freq_pos", "n_freq_dir"), 0), (train_config.f_in[0], ("n_freq_pos0", "n_freq_dir0"), -1)):
+            if hasattr(f, "enc_type"):
+                p, d = (-1, -1) if f.enc_type == "none" else (int(f.n_freq_pos), int(f.n_freq_dir))
+                scene.update({kp: p if p > 0 else min(p, zero), kd: d if d > 0 else min(d, zero)})
         return scene, [train_config.models[0], train_config.models[1]], float(f1.z_sampler.threshold), int(f1.n_ray_samples)
 
     @classmethod

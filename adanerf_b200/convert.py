@@ -8,7 +8,11 @@ without instantiating the reference's classes, so trained checkpoints run throug
 `Renderer.from_export_dir` and `adn_viewer_headless`.
 
     python -m adanerf_b200.convert --weights0 Net0_opt.weights --weights1 Net1_opt.weights \
-        --dataset-info dataset_info.txt --threshold 0.2 --samples 8 --out export_dir
+        --dataset-info dataset_info.txt --threshold 0.2 --samples 8 --out export_dir \
+        [--pos-enc nerf,nerf --pos-enc-args 10-4,10-4]
+
+The run's posEnc / posEncArgs (sampling net, shading net) go on the command line: the sampling net's split into position
+and direction bands cannot be read from the width of layers.0.
 """
 import argparse
 import ast
@@ -17,6 +21,7 @@ from collections import OrderedDict
 import torch
 
 from .onnx_weights import net_shapes, write_export_dir
+from .renderer import enc_columns
 
 SAMPLING_KEYS = ("layers.0.weight", "layers.0.bias")
 SHADING_KEYS = ("pts_linears.0.weight", "views_linears.0.weight", "feature_linear.weight", "alpha_linear.weight",
@@ -40,10 +45,35 @@ def load_weights_file(path, allow_pickle=False):
     return OrderedDict((k, v.detach().to(torch.float32).contiguous()) for k, v in obj.items() if torch.is_tensor(v))
 
 
-def check_state_dicts(sd0, sd1):
+def parse_encoding(pos_enc=("nerf", "nerf"), pos_enc_args=("10-4", "10-4")):
+    """config.ini's posEnc / posEncArgs pairs (sampling net, shading net) -> ((P0, D0), (P, D)) band counts, -1 / -1 for
+    posEnc none (whatever posEncArgs says, as NoEncoding ignores it; features.py:326-339).  Raises ValueError outside the
+    supported encodings: shading net at most 20-10 bands, sampling net at most 20 bands in all."""
+    out = []
+    for e, a in zip(pos_enc, pos_enc_args):
+        if e == "none" or a == "none":
+            out.append((-1, -1))
+        elif e == "nerf":
+            try:
+                p, d = (int(x) for x in a.split("-"))
+            except ValueError:
+                raise ValueError(f"posEncArgs {a!r}: expected P-D band counts") from None
+            out.append((p, d))
+        else:
+            raise ValueError(f"posEnc {e!r}: only nerf and none are supported")
+    (p0, d0), (p, d) = out
+    if max(p, 0) > 20 or max(d, 0) > 10 or max(p0, 0) + max(d0, 0) > 20:
+        raise ValueError(f"posEncArgs {list(pos_enc_args)} is outside the supported encodings "
+                         "(shading net at most 20-10 bands, sampling net at most 20 bands in all)")
+    return tuple(out)
+
+
+def check_state_dicts(sd0, sd1, encoding=None):
     """The architecture the hot path implements: BaseNet sampling net, NeRF shading net with a view branch, in the shapes
     adn_set_weights accepts (include/adanerf_b200.h): sampling net 1-12 layers of hidden width 128 or 256, 128 outputs,
     no skips; shading net 1-10 pts layers of width W = 128 or 256, at most one skip, view branch W/2.
+    encoding: parse_encoding's ((P0, D0), (P, D)); the input columns must be those of that encoding.  None: posEncArgs
+    [10-4, 10-4] or [2-2, 10-4].
     Returns net_shapes(sd0, sd1); raises ValueError naming the offending tensor."""
     for k in SAMPLING_KEYS:
         if k not in sd0:
@@ -51,10 +81,23 @@ def check_state_dicts(sd0, sd1):
     for k in SHADING_KEYS:
         if k not in sd1:
             raise ValueError(f"shading net: missing {k} (expected NeRF with use_viewdirs, src/models.py:214-250)")
-    if sd0["layers.0.weight"].shape[1] not in (90, 30) or sd1["pts_linears.0.weight"].shape[1] != 63:
-        raise ValueError(f"layers.0.weight / pts_linears.0.weight read {sd0['layers.0.weight'].shape[1]} / "
-                         f"{sd1['pts_linears.0.weight'].shape[1]} columns: posEncArgs other than [10-4, 10-4] / [2-2, 10-4] "
-                         "(90 or 30 / 63+27 input features) are not supported")
+    if encoding is None:
+        n_p, n_v = 63, 27
+        if sd0["layers.0.weight"].shape[1] not in (90, 30) or sd1["pts_linears.0.weight"].shape[1] != 63:
+            raise ValueError(f"layers.0.weight / pts_linears.0.weight read {sd0['layers.0.weight'].shape[1]} / "
+                             f"{sd1['pts_linears.0.weight'].shape[1]} columns: posEncArgs other than [10-4, 10-4] / [2-2, 10-4] "
+                             "(90 or 30 / 63+27 input features) are not supported")
+        enc = "posEnc 10-4"
+    else:
+        (p0, d0), (p, d) = encoding
+        n0, n_p, n_v = enc_columns(p0) + enc_columns(d0), enc_columns(p), enc_columns(d)
+        enc = "posEnc " + ("none" if p < 0 and d < 0 else f"{max(p, 0)}-{max(d, 0)}")
+        if sd0["layers.0.weight"].shape[1] != n0:
+            raise ValueError(f"sampling net: layers.0.weight reads {sd0['layers.0.weight'].shape[1]} columns, expected {n0} "
+                             f"for posEncArgs {max(p0, 0)}-{max(d0, 0)}")
+        if sd1["pts_linears.0.weight"].shape[1] != n_p:
+            raise ValueError(f"shading net: pts_linears.0.weight reads {sd1['pts_linears.0.weight'].shape[1]} columns, "
+                             f"expected {n_p} for {enc}")
     shapes = net_shapes(sd0, sd1)
     (d0, w0, _), (d1, w1, _) = shapes
 
@@ -78,13 +121,13 @@ def check_state_dicts(sd0, sd1):
     n_skips = 0
     for i in range(1, d1):
         k = int(sd1[f"pts_linears.{i}.weight"].shape[1])
-        n_skips += int(k == w1 + 63)
+        n_skips += int(k == w1 + n_p)
         if n_skips > 1:
             raise ValueError(f"shading net: pts_linears.{i}.weight reads cat[pts, h] a second time; at most one skip is supported")
-        expect(sd1, f"pts_linears.{i}.weight", w1, k if k == w1 + 63 else w1, f"shading net (W = {w1}, a skip reads W + 63)")
-    for name, rows, cols in (("feature_linear", w1, w1), ("alpha_linear", 1, w1), ("views_linears.0", w1 // 2, w1 + 27),
+        expect(sd1, f"pts_linears.{i}.weight", w1, k if k == w1 + n_p else w1, f"shading net (W = {w1}, a skip reads W + {n_p})")
+    for name, rows, cols in (("feature_linear", w1, w1), ("alpha_linear", 1, w1), ("views_linears.0", w1 // 2, w1 + n_v),
                              ("rgb_linear", 3, w1 // 2)):
-        expect(sd1, name + ".weight", rows, cols, f"shading net (W = {w1}, posEnc 10-4)")
+        expect(sd1, name + ".weight", rows, cols, f"shading net (W = {w1}, {enc})")
     return shapes
 
 
@@ -103,9 +146,14 @@ def read_dataset_info(path):
     return {k: vals[k] for k in need}
 
 
-def weights_to_export_dir(weights0, weights1, out_dir, scene, threshold, num_samples, allow_pickle=False):
+def weights_to_export_dir(weights0, weights1, out_dir, scene, threshold, num_samples, allow_pickle=False, encoding=None):
+    """encoding: parse_encoding's band counts; None keeps the scene's (posEncArgs [10-4, 10-4] unless it says otherwise)."""
     sd0, sd1 = load_weights_file(weights0, allow_pickle), load_weights_file(weights1, allow_pickle)
-    check_state_dicts(sd0, sd1)
+    if encoding is not None:
+        (p0, d0), (p, d) = encoding
+        # the sampling net's 0 means "the shading net's count" in the scene: zero bands are -1 there
+        scene = dict(scene, n_freq_pos=p, n_freq_dir=d, n_freq_pos0=p0 if p0 > 0 else -1, n_freq_dir0=d0 if d0 > 0 else -1)
+    check_state_dicts(sd0, sd1, encoding)
     write_export_dir(out_dir, scene, sd0, sd1, float(threshold), int(num_samples))
     return sd0, sd1
 
@@ -120,8 +168,15 @@ def main(argv=None):
     ap.add_argument("--out", required=True)
     ap.add_argument("--allow-pickle", action="store_true",
                     help="also read checkpoints that hold a pickled nn.Module (executes code from the file: trusted files only)")
+    ap.add_argument("--pos-enc", default=None, help="posEnc of the run, sampling net then shading net: nerf,nerf (default) or none")
+    ap.add_argument("--pos-enc-args", default=None, help="posEncArgs of the run, e.g. 10-4,10-4 (default) or 16-4,6-2")
     a = ap.parse_args(argv)
-    weights_to_export_dir(a.weights0, a.weights1, a.out, read_dataset_info(a.dataset_info), a.threshold, a.samples, a.allow_pickle)
+    encoding = None
+    if a.pos_enc is not None or a.pos_enc_args is not None:
+        split = lambda v, d: tuple(x.strip() for x in (v or d).strip("[]").split(","))
+        encoding = parse_encoding(split(a.pos_enc, "nerf,nerf"), split(a.pos_enc_args, "10-4,10-4"))
+    weights_to_export_dir(a.weights0, a.weights1, a.out, read_dataset_info(a.dataset_info), a.threshold, a.samples, a.allow_pickle,
+                          encoding)
     print(f"wrote {a.out}")
 
 

@@ -67,7 +67,7 @@ struct adn_ctx {
   Net net[2];
   int mlp0_terms = 3;
   int n_feat0 = 90;               // sampling-net input features: 6 + 6 (n_freq_pos0 + n_freq_dir0)
-  bool fuse_encoder = false;      // stage 3 inside the shading kernel: saves the [M, 90]-sized tile buffer
+  bool fuse_encoder = false;      // stage 3 inside the shading kernel: saves the [M, n_in]-sized tile buffer
   int64_t chunk_rays = 0;
   bool profile = false;
   int64_t sample_budget = 0;      // B of adn_set_option "sample_budget" (0 = off)
@@ -284,10 +284,12 @@ adn_status build_net0(adn_ctx* ctx) {
   return ADN_OK;
 }
 
-// Shading net: NeRF(D, W, skips, use_viewdirs=True) (src/models.py:199-277) with posEnc 10-4 (63 position + 27 direction
-// features).  D = 1-10 pts_linears (D + feature + view layer <= kMaxLayers), W = 128 or 256, the view branch W/2.  A skip
-// after pts layer i shows as pts_linears.{i+1} reading W + 63 columns, cat[pts, h] (models.py:226-228, 260-261); at most
-// one.  The program, the input block P (then V) in shared memory and the W/64 hidden blocks in the consumers' registers:
+// Shading net: NeRF(D, W, skips, use_viewdirs=True) (src/models.py:199-277) with the scene's encoding: kP = 3 + 6 P position
+// and kV = 3 + 6 D direction features (input_ch / input_ch_views, models.py:216-224; 63 + 27 for posEnc 10-4).  D = 1-10
+// pts_linears (D + feature + view layer <= kMaxLayers), W = 128 or 256, the view branch W/2.  A skip after pts layer i
+// shows as pts_linears.{i+1} reading W + kP columns, cat[pts, h] (models.py:226-228, 260-261); at most one.  The program,
+// the input blocks P (one, or two when kP > 64; then V) in shared memory and the W/64 hidden blocks in the consumers'
+// registers:
 //   pts layer 0 reads P; the skip consumer reads P, then the hidden blocks; the other pts layers read the hidden blocks; the
 //   last pts layer also forms alpha (LF_ALPHA_DOT); V replaces P after the skip consumer, or after layer 0 without a skip;
 //   feature_linear: W -> W without activation; views_linears.0 on cat[feature, V] -> W/2 reads the hidden blocks, then V,
@@ -296,12 +298,16 @@ adn_status build_net0(adn_ctx* ctx) {
 // rgb_linear columns: ReLU(0) = 0 adds nothing to the rgb dot products, so the result is exact.
 adn_status build_net1(adn_ctx* ctx) {
   Net& net = ctx->net[1];
-  constexpr int kP = 63, kV = 27;
+  const int kP = 3 + 6 * ctx->sc.n_freq_pos, kV = 3 + 6 * ctx->sc.n_freq_dir;
+  const std::string enc = "posEnc " + (ctx->scene.n_freq_pos < 0 && ctx->scene.n_freq_dir < 0
+                                           ? std::string("none")
+                                           : std::to_string(ctx->sc.n_freq_pos) + "-" + std::to_string(ctx->sc.n_freq_dir));
   auto bad = [&](const std::string& msg) { return fail(ctx, ADN_ERR_INVALID, "shading net: " + msg); };
   auto shape = [](int64_t r, int64_t c) { return "[" + std::to_string(r) + ", " + std::to_string(c) + "]"; };
   const HostTensor* w0 = find(net, "pts_linears.0.weight");
   if (!w0 || w0->cols != kP)
-    return bad("pts_linears.0.weight must be [W, 63] (posEnc 10-4)" + (w0 ? ", not " + shape(w0->rows, w0->cols) : std::string(", missing")));
+    return bad("pts_linears.0.weight must be [W, " + std::to_string(kP) + "] (" + enc + ")" +
+               (w0 ? ", not " + shape(w0->rows, w0->cols) : std::string(", missing")));
   const int W = int(w0->rows);
   if (W != 128 && W != 256) return bad("pts_linears.0.weight has " + std::to_string(W) + " rows; the width W must be 128 or 256");
   int D = 0;
@@ -320,7 +326,7 @@ adn_status build_net1(adn_ctx* ctx) {
       skip = i - 1;
     } else if (i > 0 && pw[i]->cols != W) {
       return bad(name + ".weight has " + std::to_string(pw[i]->cols) + " input columns; expect W = " + std::to_string(W) +
-                 " or W + 63 = " + std::to_string(W + kP) + " (a skip)");
+                 " or W + " + std::to_string(kP) + " = " + std::to_string(W + kP) + " (a skip, " + enc + ")");
     }
     if (!pb[i] || int64_t(pb[i]->data.size()) != W) return bad(name + ".bias is missing or not [" + std::to_string(W) + "]");
   }
@@ -335,7 +341,7 @@ adn_status build_net1(adn_ctx* ctx) {
     hw[j] = find(net, name + ".weight");
     hb[j] = find(net, name + ".bias");
     if (!hw[j] || hw[j]->rows != want[j].rows || hw[j]->cols != want[j].cols)
-      return bad(name + ".weight must be " + shape(want[j].rows, want[j].cols) + " for W = " + std::to_string(W) + " (posEnc 10-4)" +
+      return bad(name + ".weight must be " + shape(want[j].rows, want[j].cols) + " for W = " + std::to_string(W) + " (" + enc + ")" +
                  (hw[j] ? ", not " + shape(hw[j]->rows, hw[j]->cols) : std::string(", missing")));
     if (!hb[j] || int64_t(hb[j]->data.size()) != want[j].rows) return bad(name + ".bias is missing or not [" + std::to_string(want[j].rows) + "]");
   }
@@ -351,7 +357,10 @@ adn_status build_net1(adn_ctx* ctx) {
   for (int l = 0; l < D + 2; ++l) {
     MlpLayer& L = P.layers[l];
     std::vector<Seg> segs;
-    auto read_p = [&] { segs.push_back({0, kP}), L.in_first = 1; };
+    auto read_p = [&] {
+      for (int c = 0; c < kP; c += 64) segs.push_back({c, std::min(64, kP - c)});
+      L.in_first = uint8_t(shading_p_blocks(kP));
+    };
     auto read_hidden = [&](int col0) {
       for (int b = 0; b < nh; ++b) segs.push_back({col0 + 64 * b, 64});
       L.n_hid = uint8_t(nh);
@@ -398,8 +407,8 @@ adn_status build_net1(adn_ctx* ctx) {
   P.alpha_b_off = uint32_t(push_floats(fblob, ab->data.data(), 1));
   P.rgb_w_off = uint32_t(push_floats(fblob, rgb_w.data(), rgb_w.size()));
   P.rgb_b_off = uint32_t(push_floats(fblob, rb->data.data(), 3));
-  P.in = shading_tiles();
-  P.in_nblk0 = 1;   // P; V after layer load_v
+  P.in = shading_tiles(kP, kV);
+  P.in_nblk0 = shading_p_blocks(kP);   // P; V after layer load_v
   P.out_cols = 4;
   net.prog = P;
   adn_status s = upload(ctx, net, wblob, fblob);
@@ -748,10 +757,13 @@ adn_status adn_create(adn_ctx** out, const adn_scene* scene, int device) {
   cudaDeviceProp prop{};
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return ADN_ERR_NO_DEVICE;
   if (prop.major != 9) return ADN_ERR_NO_DEVICE;  // wgmma / setmaxnreg kernels (sm_90a): Hopper only, no fallback
-  if (scene->n_freq_pos != 10 || scene->n_freq_dir != 4) return ADN_ERR_INVALID;  // posEncArgs[1] "10-4" (F = 90)
-  const int nfp0 = scene->n_freq_pos0 ? scene->n_freq_pos0 : scene->n_freq_pos;
-  const int nfd0 = scene->n_freq_dir0 ? scene->n_freq_dir0 : scene->n_freq_dir;
-  if (!((nfp0 == 10 && nfd0 == 4) || (nfp0 == 2 && nfd0 == 2))) return ADN_ERR_INVALID;   // posEncArgs[0] "10-4" or "2-2"
+  // Band counts; a negative one is posEnc none, the same features as 0 bands.  The sampling net's fields default (0) to
+  // the shading net's.  The limits are those of the packed tile formats (tiles.cuh): the shading net's position block at
+  // most 2 x 64 columns (3 + 6 P), its view block at most 64 (3 + 6 D), the sampling net's 6 + 6 (P0 + D0) at most 128.
+  const int nfp = std::max(0, scene->n_freq_pos), nfd = std::max(0, scene->n_freq_dir);
+  const int nfp0 = std::max(0, scene->n_freq_pos0 ? scene->n_freq_pos0 : scene->n_freq_pos);
+  const int nfd0 = std::max(0, scene->n_freq_dir0 ? scene->n_freq_dir0 : scene->n_freq_dir);
+  if (nfp > 20 || nfd > 10 || nfp0 + nfd0 > 20) return ADN_ERR_INVALID;
   if (scene->use_ndc && (scene->ndc_w < 0 || scene->ndc_h < 0)) return ADN_ERR_INVALID;
   adn_ctx* ctx = new adn_ctx();
   ctx->device = device;
@@ -768,8 +780,8 @@ adn_status adn_create(adn_ctx** out, const adn_scene* scene, int device) {
   const double r = std::sqrt(r2);
   ctx->sc.r2 = float(r * r);
   ctx->sc.sqrt_max_depth = float(std::sqrt(double(scene->max_depth)));
-  ctx->sc.n_freq_pos = scene->n_freq_pos;
-  ctx->sc.n_freq_dir = scene->n_freq_dir;
+  ctx->sc.n_freq_pos = nfp;
+  ctx->sc.n_freq_dir = nfd;
   ctx->sc.n_freq_pos0 = nfp0;
   ctx->sc.n_freq_dir0 = nfd0;
   ctx->n_feat0 = 6 + 6 * (nfp0 + nfd0);

@@ -202,7 +202,39 @@ bool load_export_dir(const std::string& dir_in, ExportDir& out, std::string& err
       dir = std::atoi(it.substr(dash + 1).c_str());
     };
     if (!items.empty()) parse(items.back(), s.n_freq_pos, s.n_freq_dir);
-    if (items.size() >= 2) parse(items.front(), s.n_freq_pos0, s.n_freq_dir0);
+    if (items.size() >= 2) {
+      parse(items.front(), s.n_freq_pos0, s.n_freq_dir0);
+      // in adn_scene a sampling-net count of 0 means "the shading net's": a literal 0 bands (e.g. "0-4") is -1 there
+      if (s.n_freq_pos0 == 0) s.n_freq_pos0 = -1;
+      if (s.n_freq_dir0 == 0) s.n_freq_dir0 = -1;
+    }
+  }
+  // posEnc = [sampling net, shading net] (config.cpp:209-210): nerf, or none -- the identity, whatever posEncArgs says
+  // (NoEncoding ignores the band counts); recorded as -1 / -1 (the reference's own convention, features.py:326-328)
+  auto penc = cfg.find("posEnc");
+  if (penc != cfg.end()) {
+    const auto items = list_items(penc->second);
+    for (size_t k = 0; k < items.size() && k < 2; ++k) {
+      const bool shading = k == 0;   // the last item, then the first
+      const std::string& e = items[items.size() - 1 - k];
+      if (e == "none") {
+        (shading ? s.n_freq_pos : s.n_freq_pos0) = -1;
+        (shading ? s.n_freq_dir : s.n_freq_dir0) = -1;
+      } else if (e != "nerf") {
+        err = "config.ini: posEnc = " + strip(penc->second) + ": only nerf and none are supported";
+        return false;
+      }
+    }
+  }
+  {
+    // the limits of the packed input tiles (adn_create): shading P <= 20 and D <= 10 bands, sampling P0 + D0 <= 20
+    const int p = std::max(0, s.n_freq_pos), d = std::max(0, s.n_freq_dir);
+    const int p0 = std::max(0, s.n_freq_pos0 ? s.n_freq_pos0 : s.n_freq_pos), d0 = std::max(0, s.n_freq_dir0 ? s.n_freq_dir0 : s.n_freq_dir);
+    if (p > 20 || d > 10 || p0 + d0 > 20) {
+      err = "config.ini: posEncArgs = " + (pe != cfg.end() ? strip(pe->second) : std::string("?")) +
+            " is outside the supported encodings (shading net at most 20-10 bands, sampling net at most 20 bands in all)";
+      return false;
+    }
   }
   auto ndc = cfg.find("useNDC");
   s.use_ndc = (ndc != cfg.end() && strip(ndc->second) == "True") ? 1 : 0;   // config.cpp:265-266

@@ -88,9 +88,16 @@ int main(int argc, char** argv) {
   }
   adn_host::ImageGenerator gen;
   if (!gen.load(config, device)) { std::fprintf(stderr, "load failed: %s\n", gen.last_error()); return 1; }
+  adn_scene sc{};
+  const bool probed = adn_probe_export_dir(model.c_str(), &sc, nullptr, nullptr, nullptr) == ADN_OK;
   for (int id = 0; id < 2; ++id) {
     int d = 0, w = 0, sk = -1;
-    if (gen.net_shape(id, &d, &w, &sk)) std::printf("net %d: %s %d x %d, skip %d\n", id, id == 0 ? "sampling" : "shading", d, w, sk);
+    if (!gen.net_shape(id, &d, &w, &sk)) continue;
+    // the encoding as adn_create reads the scene: a negative band count is posEnc none; the sampling net's 0 = the shading net's
+    const int p = id == 0 && sc.n_freq_pos0 ? sc.n_freq_pos0 : sc.n_freq_pos, q = id == 0 && sc.n_freq_dir0 ? sc.n_freq_dir0 : sc.n_freq_dir;
+    char enc[32] = "?";
+    if (probed) std::snprintf(enc, sizeof(enc), p < 0 && q < 0 ? "none" : "%d-%d", p < 0 ? 0 : p, q < 0 ? 0 : q);
+    std::printf("net %d: %s %d x %d, skip %d, posEnc %s\n", id, id == 0 ? "sampling" : "shading", d, w, sk, enc);
   }
   if (budget > 0 && !gen.set_sample_budget(budget)) { std::fprintf(stderr, "sample budget: %s\n", gen.last_error()); return 1; }
   std::vector<int32_t> ns(budget > 0 ? size_t(W) * H : 0);   // per-ray sample counts, for M under a budget

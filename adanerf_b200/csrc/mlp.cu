@@ -29,10 +29,41 @@ struct MlpCfg {
 };
 static_assert(MlpCfg<1>::kSmemBytes <= 232448 && MlpCfg<2>::kSmemBytes <= 232448, "shared memory per block (sm_90)");
 
+// Row `row` of the fused encoder's input blocks for a scene with any encoding but 10-4 (n_freq_pos <= 20, n_freq_dir
+// <= 10 bands): P (3 + 6 n_freq_pos features, in one block or two) into the blocks from `blk` on, or V into block `blk`,
+// each feature written as stage3_kernel<true> writes it, then zeros up to the block's end.
+__device__ __forceinline__ void encode_row_rt(const EncodeParams& enc, long long i, long long rows, uint8_t* blk, int row,
+                                              bool view) {
+  const TileFormat act{1, 2, {0, 64, 0}, {64, 64, 0}};   // consecutive blocks: block b at blk + b * kBlkBytes
+  const int n_p = 3 + 6 * enc.sc.n_freq_pos;
+  zero_row(act, blk, uint32_t(row), 0, view ? 1 : shading_p_blocks(n_p));
+  if (i < rows) {
+    long long ray;
+    float zw;
+    if (enc.ray_idx) {
+      ray = enc.ray_idx[i];
+      zw = enc.z[i];
+    } else {
+      ray = i / enc.K;
+      zw = enc.zlut_dense[i - ray * enc.K];
+    }
+    float pos[3], dir[3];
+    sample_inputs(enc.sc, false, enc.ray_o, enc.ray_d, ray, zw, pos, dir);
+    auto put = [&](int j, float v) { put_feature(act, blk, j >> 6, uint32_t(row), j & 63, v); };
+    if (view) posenc3_rt(dir, enc.sc.n_freq_dir, put);
+    else posenc3_rt(pos, enc.sc.n_freq_pos, put);
+  }
+}
+
 // One row of a fused-encoder input block: P (the 63 position features and a zero column) or V (the 27 direction features
 // and zeros) of the shading tile format, computed and packed as stage3_kernel computes and packs them for a non-NDC scene.
+// Other encodings: encode_row_rt.
 template <bool VIEW>
 __device__ __forceinline__ void encode_row(const EncodeParams& enc, long long i, long long rows, uint8_t* blk, int row) {
+  if (enc.sc.n_freq_pos != 10 || enc.sc.n_freq_dir != 4) {
+    encode_row_rt(enc, i, rows, blk, row, VIEW);
+    return;
+  }
   float f[64];
 #pragma unroll
   for (int k = 0; k < 64; ++k) f[k] = 0.0f;

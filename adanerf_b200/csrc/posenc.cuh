@@ -41,6 +41,29 @@ __device__ __forceinline__ void posenc3(const float (&v)[3], float* out) {
   }
 }
 
+// posenc3 with a run-time band count L >= 0 (posEnc none = 0 bands: v alone): the same operations, so the same bits as
+// posenc3<L>.  Feature j of the 3 + 6L goes to emit(j, value), in no particular order, so no array of them is held.
+template <typename Emit>
+__device__ __forceinline__ void posenc3_rt(const float (&v)[3], int L, Emit emit) {
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    emit(a, v[a]);
+    float s = 0.f, c = 1.f;
+    for (int f = 0; f < L; ++f) {
+      if (f % kAnchor == 0) {
+        sincosf(__fmul_rn(v[a], float(1 << f)), &s, &c);
+      } else {
+        const float s2 = 2.0f * s * c;
+        const float c2 = fmaf(-2.0f * s, s, 1.0f);
+        s = s2;
+        c = c2;
+      }
+      emit(3 + 6 * f + a, s);
+      emit(3 + 6 * f + 3 + a, c);
+    }
+  }
+}
+
 // The shading net's inputs of one sample at world depth zw on ray r (RayMarchFromPoses.batch, src/features.py:458-479), in
 // the reference's operation order: the position into pos and the direction to encode into dir.  Stage 3 and the fused
 // encoder both call this, so their features are the same bits.

@@ -14,6 +14,7 @@
 
 namespace adn {
 
+// posEnc 10-4, the encoding with compile-time kernels (and 2-2 for the sampling net)
 constexpr int kNFreqPos = 10;
 constexpr int kNFreqDir = 4;
 constexpr int kFeat = 90;
@@ -48,7 +49,39 @@ cudaError_t launch_gen_dirs(const CameraRays& cam, long long n_rays, float* d_di
 }
 
 // ------------------------------------------------------------------------------------ stage 0b
-// SpherePosDir.batch (src/features.py:845-899): one thread per ray.
+// SpherePosDir.batch (src/features.py:845-899) up to the encodings: the pixel direction d of ray i, the ray origin p on the
+// view-cell sphere, the rotated direction nds and its unit copy dn.
+template <bool FROM_CAMERA>
+__device__ __forceinline__ void sphere_pos_dir(const SceneDev& sc, const PoseDev& pd, const float* __restrict__ dirs,
+                                               const CameraRays& cam, long long i, float (&p)[3], float (&nds)[3], float (&dn)[3]) {
+  float d[3];
+  if (FROM_CAMERA) {
+    pixel_dir(cam, i, d);
+  } else {
+    d[0] = dirs[3 * i + 0];
+    d[1] = dirs[3 * i + 1];
+    d[2] = dirs[3 * i + 2];
+  }
+  // nds = R * d : ATen bmm with K = 3 accumulates as an FMA chain over k = 0,1,2 (:858-859)
+#pragma unroll
+  for (int r = 0; r < 3; ++r)
+    nds[r] = __fmaf_rn(pd.rot[3 * r + 2], d[2], __fmaf_rn(pd.rot[3 * r + 1], d[1], __fmul_rn(pd.rot[3 * r + 0], d[0])));
+  // compute_ray_offset (:769-791)
+  float omc[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) omc[a] = __fsub_rn(pd.pose[a], sc.c[a]);
+  const float udot = __fadd_rn(__fadd_rn(__fmul_rn(omc[0], nds[0]), __fmul_rn(omc[1], nds[1])), __fmul_rn(omc[2], nds[2]));
+  const float omc2 = __fadd_rn(__fadd_rn(__fmul_rn(omc[0], omc[0]), __fmul_rn(omc[1], omc[1])), __fmul_rn(omc[2], omc[2]));
+  const float delta = __fsub_rn(__fmul_rn(udot, udot), __fsub_rn(omc2, sc.r2));
+  const float t = __fadd_rn(-udot, __fsqrt_rn(fmaxf(delta, 0.0f)));
+#pragma unroll
+  for (int a = 0; a < 3; ++a) p[a] = __fadd_rn(pd.pose[a], __fmul_rn(nds[a], t));
+  const float nn = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(nds[0], nds[0]), __fmul_rn(nds[1], nds[1])), __fmul_rn(nds[2], nds[2])));
+#pragma unroll
+  for (int a = 0; a < 3; ++a) dn[a] = __fdiv_rn(nds[a], nn);
+}
+
+// One thread per ray, the encodings "10-4" or "2-2" at compile time.
 template <bool FROM_CAMERA, int NFD = kNFreqDir, int NFP = kNFreqPos>
 __global__ void __launch_bounds__(128)
 stage0_kernel(const __grid_constant__ SceneDev sc, const __grid_constant__ PoseDev pd, const float* __restrict__ dirs,
@@ -60,34 +93,8 @@ stage0_kernel(const __grid_constant__ SceneDev sc, const __grid_constant__ PoseD
 #pragma unroll
   for (int j = 0; j < F0; ++j) f[j] = 0.0f;
   if (i < n_rays) {
-    float d[3];
-    if (FROM_CAMERA) {
-      pixel_dir(cam, i, d);
-    } else {
-      d[0] = dirs[3 * i + 0];
-      d[1] = dirs[3 * i + 1];
-      d[2] = dirs[3 * i + 2];
-    }
-    // nds = R * d : ATen bmm with K = 3 accumulates as an FMA chain over k = 0,1,2 (:858-859)
-    float nds[3];
-#pragma unroll
-    for (int r = 0; r < 3; ++r)
-      nds[r] = __fmaf_rn(pd.rot[3 * r + 2], d[2], __fmaf_rn(pd.rot[3 * r + 1], d[1], __fmul_rn(pd.rot[3 * r + 0], d[0])));
-    // compute_ray_offset (:769-791)
-    float omc[3];
-#pragma unroll
-    for (int a = 0; a < 3; ++a) omc[a] = __fsub_rn(pd.pose[a], sc.c[a]);
-    const float udot = __fadd_rn(__fadd_rn(__fmul_rn(omc[0], nds[0]), __fmul_rn(omc[1], nds[1])), __fmul_rn(omc[2], nds[2]));
-    const float omc2 = __fadd_rn(__fadd_rn(__fmul_rn(omc[0], omc[0]), __fmul_rn(omc[1], omc[1])), __fmul_rn(omc[2], omc[2]));
-    const float delta = __fsub_rn(__fmul_rn(udot, udot), __fsub_rn(omc2, sc.r2));
-    const float t = __fadd_rn(-udot, __fsqrt_rn(fmaxf(delta, 0.0f)));
-    float p[3];
-#pragma unroll
-    for (int a = 0; a < 3; ++a) p[a] = __fadd_rn(pd.pose[a], __fmul_rn(nds[a], t));
-    const float nn = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(nds[0], nds[0]), __fmul_rn(nds[1], nds[1])), __fmul_rn(nds[2], nds[2])));
-    float dn[3];
-#pragma unroll
-    for (int a = 0; a < 3; ++a) dn[a] = __fdiv_rn(nds[a], nn);
+    float p[3], nds[3], dn[3];
+    sphere_pos_dir<FROM_CAMERA>(sc, pd, dirs, cam, i, p, nds, dn);
     posenc3<NFD>(dn, f);                           // 27 / 15: direction block FIRST (:868)
     posenc3<NFP>(p, f + 3 + 6 * NFD);              // 63 / 15
     if (ray_o) {
@@ -110,6 +117,42 @@ stage0_kernel(const __grid_constant__ SceneDev sc, const __grid_constant__ PoseD
   }
 }
 
+// Any other encoding (sc.n_freq_dir0 + sc.n_freq_pos0 <= 20 bands, 0 = posEnc none): the same features, written one at a
+// time into x0 and the tile image, so no thread holds its up to 126 features at once.
+template <bool FROM_CAMERA>
+__global__ void __launch_bounds__(128)
+stage0_rt_kernel(const __grid_constant__ SceneDev sc, const __grid_constant__ PoseDev pd, const float* __restrict__ dirs,
+                 const __grid_constant__ CameraRays cam, long long n_rays, float* __restrict__ x0, float* __restrict__ ray_o,
+                 float* __restrict__ ray_d, uint8_t* __restrict__ tiles0, int tile_terms) {
+  const int nfd = sc.n_freq_dir0, nfp = sc.n_freq_pos0;
+  const int F0 = 6 + 6 * (nfd + nfp);
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;   // grid covers whole 128-ray tiles
+  extern __shared__ __align__(1024) uint8_t s_tile[];
+  const TileFormat fmt = sampling_tiles(F0, tile_terms);
+  if (tiles0) zero_row(fmt, s_tile, threadIdx.x, 0, fmt.n_blk);
+  if (i < n_rays) {
+    float p[3], nds[3], dn[3];
+    sphere_pos_dir<FROM_CAMERA>(sc, pd, dirs, cam, i, p, nds, dn);
+    auto put = [&](int c, float v) {
+      if (x0) x0[i * F0 + c] = v;
+      if (tiles0) put_feature(fmt, s_tile, c >> 6, threadIdx.x, c & 63, v);
+    };
+    posenc3_rt(dn, nfd, put);                                             // direction block FIRST (:868)
+    posenc3_rt(p, nfp, [&](int j, float v) { put(3 + 6 * nfd + j, v); });
+    if (ray_o) {
+#pragma unroll
+      for (int a = 0; a < 3; ++a) {
+        ray_o[3 * i + a] = p[a];
+        ray_d[3 * i + a] = nds[a];
+      }
+    }
+  }
+  if (tiles0) {
+    flush_tile(fmt, s_tile, tiles0 + size_t(i >> 7) * fmt.tile_bytes());
+    store_tiles_drain();
+  }
+}
+
 cudaError_t launch_stage0(const SceneDev& sc, const PoseDev& pd, const float* d_dirs, const CameraRays* cam,
                           long long n_rays, float* d_x0, float* d_ray_o, float* d_ray_d, uint8_t* d_tiles0, int tile_terms,
                           cudaStream_t s) {
@@ -119,24 +162,20 @@ cudaError_t launch_stage0(const SceneDev& sc, const PoseDev& pd, const float* d_
   CameraRays c{};
   const int tile_bytes = int(sampling_tiles(0, 2).tile_bytes());   // the largest sampling tile
   const size_t smem = d_tiles0 ? sampling_tiles(0, tile_terms).tile_bytes() : 0;
-  static unsigned long long attr_cam = 0, attr_rays = 0;   // per device
-  if (set_max_dyn_smem_once(reinterpret_cast<const void*>(stage0_kernel<true>), tile_bytes, &attr_cam) != cudaSuccess ||
-      set_max_dyn_smem_once(reinterpret_cast<const void*>(stage0_kernel<false>), tile_bytes, &attr_rays) != cudaSuccess)
-    return cudaGetLastError();
   if (cam) c = *cam;
-  if (sc.n_freq_pos0 == 2 && sc.n_freq_dir0 == 2) {   // "2-2" (NDC configs): 30 features
-    static unsigned long long attr_cam22 = 0, attr_rays22 = 0;
-    if (set_max_dyn_smem_once(reinterpret_cast<const void*>(stage0_kernel<true, 2, 2>), tile_bytes, &attr_cam22) != cudaSuccess ||
-        set_max_dyn_smem_once(reinterpret_cast<const void*>(stage0_kernel<false, 2, 2>), tile_bytes, &attr_rays22) != cudaSuccess)
+  // the compile-time encodings where the scene has them, else the run-time one
+  auto run = [&](auto k_cam, auto k_rays, unsigned long long* attr) -> cudaError_t {
+    if (set_max_dyn_smem_once(reinterpret_cast<const void*>(k_cam), tile_bytes, &attr[0]) != cudaSuccess ||
+        set_max_dyn_smem_once(reinterpret_cast<const void*>(k_rays), tile_bytes, &attr[1]) != cudaSuccess)
       return cudaGetLastError();
-    if (cam) stage0_kernel<true, 2, 2><<<grid, 128, smem, s>>>(sc, pd, d_dirs, c, n_rays, d_x0, d_ray_o, d_ray_d, d_tiles0, tile_terms);
-    else stage0_kernel<false, 2, 2><<<grid, 128, smem, s>>>(sc, pd, d_dirs, c, n_rays, d_x0, d_ray_o, d_ray_d, d_tiles0, tile_terms);
-  } else if (cam) {
-    stage0_kernel<true><<<grid, 128, smem, s>>>(sc, pd, d_dirs, c, n_rays, d_x0, d_ray_o, d_ray_d, d_tiles0, tile_terms);
-  } else {
-    stage0_kernel<false><<<grid, 128, smem, s>>>(sc, pd, d_dirs, c, n_rays, d_x0, d_ray_o, d_ray_d, d_tiles0, tile_terms);
-  }
-  return cudaGetLastError();
+    if (cam) k_cam<<<grid, 128, smem, s>>>(sc, pd, d_dirs, c, n_rays, d_x0, d_ray_o, d_ray_d, d_tiles0, tile_terms);
+    else k_rays<<<grid, 128, smem, s>>>(sc, pd, d_dirs, c, n_rays, d_x0, d_ray_o, d_ray_d, d_tiles0, tile_terms);
+    return cudaGetLastError();
+  };
+  static unsigned long long attr104[2] = {0, 0}, attr22[2] = {0, 0}, attr_rt[2] = {0, 0};   // per device
+  if (sc.n_freq_pos0 == kNFreqPos && sc.n_freq_dir0 == kNFreqDir) return run(stage0_kernel<true>, stage0_kernel<false>, attr104);
+  if (sc.n_freq_pos0 == 2 && sc.n_freq_dir0 == 2) return run(stage0_kernel<true, 2, 2>, stage0_kernel<false, 2, 2>, attr22);
+  return run(stage0_rt_kernel<true>, stage0_rt_kernel<false>, attr_rt);
 }
 
 // ------------------------------------------------------------------------------------- stage 2
@@ -873,7 +912,10 @@ cudaError_t launch_stage2_dense(long long n_rays, int K, int32_t* d_count, int32
 }
 
 // ------------------------------------------------------------------------------------- stage 3
-// RayMarchFromPoses.batch (src/features.py:458-479): one thread per packed sample.
+// RayMarchFromPoses.batch (src/features.py:458-479): one thread per packed sample.  RT == false: posEnc 10-4 at compile
+// time.  RT == true: sc.n_freq_pos (<= 20) and sc.n_freq_dir (<= 10) bands, the features written one at a time into x1
+// and the tile image, so no thread holds its up to 123 + 63 features at once.
+template <bool RT>
 __global__ void __launch_bounds__(128)
 stage3_kernel(const __grid_constant__ SceneDev sc, const float* __restrict__ ray_o, const float* __restrict__ ray_d,
               const int32_t* __restrict__ ray_idx, const float* __restrict__ z, const float* __restrict__ zlut_dense, int K,
@@ -881,10 +923,21 @@ stage3_kernel(const __grid_constant__ SceneDev sc, const float* __restrict__ ray
               uint8_t* __restrict__ tiles1) {
   const long long n_samples = n_samples_dev ? *n_samples_dev : n_samples_host;
   const long long n_pad = ((n_samples + kTileM - 1) / kTileM) * kTileM;
+  const int n_p = RT ? 3 + 6 * sc.n_freq_pos : 3 + 6 * kNFreqPos;
+  const int n_v = RT ? 3 + 6 * sc.n_freq_dir : 3 + 6 * kNFreqDir;
+  const TileFormat fmt = shading_tiles(n_p, n_v);
+  extern __shared__ __align__(1024) uint8_t s_tile[];
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n_pad; i += (long long)gridDim.x * blockDim.x) {
-    float f[kFeat];
+    float f[RT ? 1 : kFeat];
+    if (!RT) {
 #pragma unroll
-    for (int j = 0; j < kFeat; ++j) f[j] = 0.0f;
+      for (int j = 0; j < kFeat; ++j) f[j] = 0.0f;
+    }
+    if (RT && tiles1) {
+      if (threadIdx.x == 0) bulk_wait_read_all();   // the previous tile's copy has finished reading s_tile
+      __syncthreads();
+      zero_row(fmt, s_tile, threadIdx.x, 0, fmt.n_blk);
+    }
     if (i < n_samples) {
       long long r;
       float zw;
@@ -897,19 +950,34 @@ stage3_kernel(const __grid_constant__ SceneDev sc, const float* __restrict__ ray
       }
       float pos[3], d[3];
       sample_inputs(sc, sc.ndc != 0, ray_o, ray_d, r, zw, pos, d);
-      posenc3<kNFreqPos>(pos, f);                      // 63: position block FIRST (:473-479)
-      posenc3<kNFreqDir>(d, f + 63);                   // 27
-      if (x1) {
+      if (RT) {
+        const int vb = fmt.n_blk - 1;   // the view block
+        posenc3_rt(pos, sc.n_freq_pos, [&](int j, float v) {   // position block FIRST (:473-479)
+          if (x1) x1[i * (n_p + n_v) + j] = v;
+          if (tiles1) put_feature(fmt, s_tile, j >> 6, threadIdx.x, j & 63, v);
+        });
+        posenc3_rt(d, sc.n_freq_dir, [&](int j, float v) {
+          if (x1) x1[i * (n_p + n_v) + n_p + j] = v;
+          if (tiles1) put_feature(fmt, s_tile, vb, threadIdx.x, j, v);
+        });
+      } else {
+        posenc3<kNFreqPos>(pos, f);                      // 63: position block FIRST (:473-479)
+        posenc3<kNFreqDir>(d, f + 63);                   // 27
+        if (x1) {
 #pragma unroll
-        for (int j = 0; j < kFeat; ++j) x1[i * kFeat + j] = f[j];
+          for (int j = 0; j < kFeat; ++j) x1[i * kFeat + j] = f[j];
+        }
       }
     }
     if (tiles1) {   // the CTA's 128 samples are one tile of the shading net's input
-      extern __shared__ __align__(1024) uint8_t s_tile[];
-      const TileFormat fmt = shading_tiles();
-      if (threadIdx.x == 0) bulk_wait_read_all();   // the previous tile's copy has finished reading s_tile
-      __syncthreads();
-      store_tile(fmt, f, s_tile, tiles1 + size_t(i >> 7) * fmt.tile_bytes());
+      uint8_t* dst = tiles1 + size_t(i >> 7) * fmt.tile_bytes();
+      if (RT) {
+        flush_tile(fmt, s_tile, dst);
+      } else {
+        if (threadIdx.x == 0) bulk_wait_read_all();   // the previous tile's copy has finished reading s_tile
+        __syncthreads();
+        store_tile(fmt, f, s_tile, dst);
+      }
     }
   }
   if (tiles1) store_tiles_drain();
@@ -923,12 +991,16 @@ cudaError_t launch_stage3(const SceneDev& sc, const float* d_ray_o, const float*
   long long blocks = (n_samples + kTileM - 1) / kTileM;
   const long long cap = 64ll * num_sms;
   if (d_total && blocks > cap) blocks = cap;   // grid-stride when the true count lives on the device
-  static unsigned long long attr_done = 0;   // per device
-  const int tile_bytes = int(shading_tiles().tile_bytes());
-  if (set_max_dyn_smem_once(reinterpret_cast<const void*>(stage3_kernel), tile_bytes, &attr_done) != cudaSuccess) return cudaGetLastError();
-  stage3_kernel<<<unsigned(blocks), 128, d_tiles1 ? size_t(tile_bytes) : 0, s>>>(sc, d_ray_o, d_ray_d, d_ray, d_z, d_zlut_dense, K,
-                                                                                      n_samples, d_total, d_x1, d_tiles1);
-  return cudaGetLastError();
+  const int tile_bytes = 3 * kBlkBytes;        // the largest shading tile
+  const size_t smem = d_tiles1 ? shading_tiles(3 + 6 * sc.n_freq_pos, 3 + 6 * sc.n_freq_dir).tile_bytes() : 0;
+  static unsigned long long attr_done[2] = {0, 0};   // per device
+  auto run = [&](auto kernel, unsigned long long* attr) -> cudaError_t {
+    if (set_max_dyn_smem_once(reinterpret_cast<const void*>(kernel), tile_bytes, attr) != cudaSuccess) return cudaGetLastError();
+    kernel<<<unsigned(blocks), 128, smem, s>>>(sc, d_ray_o, d_ray_d, d_ray, d_z, d_zlut_dense, K, n_samples, d_total, d_x1, d_tiles1);
+    return cudaGetLastError();
+  };
+  if (sc.n_freq_pos == kNFreqPos && sc.n_freq_dir == kNFreqDir) return run(stage3_kernel<false>, &attr_done[0]);
+  return run(stage3_kernel<true>, &attr_done[1]);
 }
 
 // ------------------------------------------------------------------------------------- stage 5

@@ -20,21 +20,28 @@ constexpr int kBlkBytes = 16384;  // one [128 x 64] bf16 SWIZZLE_128B block
 
 struct TileFormat {
   int32_t n_terms;   // 1: bf16; 2: bf16 hi + lo
-  int32_t n_blk;     // input blocks per term (at most 2)
-  int32_t col0[2];   // first feature column of each input block
-  int32_t n_col[2];  // feature columns of each input block (at most 64)
+  int32_t n_blk;     // input blocks per term (at most 3)
+  int32_t col0[3];   // first feature column of each input block
+  int32_t n_col[3];  // feature columns of each input block (at most 64)
   __host__ __device__ uint32_t blk_off(int term, int b) const { return uint32_t(term * n_blk + b) * kBlkBytes; }
   __host__ __device__ uint32_t tile_bytes() const { return uint32_t(n_terms * n_blk) * kBlkBytes; }
 };
 
 // Sampling net: [hi blk0 | hi blk1 | lo blk0 | lo blk1], features 0-63 in block 0 and 64-127 in block 1.
 __host__ __device__ inline TileFormat sampling_tiles(int n_in, int n_terms) {
-  return TileFormat{n_terms, 2, {0, 64}, {n_in < 64 ? n_in : 64, n_in > 64 ? n_in - 64 : 0}};
+  return TileFormat{n_terms, 2, {0, 64, 0}, {n_in < 64 ? n_in : 64, n_in > 64 ? n_in - 64 : 0, 0}};
 }
 
-// Shading net: [P | V], P = the 63 position features and one zero column, V = the 27 view-direction features and zeros.
-// The kernel loads P at tile start and V in its place after layer 5 (LF_LOAD_IN1_AFTER).
-__host__ __device__ inline TileFormat shading_tiles() { return TileFormat{1, 2, {0, 63}, {63, 27}}; }
+// Shading net with n_p position and n_v view-direction features (3 + 6 bands each, n_p <= 128, n_v <= 64): [P | V] when
+// P fits one block, else [P0 | P1 | V] with P0 = features 0-63.  Each block holds its features and zeros after them.
+// The kernel loads the P blocks at tile start and V in place of block 0 after the LF_LOAD_IN1_AFTER layer.
+// posEnc 10-4: [P | V] = [63 features and a zero column | 27 features and zeros].
+__host__ __device__ inline TileFormat shading_tiles(int n_p, int n_v) {
+  if (n_p <= 64) return TileFormat{1, 2, {0, n_p, 0}, {n_p, n_v, 0}};
+  return TileFormat{1, 3, {0, 64, n_p}, {64, n_p - 64, n_v}};
+}
+// The number of P blocks of shading_tiles(n_p, .).
+__host__ __device__ inline int shading_p_blocks(int n_p) { return n_p > 64 ? 2 : 1; }
 
 // Round to nearest even, a in the low half.
 __device__ __forceinline__ uint32_t bf16x2(float a, float b) {
@@ -67,10 +74,21 @@ __device__ __forceinline__ void pack_tile_chunk(const TileFormat& fmt, uint8_t* 
   pack_chunk8(v, row, ch, tile + fmt.blk_off(0, b), fmt.n_terms == 2 ? tile + fmt.blk_off(1, b) : nullptr);
 }
 
-// One thread per tile row (a 128-thread CTA): packs the thread's features f (a register array, feature c = f[c]) into the
-// tile image in shared memory, then thread 0 writes the image to `dst` with one bulk shared -> global copy (TMA engine)
-// instead of strided 16-byte global stores.  Before s_tile is filled again, thread 0 waits for the copy to have read it
-// (bulk_wait_read_all) and the CTA synchronises; the CTA calls store_tiles_drain() before it exits.
+// One thread per tile row (a 128-thread CTA): the tile image in shared memory goes to `dst` with one bulk shared -> global
+// copy (TMA engine) from thread 0 instead of strided 16-byte global stores.  Before s_tile is filled again, thread 0 waits
+// for the copy to have read it (bulk_wait_read_all) and the CTA synchronises; the CTA calls store_tiles_drain() before it
+// exits.
+__device__ __forceinline__ void flush_tile(const TileFormat& fmt, uint8_t* s_tile, uint8_t* dst) {
+  fence_proxy_async_smem();
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    bulk_s2g(dst, s_tile, fmt.tile_bytes());
+    bulk_commit();
+  }
+}
+
+// Packs the thread's features f (a register array, feature c = f[c]) into the image of input blocks 0 and 1, then
+// flush_tile.
 template <int NF>
 __device__ __forceinline__ void store_tile(const TileFormat& fmt, const float (&f)[NF], uint8_t* s_tile, uint8_t* dst) {
 #pragma unroll
@@ -81,12 +99,25 @@ __device__ __forceinline__ void store_tile(const TileFormat& fmt, const float (&
         pack_tile_chunk(fmt, s_tile, b, threadIdx.x, ch, [&](int c) { return c < NF ? f[c] : 0.0f; });
     }
   }
-  fence_proxy_async_smem();
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    bulk_s2g(dst, s_tile, fmt.tile_bytes());
-    bulk_commit();
-  }
+  flush_tile(fmt, s_tile, dst);
+}
+
+// Run-time encodings: a row written one feature at a time.  zero_row clears row `row` of blocks [b0, b1) of every term of
+// the image at `tile` (block (term, b) at fmt.blk_off); put_feature then writes feature column `col` of block b, its bf16
+// hi term and, with two terms, its lo term -- the bits pack_chunk8 writes for the same value.
+__device__ __forceinline__ void zero_row(const TileFormat& fmt, uint8_t* tile, uint32_t row, int b0, int b1) {
+  for (int term = 0; term < fmt.n_terms; ++term)
+    for (int b = b0; b < b1; ++b)
+#pragma unroll
+      for (int ch = 0; ch < 8; ++ch)
+        *reinterpret_cast<uint4*>(tile + fmt.blk_off(term, b) + sw128_offset(row, uint32_t(ch * 8))) = make_uint4(0u, 0u, 0u, 0u);
+}
+
+__device__ __forceinline__ void put_feature(const TileFormat& fmt, uint8_t* tile, int b, uint32_t row, int col, float v) {
+  const __nv_bfloat16 hi = __float2bfloat16_rn(v);
+  const uint32_t off = sw128_offset(row, uint32_t(col));
+  *reinterpret_cast<__nv_bfloat16*>(tile + fmt.blk_off(0, b) + off) = hi;
+  if (fmt.n_terms == 2) *reinterpret_cast<__nv_bfloat16*>(tile + fmt.blk_off(1, b) + off) = __float2bfloat16_rn(v - __bfloat162float(hi));
 }
 
 __device__ __forceinline__ void store_tiles_drain() {

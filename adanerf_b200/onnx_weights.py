@@ -141,8 +141,8 @@ def write_onnx_initializers(path, tensors):
 def net_shapes(sd0, sd1):
     """The reference's `layers`, `layerWidth` and `skips` of the two networks, read from the tensor shapes as
     adn_set_weights reads them: depth = the number of layers.{i} / pts_linears.{i} weights, width = the rows of the first,
-    and a shading-net skip after layer i when pts_linears.{i+1} reads W + 63 columns (-1: none).
-    Returns ((D0, W0, -1), (D1, W1, skip))."""
+    and a shading-net skip after layer i when pts_linears.{i+1} reads W + P columns, P = the columns of pts_linears.0
+    (-1: none).  Returns ((D0, W0, -1), (D1, W1, skip))."""
     def depth(sd, prefix):
         d = 0
         while f"{prefix}{d}.weight" in sd:
@@ -150,7 +150,8 @@ def net_shapes(sd0, sd1):
         return d
     d0, d1 = depth(sd0, "layers."), depth(sd1, "pts_linears.")
     w0, w1 = int(sd0["layers.0.weight"].shape[0]), int(sd1["pts_linears.0.weight"].shape[0])
-    skips = [i - 1 for i in range(1, d1) if int(sd1[f"pts_linears.{i}.weight"].shape[1]) == w1 + 63]
+    p = int(sd1["pts_linears.0.weight"].shape[1])
+    skips = [i - 1 for i in range(1, d1) if int(sd1[f"pts_linears.{i}.weight"].shape[1]) == w1 + p]
     return (d0, w0, -1), (d1, w1, skips[0] if skips else -1)
 
 
@@ -162,9 +163,25 @@ def _skips_entry(depth, skip):
     return str(skip if skip >= 0 else depth)
 
 
+def _enc_entries(scene):
+    """config.ini's posEnc and posEncArgs lists of a scene dict (renderer.make_scene's band-count fields)."""
+    ndc = bool(scene.get("use_ndc"))
+    p, d = int(scene.get("n_freq_pos", 10)), int(scene.get("n_freq_dir", 4))
+    p0, d0 = scene.get("n_freq_pos0"), scene.get("n_freq_dir0")
+    p0 = (2 if ndc else p) if p0 is None or p0 == 0 else int(p0)
+    d0 = (2 if ndc else d) if d0 is None or d0 == 0 else int(d0)
+    def entry(a, b):
+        if a < 0 and b < 0:
+            return "none", "10-4"    # NoEncoding ignores posEncArgs
+        return "nerf", f"{max(a, 0)}-{max(b, 0)}"
+    (e0, a0), (e1, a1) = entry(p0, d0), entry(p, d)
+    return f"[{e0}, {e1}]", f"[{a0}, {a1}]"
+
+
 def write_export_dir(path, scene, sd0, sd1, thr, K):
     """Writes {config.ini, dataset_info.txt, model0.onnx, model1.onnx} in the reference's export format
-    (src/export.py:28-93, src/train_data.py:180-195), config.ini with the networks' layers / layerWidth / skips."""
+    (src/export.py:28-93, src/train_data.py:180-195), config.ini with the networks' layers / layerWidth / skips and the
+    scene's posEnc / posEncArgs."""
     import os
     os.makedirs(path, exist_ok=True)
     (d0, w0, _), (d1, w1, skip) = net_shapes(sd0, sd1)
@@ -179,15 +196,17 @@ def write_export_dir(path, scene, sd0, sd1, thr, K):
         f.write(f"fov = {scene['fov']}\nfocal = 0.0\ncamera_scale = 1.0\nmax_depth = {scene['max_depth']}\n")
         if ndc and scene.get("w") and scene.get("h"):   # not written by src/export.py; read by our loader when present
             f.write(f"w = {int(scene['w'])}\nh = {int(scene['h'])}\n")
+    pos_enc, pos_enc_args = _enc_entries(scene)
     with open(os.path.join(path, "config.ini"), "w") as f:
+        f.write(f"posEnc = {pos_enc}\nposEncArgs = {pos_enc_args}\n")
         if ndc:   # configs/fine_training_ndc.ini
-            f.write("posEnc = [nerf, nerf]\nposEncArgs = [2-2, 10-4]\ninFeatures = [SpherePosDir, RayMarchFromPoses]\n"
+            f.write("inFeatures = [SpherePosDir, RayMarchFromPoses]\n"
                     "outFeatures = [RawSigmoid, RGBARayMarch]\nrayMarchSampler = [none, FromClassifiedDepthAdaptiveNoDepthRange]\n"
                     "rayMarchNormalization = [InverseSqrtDistCentered, None]\nuseNDC = True\n"
                     f"numRaymarchSamples = [{K}, {K}]\ndepthTransform = linear\nzNear = [0.001, 0.001]\nzFar = [1.0, 1.0]\n"
                     f"adaptiveSamplingThreshold = {thr}\nmultiDepthFeatures = [128, 128]\naccumulationMult = alpha\n")
         else:
-            f.write("posEnc = [nerf, nerf]\nposEncArgs = [10-4, 10-4]\ninFeatures = [SpherePosDir, RayMarchFromPoses]\n"
+            f.write("inFeatures = [SpherePosDir, RayMarchFromPoses]\n"
                     "outFeatures = [RawSigmoid, RGBARayMarch]\nrayMarchSampler = [none, FromClassifiedDepthAdaptive]\n"
                     "rayMarchNormalization = [InverseSqrtDistCentered, InverseSqrtDistCentered]\n"
                     f"numRaymarchSamples = [{K}, {K}]\ndepthTransform = log\nzNear = [0.001, 0.001]\nzFar = [1.0, 1.0]\n"

@@ -10,11 +10,27 @@ from . import _lib
 from ._lib import AdnError, AuxOutputs, Scene, Stats, TensorDesc
 
 
+def enc_columns(n_bands):
+    """Columns of one encoded 3-vector with n_bands frequency bands (3 + 6 n_bands); a negative count is posEnc none,
+    the 3-column identity."""
+    return 3 + 6 * max(0, int(n_bands))
+
+
+def scene_columns(sc):
+    """(sampling-net inputs, shading-net position columns, shading-net view columns) of a Scene, as adn_create reads its
+    band counts: a negative one is posEnc none; the sampling net's 0 is "the shading net's"."""
+    p0 = sc.n_freq_pos0 if sc.n_freq_pos0 else sc.n_freq_pos
+    d0 = sc.n_freq_dir0 if sc.n_freq_dir0 else sc.n_freq_dir
+    return enc_columns(p0) + enc_columns(d0), enc_columns(sc.n_freq_pos), enc_columns(sc.n_freq_dir)
+
+
 def make_scene(view_cell_center, view_cell_size, depth_range, max_depth, fov, z_near=0.001, z_far=1.0,
                n_freq_pos=10, n_freq_dir=4, use_ndc=False, w=0, h=0, focal=0.0, n_freq_pos0=None, n_freq_dir0=None, **_):
     """use_ndc: the NDC / LLFF variant (configs/fine_training_ndc.ini); w, h, focal = the dataset's image size and focal
     length that ndc_rays uses (src/features.py:350-351,430); the sampling net then takes the "2-2" encoding (30 features)
-    unless n_freq_pos0 / n_freq_dir0 say otherwise."""
+    unless n_freq_pos0 / n_freq_dir0 say otherwise.
+    n_freq_pos / n_freq_dir: the shading net's posEncArgs band counts (-1: posEnc none); n_freq_pos0 / n_freq_dir0 the
+    sampling net's (0: the same as the shading net's; -1: posEnc none or zero bands)."""
     s = Scene()
     s.view_cell_center[:] = [float(x) for x in view_cell_center]
     s.view_cell_size[:] = [float(x) for x in view_cell_size]
@@ -48,13 +64,13 @@ class Renderer:
         self.handle = C.c_void_p()
         self._registered = {}    # address -> numpy array page-locked through register_host_buffer (kept alive here)
         self.n_feat0 = 90        # sampling-net input features (30 with the "2-2" encoding of the NDC configs)
+        self.n_feat1 = 90        # shading-net input features: position, then view columns
         if _handle is not None:
             self.handle = _handle
         else:
             sc = scene if isinstance(scene, Scene) else make_scene(**scene)
             self._check(self.lib.adn_create(C.byref(self.handle), C.byref(sc), self.device), create=True)
-            if sc.n_freq_pos0 or sc.n_freq_dir0:
-                self.n_feat0 = 6 + 6 * (sc.n_freq_pos0 + sc.n_freq_dir0)
+            self._set_columns(sc)
         if sampling_net is not None:
             self.set_weights(0, sampling_net)
         if shading_net is not None:
@@ -70,9 +86,13 @@ class Renderer:
             raise AdnError(st, f"loading export dir {path}")
         r = cls(None, device=device, _handle=h)
         sc, nt = Scene(), (C.c_int * 2)()
-        if lib.adn_probe_export_dir(str(path).encode(), C.byref(sc), None, None, nt) == 0 and (sc.n_freq_pos0 or sc.n_freq_dir0):
-            r.n_feat0 = 6 + 6 * (sc.n_freq_pos0 + sc.n_freq_dir0)
+        if lib.adn_probe_export_dir(str(path).encode(), C.byref(sc), None, None, nt) == 0:
+            r._set_columns(sc)
         return r, float(thr.value), int(k.value)
+
+    def _set_columns(self, sc):
+        n0, n_p, n_v = scene_columns(sc)
+        self.n_feat0, self.n_feat1 = n0, n_p + n_v
 
     def _check(self, st, create=False):
         if st != 0:
@@ -317,7 +337,7 @@ class Renderer:
         ro, rd, zz = self._f32(ray_o), self._f32(ray_d), self._f32(z)
         ri = ray_idx.to(device=self._dev(), dtype=torch.int32).contiguous()
         m = zz.shape[0]
-        x1 = torch.empty((m, 90), dtype=torch.float32, device=self._dev())
+        x1 = torch.empty((m, self.n_feat1), dtype=torch.float32, device=self._dev())
         self._check(self.lib.adn_stage3_encode(self.handle, ro.data_ptr(), rd.data_ptr(), ri.data_ptr(), zz.data_ptr(), m,
                                                x1.data_ptr(), self._stream()))
         return x1

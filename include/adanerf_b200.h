@@ -39,7 +39,7 @@ enum {
 
 /* Scene constants.  Source: the export's dataset_info.txt written by src/export.py:47-54
  * (view_cell_center, view_cell_size, depth_range = WARPED range, fov, max_depth) and the feature
- * set constructors src/features.py:286-287 (zNear/zFar), :338-339 (posEncArgs "10-4"). */
+ * set constructors src/features.py:286-287 (zNear/zFar), :326-339 (posEnc / posEncArgs). */
 typedef struct adn_scene {
   float view_cell_center[3];
   float view_cell_size[3];
@@ -47,10 +47,14 @@ typedef struct adn_scene {
   float max_depth;
   float fov;            /* radians; focal = 0.5*W/tan(fov/2)  (src/datasets.py:181-182) */
   float z_near, z_far;  /* 0.001, 1.0 */
-  int32_t n_freq_pos;   /* 10: shading-net encoding, posEncArgs[1] = "10-4" */
-  int32_t n_freq_dir;   /* 4 */
-  /* Sampling-net encoding, posEncArgs[0]: 0/0 = same as above ("10-4", 90 features) or 2/2 ("2-2", 30 features,
-   * configs/fine_training_ndc.ini:8). */
+  /* Shading-net encoding, posEnc[1] / posEncArgs[1] (default "10-4"): position and direction band counts P <= 20, D <= 10;
+   * the net reads 3 + 6 P position and 3 + 6 D direction columns.  Negative: posEnc none, the 3-column identity (the
+   * reference's -1, src/features.py:326-328), the same as 0 bands. */
+  int32_t n_freq_pos;
+  int32_t n_freq_dir;
+  /* Sampling-net encoding, posEnc[0] / posEncArgs[0], 6 + 6 (P0 + D0) input columns, P0 + D0 <= 20: 0 = the shading
+   * net's field above (e.g. "10-4", 90 features), negative = 0 bands or posEnc none, positive = that count (e.g. 2/2,
+   * "2-2", 30 features, configs/fine_training_ndc.ini:8).  Outside these limits adn_create returns ADN_ERR_INVALID. */
   int32_t n_freq_pos0, n_freq_dir0;
   /* NDC / LLFF variant (configs/fine_training_ndc.ini: useNDC, FromClassifiedDepthAdaptiveNoDepthRange,
    * rayMarchNormalization[1] = None): rays go through ndc_rays(H, W, focal, near = 1)
@@ -94,10 +98,13 @@ const char* adn_version(void);
  * The network's shape (the reference's `layers`, `layerWidth`, `skips`) is read from the tensor shapes:
  *   sampling net: layers.0 .. layers.{D-1}, D = 1-12, at most 128 inputs, hidden width W = 128 or 256 in every hidden
  *     layer, 128 or 256 outputs (a render needs 128); no skips.
- *   shading net: posEnc 10-4 (pts_linears.0 reads 63 columns, views_linears.0 reads W + 27), D = 1-10 pts_linears,
- *     W = 128 or 256, view branch W/2; no skip, or one skip after layer i in [0, D-2], which shows as pts_linears.{i+1}
- *     reading W + 63 columns (the reference's skips = auto is a skip at 4 for D >= 6 and none for D <= 4).
- * Any other shape fails with ADN_ERR_INVALID and adn_last_error names the offending tensor. */
+ *   shading net: the scene's encoding, P = 3 + 6 n_freq_pos and V = 3 + 6 n_freq_dir columns (63 and 27 for posEnc
+ *     10-4): pts_linears.0 reads P columns, views_linears.0 reads W + V; D = 1-10 pts_linears, W = 128 or 256, view
+ *     branch W/2; no skip, or one skip after layer i in [0, D-2], which shows as pts_linears.{i+1} reading W + P columns
+ *     (the reference's skips = auto is a skip at 4 for D >= 6 and none for D <= 4).
+ *   The sampling net must read the 6 + 6 (n_freq_pos0 + n_freq_dir0) columns of the scene's encoding to render.
+ * Any other shape fails with ADN_ERR_INVALID and adn_last_error names the offending tensor and, for the shading net, the
+ * column count the scene's encoding expects. */
 adn_status adn_set_weights(adn_ctx* ctx, int net_id, const adn_tensor_desc* tensors, int n_tensors);
 
 /* The shape adn_set_weights inferred: depth D, width W (of a one-layer sampling net: its output width) and the skip layer
@@ -117,7 +124,7 @@ adn_status adn_probe_export_dir(const char* dir, adn_scene* scene_out, float* th
 
 /* name: "chunk_rays" (rays per internal batch, 0 = auto), "profile" (0/1 per-stage event timing),
  * "mlp0_terms" (3 = bf16x3 split precision [default], 1 = plain bf16; parity experiments only),
- * "fuse_encoder" (1 = positional encoding of the samples inside the shading kernel: no [M,90]-sized tile buffer;
+ * "fuse_encoder" (1 = positional encoding of the samples inside the shading kernel: no [M, P + V]-sized tile buffer;
  *   0 = separate kernel [default]),
  * "sample_budget" (B > 0 = every adaptive render -- rays, aux, camera, rgba8, surface, *_host -- takes its `thr` as a floor
  *   and renders with the smallest threshold t* >= thr whose total sample count M over the whole call is <= B, chosen on
@@ -202,7 +209,7 @@ adn_status adn_unregister_host_buffer(adn_ctx* ctx, const void* p);
 adn_status adn_net_dims(adn_ctx* ctx, int net_id, int* n_in, int* n_out);
 
 /* ---- stage-level entry points (parity tests drive each kernel in isolation) ------------- */
-/* stage 0: SpherePosDir.batch (src/features.py:845-899). d_x0 [N,90] fp32 (dir block first), d_ray_o/d [N,3]. */
+/* stage 0: SpherePosDir.batch (src/features.py:845-899). d_x0 [N, 6 + 6 (P0 + D0)] fp32 (dir block first), d_ray_o/d [N,3]. */
 adn_status adn_stage0_features(adn_ctx* ctx, const float* pose, const float* rot, const float* d_dirs, int64_t n_rays,
                                float* d_x0, float* d_ray_o, float* d_ray_d, void* stream);
 /* stage 0a: generate_ray_directions (src/util/raygeneration.py:10-26). d_dirs [rows*W,3]. */
@@ -222,10 +229,10 @@ adn_status adn_stage2_sample(adn_ctx* ctx, const float* d_raw0, int64_t n_rays, 
  * rank-2..K values. */
 adn_status adn_budget_threshold(adn_ctx* ctx, const float* d_raw0, int64_t n_rays, float thr_min, int K, int64_t max_samples,
                                 float* d_thr, void* stream);
-/* stage 3: RayMarchFromPoses.batch encode (src/features.py:458-479). d_x1 [M,90] fp32 (pos block first). */
+/* stage 3: RayMarchFromPoses.batch encode (src/features.py:458-479). d_x1 [M, P + V] fp32 (pos block first; adn_net_dims). */
 adn_status adn_stage3_encode(adn_ctx* ctx, const float* d_ray_o, const float* d_ray_d, const int32_t* d_ray,
                              const float* d_z, int64_t n_samples, float* d_x1, void* stream);
-/* stage 4: NeRF.forward (src/models.py:254-277). d_x1 [M,90] fp32 -> d_raw1 [M,4] fp32 = [rgb, alpha]. */
+/* stage 4: NeRF.forward (src/models.py:254-277). d_x1 [M, P + V] fp32 -> d_raw1 [M,4] fp32 = [rgb, alpha]. */
 adn_status adn_mlp1_forward(adn_ctx* ctx, const float* d_x1, int64_t n_samples, float* d_raw1, void* stream);
 /* stage 5: adaptive_raw2outputs (src/nerf_raymarch_common.py:91-144, accumulation_mult "alpha").
  * d_weights / d_depth_map may be NULL; d_weights is [N,K] zero padded like the reference's. */
