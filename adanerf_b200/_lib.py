@@ -83,6 +83,7 @@ def load_library():
     lib.adn_render_rays_aux.argtypes = [vp, fp, fp, f32p, i64, C.c_float, C.c_int, f32p, i32p, f32p, C.POINTER(AuxOutputs), vp]
     lib.adn_render_camera.argtypes = [vp, fp, fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, f32p, i32p, vp]
     lib.adn_render_camera_rgba8.argtypes = [vp, fp, fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, vp, vp]
+    lib.adn_render_camera_surface.argtypes = [vp, fp, fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, C.c_ulonglong, vp]
     lib.adn_render_rays_host.argtypes = [vp, fp, fp, f32p, i64, C.c_float, C.c_int, f32p, i32p]
     lib.adn_render_camera_host.argtypes = [vp, fp, fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, f32p, i32p]
     lib.adn_stage0_features.argtypes = [vp, fp, fp, f32p, i64, f32p, f32p, f32p, vp]

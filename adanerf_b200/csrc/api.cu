@@ -89,6 +89,9 @@ struct adn_ctx {
   struct Reg { const void* p = nullptr; size_t bytes = 0; };
   std::vector<Reg> regs;
   cudaStream_t own_stream = nullptr;
+  // issue order across streams (CallOrder): recorded after the last enqueue of every call, waited on before the first
+  // enqueue of the next one
+  cudaEvent_t order = nullptr;
   cudaEvent_t ev[8] = {};
   adn_stats stats{};
   std::string last_error;
@@ -111,6 +114,42 @@ adn_status cuda_fail(adn_ctx* ctx, cudaError_t e, const char* where) {
     cudaError_t e__ = (call);                                 \
     if (e__ != cudaSuccess) return cuda_fail(ctx, e__, #call); \
   } while (0)
+
+// Makes the calls on one context execute in the order they were made, whatever stream each names.  They share the
+// context's scratch (tiles, raw0 / raw1, the stage-2 look-back state and tickets, the budget state) and often each other's
+// outputs, so two calls in flight on different streams would overwrite what the other still reads.  begin(): the call's
+// stream waits on ctx->order, recorded by the previous call after its last enqueue; the guard records it again when the call
+// returns, on an error return after a partial enqueue too.  The wait is made even when the stream is the previous call's: it
+// costs one driver call, and a stream handle can be destroyed and handed out again.  One guard per entry point, after
+// cudaSetDevice (a null stream is the legacy stream of the current device).
+//
+// A stream that is capturing a CUDA graph is refused before anything is enqueued: stage 2 takes its launch epoch and ticket
+// base from host state (Stage2Sync), so a replayed launch would run with stale ones.
+class CallOrder {
+ public:
+  CallOrder(adn_ctx* ctx, cudaStream_t st) : ctx_(ctx), st_(st) {}
+  CallOrder(const CallOrder&) = delete;
+  CallOrder& operator=(const CallOrder&) = delete;
+  ~CallOrder() {
+    if (armed_) cudaEventRecord(ctx_->order, st_);
+  }
+  adn_status begin(const char* who) {
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    const cudaError_t e = cudaStreamIsCapturing(st_, &cs);
+    if (e != cudaSuccess) cudaGetLastError();   // e.g. the legacy stream while another stream captures: treat as capturing
+    if (e != cudaSuccess || cs != cudaStreamCaptureStatusNone)
+      return fail(ctx_, ADN_ERR_INVALID, std::string(who) + ": the stream is capturing a CUDA graph; calls cannot be captured "
+                                                            "(stage 2's launch epoch and tickets are host state)");
+    ADN_CUDA(ctx_, cudaStreamWaitEvent(st_, ctx_->order, 0));
+    armed_ = true;
+    return ADN_OK;
+  }
+
+ private:
+  adn_ctx* ctx_;
+  cudaStream_t st_;
+  bool armed_ = false;
+};
 
 // Grows b to at least `bytes` (device buffers with some slack); the old contents are not kept.
 adn_status ensure(adn_ctx* ctx, Buf& b, size_t bytes) {
@@ -687,6 +726,15 @@ adn_status render(adn_ctx* ctx, const RenderCall& call) {
   return ADN_OK;
 }
 
+// render() as one call of a device entry point, ordered after the context's earlier calls (CallOrder).
+adn_status render_ordered(adn_ctx* ctx, const RenderCall& call, const char* who) {
+  if (!ctx) return ADN_ERR_INVALID;
+  ADN_CUDA(ctx, cudaSetDevice(ctx->device));
+  CallOrder order(ctx, call.st);
+  const adn_status s = order.begin(who);
+  return s != ADN_OK ? s : render(ctx, call);
+}
+
 adn_status check_device_error(adn_ctx* ctx) {
   int err = 0;
   cudaError_t e = cudaDeviceSynchronize();
@@ -712,8 +760,10 @@ adn_status copy_out(adn_ctx* ctx, void* h, const void* d, size_t bytes, Buf& sta
 adn_status render_host(adn_ctx* ctx, RenderCall c, const float* h_dirs, float* h_rgb, int32_t* h_nsamples) {
   const size_t n = size_t(c.n_rays);
   ADN_CUDA(ctx, cudaSetDevice(ctx->device));
-  adn_status s;
   c.st = ctx->own_stream;
+  CallOrder order(ctx, c.st);
+  adn_status s = order.begin("render_host");
+  if (s != ADN_OK) return s;
   if (h_dirs) {
     const bool staged = !pin_in_place(ctx, h_dirs, n * 12);
     if ((s = ensure(ctx, ctx->dirs, n * 12)) != ADN_OK || (staged && (s = ensure(ctx, ctx->h_in, n * 12)) != ADN_OK)) return s;
@@ -802,7 +852,8 @@ adn_status adn_create(adn_ctx** out, const adn_scene* scene, int device) {
             cudaMemset(ctx->total.p, 0, sizeof(long long)) == cudaSuccess &&
             cudaHostAlloc(&ctx->watchdog.p, sizeof(int), cudaHostAllocMapped) == cudaSuccess &&
             cudaHostGetDevicePointer(&ctx->d_err, ctx->watchdog.p, 0) == cudaSuccess && (*ctx->watchdog.as<int>() = 0, true) &&
-            cudaStreamCreateWithFlags(&ctx->own_stream, cudaStreamNonBlocking) == cudaSuccess;
+            cudaStreamCreateWithFlags(&ctx->own_stream, cudaStreamNonBlocking) == cudaSuccess &&
+            cudaEventCreateWithFlags(&ctx->order, cudaEventDisableTiming) == cudaSuccess;
   for (int i = 0; ok && i < 8; ++i) ok = cudaEventCreate(&ctx->ev[i]) == cudaSuccess;
   if (!ok) {
     adn_destroy(ctx);
@@ -820,6 +871,7 @@ void adn_destroy(adn_ctx* ctx) {
     if (r.p) cudaHostUnregister(const_cast<void*>(r.p));
   for (int i = 0; i < 8; ++i)
     if (ctx->ev[i]) cudaEventDestroy(ctx->ev[i]);
+  if (ctx->order) cudaEventDestroy(ctx->order);
   if (ctx->own_stream) cudaStreamDestroy(ctx->own_stream);
   delete ctx;   // frees every Buf on this device
 }
@@ -927,7 +979,7 @@ adn_status adn_render_rays_aux(adn_ctx* ctx, const float* pose, const float* rot
   c.d_nsamples = d_nsamples;
   c.d_oracle_w = d_oracle_weights;
   if (aux) c.aux = *aux;
-  return render(ctx, c);
+  return render_ordered(ctx, c, "render_rays");
 }
 
 adn_status adn_render_camera(adn_ctx* ctx, const float* pose, const float* rot, int W, int H, int row0, int rows, float thr,
@@ -937,7 +989,7 @@ adn_status adn_render_camera(adn_ctx* ctx, const float* pose, const float* rot, 
   if (!c.cam) return fail(ctx, ADN_ERR_INVALID, "render_camera: bad image window");
   c.d_rgb = d_rgb;
   c.d_nsamples = d_nsamples;
-  return render(ctx, c);
+  return render_ordered(ctx, c, "render_camera");
 }
 
 adn_status adn_render_camera_rgba8(adn_ctx* ctx, const float* pose, const float* rot, int W, int H, int row0, int rows,
@@ -946,7 +998,7 @@ adn_status adn_render_camera_rgba8(adn_ctx* ctx, const float* pose, const float*
   c.cam = camera_rays(ctx, W, H, row0, rows);
   if (!c.cam) return fail(ctx, ADN_ERR_INVALID, "render_camera: bad image window");
   c.d_rgba8 = d_rgba8;
-  return render(ctx, c);
+  return render_ordered(ctx, c, "render_camera_rgba8");
 }
 
 adn_status adn_render_camera_surface(adn_ctx* ctx, const float* pose, const float* rot, int W, int H, int row0, int rows,
@@ -955,8 +1007,9 @@ adn_status adn_render_camera_surface(adn_ctx* ctx, const float* pose, const floa
   c.cam = camera_rays(ctx, W, H, row0, rows);
   if (!c.cam || !surface) return fail(ctx, ADN_ERR_INVALID, "render_camera_surface: bad image window / surface");
   ADN_CUDA(ctx, cudaSetDevice(ctx->device));
-  adn_status s = ensure(ctx, ctx->rgba, size_t(rows) * W * 4);
-  if (s != ADN_OK) return s;
+  CallOrder order(ctx, c.st);   // the render and the surface write: one call
+  adn_status s = order.begin("render_camera_surface");
+  if (s != ADN_OK || (s = ensure(ctx, ctx->rgba, size_t(rows) * W * 4)) != ADN_OK) return s;
   c.d_rgba8 = ctx->rgba.as<uint8_t>();
   if ((s = render(ctx, c)) != ADN_OK) return s;
   ADN_CUDA(ctx, launch_rgba_to_surface(c.d_rgba8, W, row0, rows, surface, c.st));
@@ -1026,6 +1079,8 @@ adn_status adn_generate_ray_directions(adn_ctx* ctx, int W, int H, int row0, int
   const std::optional<CameraRays> cam = camera_rays(ctx, W, H, row0, rows);
   if (!cam || !d_dirs) return fail(ctx, ADN_ERR_INVALID, "generate_ray_directions: bad arguments");
   ADN_CUDA(ctx, cudaSetDevice(ctx->device));
+  CallOrder order(ctx, static_cast<cudaStream_t>(stream));
+  if (adn_status s = order.begin("generate_ray_directions"); s != ADN_OK) return s;
   ADN_CUDA(ctx, launch_gen_dirs(*cam, int64_t(rows) * W, d_dirs, static_cast<cudaStream_t>(stream)));
   ctx->stats.kernel_launches++;
   return ADN_OK;
@@ -1036,6 +1091,8 @@ adn_status adn_stage0_features(adn_ctx* ctx, const float* pose, const float* rot
   if (!ctx || !pose || !rot || !d_dirs || n_rays < 0 || (d_ray_o == nullptr) != (d_ray_d == nullptr))
     return fail(ctx, ADN_ERR_INVALID, "stage0: bad arguments");
   ADN_CUDA(ctx, cudaSetDevice(ctx->device));
+  CallOrder order(ctx, static_cast<cudaStream_t>(stream));
+  if (adn_status s = order.begin("stage0"); s != ADN_OK) return s;
   ADN_CUDA(ctx, launch_stage0(ctx->sc, make_pose(pose, rot), d_dirs, nullptr, n_rays, d_x0, d_ray_o, d_ray_d, nullptr, 0,
                               static_cast<cudaStream_t>(stream)));
   ctx->stats.kernel_launches++;
@@ -1048,9 +1105,10 @@ adn_status adn_mlp0_forward(adn_ctx* ctx, const float* d_x0, int64_t n_rays, flo
   if (n_rays == 0) return ADN_OK;
   ADN_CUDA(ctx, cudaSetDevice(ctx->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CallOrder order(ctx, st);
+  adn_status s = order.begin("mlp0_forward");
   Net& n = ctx->net[0];
-  adn_status s = ensure(ctx, ctx->tiles0, size_t(pad128(n_rays) / 128) * n.prog.in.tile_bytes());
-  if (s != ADN_OK) return s;
+  if (s != ADN_OK || (s = ensure(ctx, ctx->tiles0, size_t(pad128(n_rays) / 128) * n.prog.in.tile_bytes())) != ADN_OK) return s;
   ADN_CUDA(ctx, launch_pack_rows(d_x0, n_rays, nullptr, n.n_in, n.prog.in, static_cast<uint8_t*>(ctx->tiles0.p), ctx->num_sms, st));
   ctx->stats.kernel_launches++;
   return run_mlp(ctx, 0, static_cast<uint8_t*>(ctx->tiles0.p), d_raw0, nullptr, n_rays, st);
@@ -1063,8 +1121,9 @@ adn_status adn_stage2_sample(adn_ctx* ctx, const float* d_raw0, int64_t n_rays, 
       (n_rays > 0 && (!d_raw0 || !d_count || !d_offset || !d_ray || !d_z || !d_zp)))
     return fail(ctx, ADN_ERR_INVALID, "stage2: bad arguments (adaptive path needs thr > 0)");
   ADN_CUDA(ctx, cudaSetDevice(ctx->device));
-  adn_status s = ensure(ctx, ctx->s2scratch, stage2_scratch_bytes(n_rays));
-  if (s != ADN_OK) return s;
+  CallOrder order(ctx, static_cast<cudaStream_t>(stream));
+  adn_status s = order.begin("stage2");
+  if (s != ADN_OK || (s = ensure(ctx, ctx->s2scratch, stage2_scratch_bytes(n_rays))) != ADN_OK) return s;
   ADN_CUDA(ctx, launch_stage2(d_raw0, n_rays, thr, K, ctx->zlut.as<float>(), d_count, d_offset, d_cell, d_ray, d_z, d_zp,
                               reinterpret_cast<long long*>(d_total), ctx->s2scratch.p, &ctx->s2sync, static_cast<cudaStream_t>(stream)));
   ctx->stats.kernel_launches++;
@@ -1079,8 +1138,11 @@ adn_status adn_budget_threshold(adn_ctx* ctx, const float* d_raw0, int64_t n_ray
     return fail(ctx, ADN_ERR_INVALID, "budget_threshold: at most 2^32 - 1 candidate samples (N * (K - 1))");
   if (reinterpret_cast<uintptr_t>(d_raw0) & 15u) return fail(ctx, ADN_ERR_INVALID, "budget_threshold: d_raw0 must be 16-byte aligned");
   ADN_CUDA(ctx, cudaSetDevice(ctx->device));
-  adn_status s = ensure(ctx, ctx->budget_keys, size_t(std::max<int64_t>(1, n_rays * (K - 1))) * 4);
-  if (s != ADN_OK || (s = ensure(ctx, ctx->budget_work, budget_work_bytes())) != ADN_OK) return s;
+  CallOrder order(ctx, static_cast<cudaStream_t>(stream));
+  adn_status s = order.begin("budget_threshold");
+  if (s != ADN_OK || (s = ensure(ctx, ctx->budget_keys, size_t(std::max<int64_t>(1, n_rays * (K - 1))) * 4)) != ADN_OK ||
+      (s = ensure(ctx, ctx->budget_work, budget_work_bytes())) != ADN_OK)
+    return s;
   int launches = 0;
   ADN_CUDA(ctx, launch_budget_threshold(d_raw0, n_rays, thr_min, K, max_samples, static_cast<uint32_t*>(ctx->budget_keys.p),
                                         ctx->budget_work.p, d_thr, ctx->num_sms, static_cast<cudaStream_t>(stream), &launches));
@@ -1092,6 +1154,8 @@ adn_status adn_stage3_encode(adn_ctx* ctx, const float* d_ray_o, const float* d_
                              int64_t n_samples, float* d_x1, void* stream) {
   if (!ctx || !d_ray_o || !d_ray_d || !d_ray || !d_z || !d_x1 || n_samples < 0) return fail(ctx, ADN_ERR_INVALID, "stage3: bad arguments");
   ADN_CUDA(ctx, cudaSetDevice(ctx->device));
+  CallOrder order(ctx, static_cast<cudaStream_t>(stream));
+  if (adn_status s = order.begin("stage3"); s != ADN_OK) return s;
   ADN_CUDA(ctx, launch_stage3(ctx->sc, d_ray_o, d_ray_d, d_ray, d_z, nullptr, 1, n_samples, nullptr, d_x1, nullptr, ctx->num_sms,
                               static_cast<cudaStream_t>(stream)));
   ctx->stats.kernel_launches++;
@@ -1104,9 +1168,10 @@ adn_status adn_mlp1_forward(adn_ctx* ctx, const float* d_x1, int64_t n_samples, 
   if (n_samples == 0) return ADN_OK;
   ADN_CUDA(ctx, cudaSetDevice(ctx->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CallOrder order(ctx, st);
+  adn_status s = order.begin("mlp1_forward");
   Net& n = ctx->net[1];
-  adn_status s = ensure(ctx, ctx->tiles1, size_t(pad128(n_samples) / 128) * n.prog.in.tile_bytes());
-  if (s != ADN_OK) return s;
+  if (s != ADN_OK || (s = ensure(ctx, ctx->tiles1, size_t(pad128(n_samples) / 128) * n.prog.in.tile_bytes())) != ADN_OK) return s;
   ADN_CUDA(ctx, launch_pack_rows(d_x1, n_samples, nullptr, n.n_in, n.prog.in, static_cast<uint8_t*>(ctx->tiles1.p), ctx->num_sms, st));
   ctx->stats.kernel_launches++;
   return run_mlp(ctx, 1, static_cast<uint8_t*>(ctx->tiles1.p), d_raw1, nullptr, n_samples, st);
@@ -1122,8 +1187,9 @@ adn_status adn_stage5_composite_aux(adn_ctx* ctx, const float* d_raw1, const flo
   if (n_rays > 0 && (!d_raw1 || !d_zp || (!dense && (!d_offset || !d_count || (reads_z && !d_z)))))
     return fail(ctx, ADN_ERR_INVALID, "stage5: bad arguments");
   ADN_CUDA(ctx, cudaSetDevice(ctx->device));
-  adn_status s;
-  if (dense && (s = ensure_dense_lut(ctx, K)) != ADN_OK) return s;
+  CallOrder order(ctx, static_cast<cudaStream_t>(stream));
+  adn_status s = order.begin("stage5");
+  if (s != ADN_OK || (dense && (s = ensure_dense_lut(ctx, K)) != ADN_OK)) return s;
   ADN_CUDA(ctx, launch_stage5(d_raw1, d_zp, dense ? nullptr : d_z, ctx->zlut_dense.as<float>(), dense ? nullptr : d_offset,
                               d_count, n_rays, K, dense, d_rgb, d_rgba8, stage5_aux(ctx, a), static_cast<cudaStream_t>(stream)));
   ctx->stats.kernel_launches++;
@@ -1145,10 +1211,11 @@ adn_status adn_image_metrics(adn_ctx* ctx, const float* d_image, const float* d_
   if (!ctx || !d_image || !d_reference || n_values < 1 || (!mse_out && !psnr_out))
     return fail(ctx, ADN_ERR_INVALID, "image_metrics: bad arguments");
   ADN_CUDA(ctx, cudaSetDevice(ctx->device));
-  adn_status s = ensure(ctx, ctx->metric, sizeof(double) * (kMetricBlocks + 1));
-  if (s != ADN_OK) return s;
-  double* part = static_cast<double*>(ctx->metric.p);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CallOrder order(ctx, st);
+  adn_status s = order.begin("image_metrics");
+  if (s != ADN_OK || (s = ensure(ctx, ctx->metric, sizeof(double) * (kMetricBlocks + 1))) != ADN_OK) return s;
+  double* part = static_cast<double*>(ctx->metric.p);
   ADN_CUDA(ctx, launch_image_sqdiff(d_image, d_reference, n_values, clamp01, part, part + kMetricBlocks, st));
   ctx->stats.kernel_launches += 2;
   double sum = 0.0;

@@ -13,6 +13,13 @@
  * void*, NULL = legacy default stream); no host synchronisation inside unless stated; one context
  * per device; a context is not thread safe.  There is NO CPU fallback: every call fails with
  * ADN_ERR_CUDA / ADN_ERR_NO_DEVICE when no sm_90 device is usable.
+ * Order across streams: the calls on one context execute in the order they were issued, whatever
+ * stream each names (the *_host entries run on a stream of the context's own): every call that
+ * enqueues work waits for the previous call's work and records an event after its own, since all
+ * calls share the context's scratch.  The caller still orders its own kernels against a call's
+ * outputs (on the call's stream, or with an event recorded there).  A call on a stream that is
+ * capturing a CUDA graph fails with ADN_ERR_INVALID before it enqueues anything: stage 2's launch
+ * epoch and ticket base are host state that a replayed graph would not update.
  */
 #ifndef ADANERF_B200_H
 #define ADANERF_B200_H
