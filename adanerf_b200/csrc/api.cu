@@ -67,7 +67,7 @@ struct adn_ctx {
   Net net[2];
   int mlp0_terms = 3;
   int n_feat0 = 90;               // sampling-net input features: 6 + 6 (n_freq_pos0 + n_freq_dir0)
-  bool fuse_encoder = false;      // stage 3 inside the shading kernel: saves the [M, n_in]-sized tile buffer
+  bool fuse_encoder = true;       // stage 3 inside the shading kernel (non-NDC scenes): no [M, n_in]-sized tile buffer
   int64_t chunk_rays = 0;
   bool profile = false;
   int64_t sample_budget = 0;      // B of adn_set_option "sample_budget" (0 = off)
@@ -330,9 +330,8 @@ adn_status build_net0(adn_ctx* ctx) {
 // the input blocks P (one, or two when kP > 64; then V) in shared memory and the W/64 hidden blocks in the consumers'
 // registers:
 //   pts layer 0 reads P; the skip consumer reads P, then the hidden blocks; the other pts layers read the hidden blocks; the
-//   last pts layer also forms alpha (LF_ALPHA_DOT); V replaces P after the skip consumer, or after layer 0 without a skip;
-//   feature_linear: W -> W without activation; views_linears.0 on cat[feature, V] -> W/2 reads the hidden blocks, then V,
-//   with rgb_linear in its epilogue.
+//   last pts layer also forms alpha (LF_ALPHA_DOT); feature_linear: W -> W without activation; views_linears.0 on
+//   cat[feature, V] -> W/2 reads the hidden blocks, then V, with rgb_linear in its epilogue.
 // At W = 128 the view layer's 64 outputs are padded to the kernel's 128 rows with zero weights, zero biases and zero
 // rgb_linear columns: ReLU(0) = 0 adds nothing to the rgb dot products, so the result is exact.
 adn_status build_net1(adn_ctx* ctx) {
@@ -388,7 +387,6 @@ adn_status build_net1(adn_ctx* ctx) {
   net.n_in = kP + kV;
   net.n_out = 4;
   const int nh = W / 64;                       // hidden activation blocks 1 .. nh
-  const int load_v = skip >= 0 ? skip + 1 : 0;   // the layer after which V replaces P
   MlpProgram P{};
   P.n_layers = D + 2;
   std::vector<uint8_t> wblob;
@@ -415,7 +413,7 @@ adn_status build_net1(adn_ctx* ctx) {
       } else {
         read_hidden(0);
       }
-      L.flags = LF_RELU | LF_OUT_ACT | (l == D - 1 ? LF_ALPHA_DOT : 0) | (l == load_v ? LF_LOAD_IN1_AFTER : 0);
+      L.flags = LF_RELU | LF_OUT_ACT | (l == D - 1 ? LF_ALPHA_DOT : 0);
       Wt = pw[l];
       B = pb[l];
     } else if (l == D) {  // feature_linear: no activation (models.py:265)
@@ -447,7 +445,7 @@ adn_status build_net1(adn_ctx* ctx) {
   P.rgb_w_off = uint32_t(push_floats(fblob, rgb_w.data(), rgb_w.size()));
   P.rgb_b_off = uint32_t(push_floats(fblob, rb->data.data(), 3));
   P.in = shading_tiles(kP, kV);
-  P.in_nblk0 = shading_p_blocks(kP);   // P; V after layer load_v
+  P.in_nblk0 = shading_p_blocks(kP);   // P; V is the block after it
   P.out_cols = 4;
   net.prog = P;
   adn_status s = upload(ctx, net, wblob, fblob);
@@ -608,7 +606,8 @@ adn_status run_stages_2_5(adn_ctx* ctx, const RenderCall& c, int64_t w, const fl
     if ((s = ensure(ctx, ctx->zpbuf, size_t(cap) * 4)) != ADN_OK) return s;
     if ((s = ensure(ctx, ctx->s2scratch, stage2_scratch_bytes(n))) != ADN_OK) return s;
   }
-  // stage 3 runs inside the shading kernel (encoder warp) unless the variant needs the stand-alone kernel
+  // stage 3 runs inside the shading kernel (its producer warps encode the next tile) unless option fuse_encoder is 0 or
+  // the scene is NDC: then stage3_kernel writes the packed tiles that the kernel's producer copies in
   const bool fused_enc = ctx->fuse_encoder && !ctx->scene.use_ndc;
   if (!fused_enc && (s = ensure(ctx, ctx->tiles1, size_t(pad128(cap) / 128) * ctx->net[1].prog.in.tile_bytes())) != ADN_OK) return s;
   if ((s = ensure(ctx, ctx->raw1, size_t(pad128(cap)) * 16)) != ADN_OK) return s;
@@ -914,7 +913,7 @@ adn_status adn_set_option(adn_ctx* ctx, const char* name, int64_t value) {
     ctx->sample_budget = value;
     return ADN_OK;
   }
-  if (n == "fuse_encoder") {   // 1: positional encoding inside the shading kernel (no tile buffer); 0 (default): stage3_kernel + packed tiles
+  if (n == "fuse_encoder") {   // 1 (default): positional encoding inside the shading kernel (no tile buffer); 0: stage3_kernel + packed tiles
     ctx->fuse_encoder = value != 0;
     return ADN_OK;
   }

@@ -15,25 +15,36 @@ struct ConstFlags {
   __device__ constexpr operator uint8_t() const { return V; }
 };
 
+constexpr int kInSlots = 2;   // mlp_kernel<1>: input slots, so the producer fills one tile ahead of the consumers
+
 template <int NSPLIT>
 struct MlpCfg {
-  // activation blocks per term: the split net's input / hidden blocks; with NSPLIT == 1 the input blocks only (the
-  // sampling net's two, the shading net's P, then V), the hidden activations stay in registers
+  // NSPLIT == 2: activation blocks per term, the split net's input / hidden blocks.  NSPLIT == 1: the most input blocks a
+  // layer reads first (the sampling net's two, the shading net's one or two P blocks); the hidden activations stay in
+  // registers and the inputs sit in kInSlots slots of one packed tile each.
   static constexpr int kNB = (NSPLIT == 2) ? 4 : 2;
   static constexpr int kStageBytes = NSPLIT * kBlkBytes;              // one [128 x 64] weight block (+ its lo part)
-  // as many ring stages as fit next to the activations and the side parameters (227 KB per block)
-  static constexpr int kStages = (NSPLIT == 2) ? 2 : 8;
-  static constexpr size_t kActBytes = size_t(NSPLIT) * kNB * kBlkBytes;
-  static constexpr size_t kSmemBytes =
-      kActBytes + size_t(kStages) * kStageBytes + size_t(kSideFloats) * 4 + 2 * kStages * 8 + 1024 /*alignment slack*/;
+  // As many ring stages as fit next to the inputs and the side parameters (227 KB per block): two slots of a three-block
+  // tile (P > 64 columns) take two stages' room.
+  __host__ __device__ static constexpr int stages(int n_blk) { return NSPLIT == 2 ? 2 : (n_blk > 2 ? 6 : 8); }
+  __host__ __device__ static constexpr size_t in_bytes(int n_blk) {
+    return NSPLIT == 2 ? size_t(NSPLIT) * kNB * kBlkBytes : size_t(kInSlots) * n_blk * kBlkBytes;
+  }
+  __host__ __device__ static constexpr int n_bars(int n_blk) { return 2 * stages(n_blk) + (NSPLIT == 1 ? 2 * kInSlots : 0); }
+  __host__ __device__ static constexpr size_t smem_bytes(int n_blk) {
+    return in_bytes(n_blk) + size_t(stages(n_blk)) * kStageBytes + size_t(kSideFloats) * 4 + size_t(n_bars(n_blk)) * 8 +
+           1024 /*alignment slack*/;
+  }
+  // the largest over the tile formats the kernel runs (the split net's is fixed)
+  static constexpr size_t kMaxSmemBytes = smem_bytes(2) > smem_bytes(3) ? smem_bytes(2) : smem_bytes(3);
 };
-static_assert(MlpCfg<1>::kSmemBytes <= 232448 && MlpCfg<2>::kSmemBytes <= 232448, "shared memory per block (sm_90)");
+static_assert(MlpCfg<1>::kMaxSmemBytes <= 232448 && MlpCfg<2>::kMaxSmemBytes <= 232448, "shared memory per block (sm_90)");
 
-// Row `row` of the fused encoder's input blocks for a scene with any encoding but 10-4 (n_freq_pos <= 20, n_freq_dir
-// <= 10 bands): P (3 + 6 n_freq_pos features, in one block or two) into the blocks from `blk` on, or V into block `blk`,
-// each feature written as stage3_kernel<true> writes it, then zeros up to the block's end.
-__device__ __forceinline__ void encode_row_rt(const EncodeParams& enc, long long i, long long rows, uint8_t* blk, int row,
-                                              bool view) {
+// Row `row` of the fused encoder's input blocks (n_freq_pos <= 20, n_freq_dir <= 10 bands): P (3 + 6 n_freq_pos
+// features, in one block or two) into the blocks from `blk` on, or V into block `blk`, each feature written as stage 3
+// writes it (posenc3_rt, the bits of posenc3<L>; put_feature, the bits of pack_chunk8), then zeros up to the block's end.
+__device__ __forceinline__ void encode_row(const EncodeParams& enc, long long i, long long rows, uint8_t* blk, int row,
+                                           bool view) {
   const TileFormat act{1, 2, {0, 64, 0}, {64, 64, 0}};   // consecutive blocks: block b at blk + b * kBlkBytes
   const int n_p = 3 + 6 * enc.sc.n_freq_pos;
   zero_row(act, blk, uint32_t(row), 0, view ? 1 : shading_p_blocks(n_p));
@@ -53,37 +64,6 @@ __device__ __forceinline__ void encode_row_rt(const EncodeParams& enc, long long
     if (view) posenc3_rt(dir, enc.sc.n_freq_dir, put);
     else posenc3_rt(pos, enc.sc.n_freq_pos, put);
   }
-}
-
-// One row of a fused-encoder input block: P (the 63 position features and a zero column) or V (the 27 direction features
-// and zeros) of the shading tile format, computed and packed as stage3_kernel computes and packs them for a non-NDC scene.
-// Other encodings: encode_row_rt.
-template <bool VIEW>
-__device__ __forceinline__ void encode_row(const EncodeParams& enc, long long i, long long rows, uint8_t* blk, int row) {
-  if (enc.sc.n_freq_pos != 10 || enc.sc.n_freq_dir != 4) {
-    encode_row_rt(enc, i, rows, blk, row, VIEW);
-    return;
-  }
-  float f[64];
-#pragma unroll
-  for (int k = 0; k < 64; ++k) f[k] = 0.0f;
-  if (i < rows) {
-    long long ray;
-    float zw;
-    if (enc.ray_idx) {
-      ray = enc.ray_idx[i];
-      zw = enc.z[i];
-    } else {
-      ray = i / enc.K;
-      zw = enc.zlut_dense[i - ray * enc.K];
-    }
-    float pos[3], dir[3];
-    sample_inputs(enc.sc, false, enc.ray_o, enc.ray_d, ray, zw, pos, dir);
-    if (VIEW) posenc3<4>(dir, f);
-    else posenc3<10>(pos, f);
-  }
-#pragma unroll
-  for (int ch = 0; ch < 8; ++ch) pack_chunk8(f + ch * 8, uint32_t(row), ch, blk, nullptr);
 }
 
 // This warpgroup's 64 rows (the first or second 8 KB) of `nblk` consecutive packed blocks, global -> shared.
@@ -107,19 +87,28 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
   static_assert(!ENC || NSPLIT == 1, "fused input encoder: shading net (plain bf16) only");
   using Cfg = MlpCfg<NSPLIT>;
   constexpr int NB = Cfg::kNB;
-  constexpr int STAGES = Cfg::kStages;
+  const int STAGES = Cfg::stages(prog.in.n_blk);   // a constant for NSPLIT == 2
   constexpr int STAGE_BYTES = Cfg::kStageBytes;
   constexpr int kConsumerWarps = 8, kProducerWarp = 8;
+  constexpr int kEncThreads = 96;   // ENC: producer warps 9-11 encode the inputs
+  // The launch gives every thread 168 registers (__launch_bounds__(384, 1)); setmaxnreg only moves them between
+  // warpgroups, so 2 x kConsumerRegs + kProducerRegs <= 3 x 168 (a consumer increase beyond what the producers released
+  // would wait forever).  The shading net's consumers keep 128 accumulator and 64 A-fragment registers live through the
+  // MMAs; the encoder warps need more than the weight issuer's 24.
+  constexpr int kConsumerRegs = ENC ? 232 : 240, kProducerRegs = ENC ? 40 : 24;
+  static_assert(2 * kConsumerRegs + kProducerRegs <= 3 * 168, "registers the launch allocates");
 
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte aligned.  Offsetting smem_raw (rather than rounding an integer address) keeps every pointer below in the
   // shared state space, so the epilogue's reads of `side` and writes of `act` compile to LDS / STS, not generic accesses.
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* act = smem;                                                   // [NSPLIT][NB] blocks
-  uint8_t* ring = act + Cfg::kActBytes;                                  // [STAGES] stages
+  uint8_t* act = smem;   // NSPLIT == 2: [NSPLIT][NB] activation blocks; NSPLIT == 1: [kInSlots] input tiles
+  uint8_t* ring = act + Cfg::in_bytes(prog.in.n_blk);                    // [STAGES] stages
   float* side = reinterpret_cast<float*>(ring + size_t(STAGES) * STAGE_BYTES);
   uint64_t* w_full = reinterpret_cast<uint64_t*>(side + kSideFloats);   // [STAGES] the stage has landed
   uint64_t* w_empty = w_full + STAGES;                                   // [STAGES] every consumer warp's MMAs on it retired
+  uint64_t* in_full = w_empty + STAGES;                                  // NSPLIT == 1, [kInSlots]: the slot holds its tile
+  uint64_t* in_empty = in_full + kInSlots;                               // [kInSlots] every consumer warp is done with it
 
   const int warp = __shfl_sync(0xffffffffu, int(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
@@ -133,15 +122,52 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
       mbar_init(&w_full[s], 1);
       mbar_init(&w_empty[s], kConsumerWarps);
     }
+    if (NSPLIT == 1) {
+      for (int s = 0; s < kInSlots; ++s) {
+        mbar_init(&in_full[s], ENC ? kEncThreads : 1);
+        mbar_init(&in_empty[s], kConsumerWarps);
+      }
+    }
     mbar_fence_init();
   }
   __syncthreads();
 
   if (warp >= kProducerWarp) {
-    // ===================================================================== weight producer
-    setmaxnreg_dec<24>();
+    // ===================================================================== producers
+    setmaxnreg_dec<kProducerRegs>();
+    if (NSPLIT == 1 && warp > kProducerWarp) {
+      // ------------------------------------------------------------------- input producer (NSPLIT == 1)
+      // Fills the CTA's tiles into the slots in turn, one tile ahead of the consumers: ENC, warps 9-11 encode the rows
+      // (P, then V, of every row; 256 row tasks); otherwise one thread copies the packed tile with one bulk copy.
+      if (!ENC && !(warp == kProducerWarp + 1 && lane == 0)) return;
+      const uint32_t tile_bytes = prog.in.tile_bytes();
+      int slot = 0;
+      uint32_t phase = 0;
+      for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+        mbar_wait(&in_empty[slot], phase ^ 1, err_flag, 3);
+        uint8_t* dst = act + size_t(slot) * tile_bytes;
+        if constexpr (ENC) {
+          for (int task = int(threadIdx.x) - 32 * (kProducerWarp + 1); task < 2 * kTileM; task += kEncThreads) {
+            const int row = task & (kTileM - 1);
+            const bool view = task >= kTileM;
+            encode_row(enc, t * kTileM + row, rows, dst + (view ? prog.in_nblk0 : 0) * kBlkBytes, row, view);
+          }
+          fence_proxy_async_smem();   // generic-proxy stores -> visible to the consumers' wgmma reads
+          mbar_arrive(&in_full[slot]);
+        } else {
+          mbar_arrive_expect_tx(&in_full[slot], tile_bytes);
+          bulk_g2s(dst, in_tiles + size_t(t) * tile_bytes, tile_bytes, &in_full[slot]);
+        }
+        if (++slot == kInSlots) {
+          slot = 0;
+          phase ^= 1;
+        }
+      }
+      return;
+    }
+    // -------------------------------------------------------------------- weight producer
     // Stage i of a layer is [128 N rows x 64 K] (hi, then lo when NSPLIT == 2), N half outermost: the order the
-    // consumers walk them in.
+    // consumers walk them in.  It never waits on an input slot.
     if (warp == kProducerWarp && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -165,9 +191,7 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
   }
 
   // ============================================================================ consumer warpgroups
-  // 2 x 128 x 240 + 128 x 24 <= 64 K registers.  The shading net's consumers keep 128 accumulator and 64 A-fragment
-  // registers live through the MMAs; at 232 the fused encoder, which runs while a layer's fragments are live, spills.
-  setmaxnreg_inc<240>();
+  setmaxnreg_inc<kConsumerRegs>();
   const int wg = warp >> 2;                               // rows [64 wg, 64 wg + 64) of every tile
   const int tw = threadIdx.x & 127;
   const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2); // accumulator rows r0 and r0 + 8 of this thread
@@ -176,7 +200,8 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
   const uint32_t act_s = smem_u32(act);
   const uint32_t ring_s = smem_u32(ring);
   const uint32_t wg_off = uint32_t(wg) * (kBlkBytes / 2); // this warpgroup's rows inside a block
-  auto blk_addr = [&](int term, int blk) -> uint32_t { return act_s + uint32_t(term * NB + blk) * kBlkBytes; };
+  uint32_t in_s = act_s;                                  // the current tile's input blocks (NSPLIT == 1: its slot)
+  auto blk_addr = [&](int term, int blk) -> uint32_t { return in_s + uint32_t(term * NB + blk) * kBlkBytes; };
   const uint64_t desc_hi = make_desc_sw128(0) & ~uint64_t(0x3FFF);
   auto desc = [&](uint32_t addr) -> uint64_t { return desc_hi | uint64_t((addr & 0x3FFFF) >> 4); };
 
@@ -185,7 +210,7 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
   uint32_t afrag[4][4][4];
   // The compiler cannot see which layers read afrag (the layer program is read at run time), so every epilogue and every
   // tile start define all of it; the registers a layer does not write are never read.  Otherwise the previous values
-  // stay alive through MMAs, epilogues and the fused encoder, and spill.
+  // stay alive through MMAs and epilogues, and spill.
   auto clear_afrag = [&](int kb0, int kb1) {
 #pragma unroll
     for (int kb = 0; kb < 4; ++kb)
@@ -219,18 +244,21 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
     }
   };
 
+  int in_slot = 0;
+  uint32_t in_phase = 0;
   for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) {
-    // tile input (the previous tile's last MMAs retired before its epilogue: the blocks are free)
-    if (ENC) {
-      if (tw < 64) encode_row<false>(enc, t * kTileM + 64 * wg + tw, rows, act, 64 * wg + tw);
-    } else {
+    if constexpr (NSPLIT == 2) {
+      // tile input (the previous tile's last MMAs retired before its epilogue: the blocks are free)
 #pragma unroll
       for (int term = 0; term < NSPLIT; ++term)
         copy_rows(in_tiles + size_t(t) * prog.in.tile_bytes() + prog.in.blk_off(term, 0), blk_addr(term, 0), prog.in_nblk0, wg, tw);
+      fence_proxy_async_smem();
+      named_bar_sync(bar_id, 128);
+    } else {
+      mbar_wait(&in_full[in_slot], in_phase, err_flag, 4);   // the producer has filled this tile's slot
+      in_s = act_s + uint32_t(in_slot) * prog.in.tile_bytes();
+      clear_afrag(0, 4);
     }
-    fence_proxy_async_smem();
-    named_bar_sync(bar_id, 128);
-    if (NSPLIT == 1) clear_afrag(0, 4);
     float alpha[2] = {0.0f, 0.0f};
     for (int l = 0; l < prog.n_layers; ++l) {
       const MlpLayer& L = prog.layers[l];
@@ -268,16 +296,19 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
               wgmma_m64n128_bf16_rs(acc[nh], afrag[hb][k], desc(b + 32 * k), accumulate);
             });
           }
-          if (L.in_last) k_block(L.n_kb == 1, L.k_cnt[L.n_kb - 1], from_smem(0));
+          if (L.in_last) k_block(L.n_kb == 1, L.k_cnt[L.n_kb - 1], from_smem(prog.in_nblk0));   // V
         }
       }
       wgmma_wait<0>();
       if (lane == 0) mbar_arrive(&w_empty[prev]);
       prev = -1;
-      // All of the warpgroup's MMAs retired: the A blocks in shared memory may be overwritten in place.  The shading net
-      // overwrites its input block only after the LF_LOAD_IN1_AFTER layer and at the next tile's start.
-      const bool input_next = (L.flags & LF_LOAD_IN1_AFTER) || l + 1 == prog.n_layers;
-      if (NSPLIT == 2 || input_next) named_bar_sync(bar_id, 128);
+      if constexpr (NSPLIT == 2) {
+        // all of the warpgroup's MMAs retired: the A blocks in shared memory may be overwritten in place
+        named_bar_sync(bar_id, 128);
+      } else {
+        // the tile's last MMAs retired: its slot goes back to the input producer
+        if (l + 1 == prog.n_layers && lane == 0) mbar_arrive(&in_empty[in_slot]);
+      }
 
       // ------------------------------------------------------------------ epilogue
       // Instantiated per set of layer flags (a compile-time constant for the sets the networks use): with no branches in
@@ -362,17 +393,14 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
         case LF_FINAL_RAW: epilogue(ConstFlags<LF_FINAL_RAW>{}); break;
         default: epilogue(F(L.flags)); break;   // any other combination: the same code with run-time tests
       }
-      if (L.flags & LF_LOAD_IN1_AFTER) {   // the next input block (view directions) replaces activation block 0
-        if (ENC) {
-          if (tw < 64) encode_row<true>(enc, t * kTileM + 64 * wg + tw, rows, act, 64 * wg + tw);
-        } else {
-          copy_rows(in_tiles + size_t(t) * prog.in.tile_bytes() + prog.in.blk_off(0, prog.in_nblk0), blk_addr(0, 0), 1, wg, tw);
-        }
-      }
-      if (NSPLIT == 2 || (L.flags & LF_LOAD_IN1_AFTER)) {
+      if constexpr (NSPLIT == 2) {
         fence_proxy_async_smem();        // generic-proxy stores -> visible to the next layer's wgmma reads
         named_bar_sync(bar_id, 128);
       }
+    }
+    if (NSPLIT == 1 && ++in_slot == kInSlots) {
+      in_slot = 0;
+      in_phase ^= 1;
     }
   }
 }
@@ -413,9 +441,10 @@ static cudaError_t launch_mlp_t(const MlpProgram& prog, const uint8_t* wblob, co
                                 const long long* rows_dev, long long rows_host, int* err_flag, int num_sms, cudaStream_t stream,
                                 const EncodeParams& enc) {
   static unsigned long long attr_done = 0;   // per device
-  const size_t smem = MlpCfg<NSPLIT>::kSmemBytes;
+  if (prog.in.n_blk < 1 || prog.in.n_blk > 3) return cudaErrorInvalidValue;
+  const size_t smem = MlpCfg<NSPLIT>::smem_bytes(prog.in.n_blk);
   auto kernel = mlp_kernel<NSPLIT, ENC>;
-  cudaError_t e = set_max_dyn_smem_once(reinterpret_cast<const void*>(kernel), int(smem), &attr_done);
+  cudaError_t e = set_max_dyn_smem_once(reinterpret_cast<const void*>(kernel), int(MlpCfg<NSPLIT>::kMaxSmemBytes), &attr_done);
   if (e != cudaSuccess) return e;
   long long grid = num_sms;   // persistent: one CTA per SM
   if (!rows_dev) {

@@ -9,8 +9,10 @@
 //     bf16 nets (the accumulator fragment is the register-A fragment, 64 registers at W = 256), in
 //     swizzled shared memory as a hi+lo split for the split-precision net; a warpgroup only ever touches its own
 //     rows, so the layers of one warpgroup need no synchronisation with the other beyond the shared weight ring,
-//   * warp roles: warpgroups 0, 1 = consumers, warpgroup 2 = weight producer (one thread issues the copies); the
-//     producer hands most of its registers to the consumers (setmaxnreg), whose accumulators take 128 per thread.
+//   * warp roles: warpgroups 0, 1 = consumers, warpgroup 2 = producers: warp 8 issues the weight copies; with NSPLIT == 1
+//     warps 9-11 fill the next tile's inputs into the second of two input slots while the consumers run the current one
+//     (the fused encoder computes them; otherwise one bulk copy of the packed tile).  The producers hand most of their
+//     registers to the consumers (setmaxnreg), whose accumulators take 128 per thread.
 //
 // NSPLIT = 2 is the split-precision mode of the sampling network: x = hi + lo (both bf16) for
 // activations and weights and three MMAs per K step (hi*hi + lo*hi + hi*lo), fp32 accumulate --
@@ -35,13 +37,12 @@ enum : uint8_t {
   LF_ALPHA_DOT = 2,      // accumulate alpha = <post-activation row, alpha_w> on CUDA cores (fp32)
   LF_OUT_ACT = 4,        // write bf16 activations for the next layer
   LF_FINAL_RAW = 8,      // write fp32 rows to global (sampling net output / test programs)
-  LF_FINAL_RGB = 16,     // rgb_linear on CUDA cores + write float4 (rgb, alpha)
-  LF_LOAD_IN1_AFTER = 32   // once this layer's MMAs are done, fetch the input block after the tile-start ones (view dirs)
+  LF_FINAL_RGB = 16      // rgb_linear on CUDA cores + write float4 (rgb, alpha)
 };
 
-// Where a layer's A operand comes from, in K order: in_first input blocks (activation blocks 0, 1) in shared memory, then
-// n_hid hidden blocks, then input block 0 when in_last; n_kb = in_first + n_hid + in_last.  With NSPLIT == 1 (the shading
-// net, and the plain bf16 sampling net) the hidden blocks are in the registers the previous layer's epilogue wrote; the
+// Where a layer's A operand comes from, in K order: in_first input blocks (input blocks 0, 1) in shared memory, then
+// n_hid hidden blocks, then input block in_nblk0 (V) when in_last; n_kb = in_first + n_hid + in_last.  With NSPLIT == 1
+// (the shading net, and the plain bf16 sampling net) the hidden blocks are in the registers the previous layer's epilogue wrote; the
 // split-precision sampling net (NSPLIT == 2) keeps them as activation blocks 0 .. n_hid - 1, which each epilogue
 // overwrites in place, so there K block kb reads activation block kb.
 struct MlpLayer {
@@ -59,17 +60,16 @@ struct MlpLayer {
 struct MlpProgram {
   int32_t n_layers;
   TileFormat in;              // the packed input tiles (in.n_terms == NSPLIT)
-  int32_t in_nblk0;           // input blocks (per term) loaded into activation blocks 0.. at tile start; the next one
-                              // replaces block 0 after the LF_LOAD_IN1_AFTER layer
+  int32_t in_nblk0;           // input blocks (per term) the first layer reads; the shading net's V is the block after them
   uint32_t alpha_w_off, alpha_b_off, rgb_w_off, rgb_b_off;  // float offsets in `side`
   int32_t out_cols;           // row stride of the FINAL_RAW output
   MlpLayer layers[kMaxLayers];
   float side[kSideFloats];
 };
 
-// Fused input encoder of the shading MLP (stage 3 inside the kernel): the consumer warpgroups compute the positional
-// encoding of their packed samples (RayMarchFromPoses.batch, src/features.py:458-479) straight into the tile's input
-// block, so the [M, 90] feature tensor and its packed tiles never exist in HBM.  ray_idx == nullptr: dense mode
+// Fused input encoder of the shading MLP (stage 3 inside the kernel): producer warps 9-11 compute the positional encoding
+// of the packed samples (RayMarchFromPoses.batch, src/features.py:458-479) straight into the next tile's input slot, so
+// the [M, 90] feature tensor and its packed tiles never exist in HBM.  ray_idx == nullptr: dense mode
 // (ray = sample / K, z = zlut_dense[sample % K]).
 struct EncodeParams {
   const float* ray_o = nullptr;       // [N,3]

@@ -34,7 +34,7 @@ __host__ __device__ inline TileFormat sampling_tiles(int n_in, int n_terms) {
 
 // Shading net with n_p position and n_v view-direction features (3 + 6 bands each, n_p <= 128, n_v <= 64): [P | V] when
 // P fits one block, else [P0 | P1 | V] with P0 = features 0-63.  Each block holds its features and zeros after them.
-// The kernel loads the P blocks at tile start and V in place of block 0 after the LF_LOAD_IN1_AFTER layer.
+// The kernel holds the whole tile in one input slot: the P blocks feed layer 0 (and the skip consumer), V the view layer.
 // posEnc 10-4: [P | V] = [63 features and a zero column | 27 features and zeros].
 __host__ __device__ inline TileFormat shading_tiles(int n_p, int n_v) {
   if (n_p <= 64) return TileFormat{1, 2, {0, n_p, 0}, {n_p, n_v, 0}};

@@ -131,8 +131,9 @@ adn_status adn_probe_export_dir(const char* dir, adn_scene* scene_out, float* th
 
 /* name: "chunk_rays" (rays per internal batch, 0 = auto), "profile" (0/1 per-stage event timing),
  * "mlp0_terms" (3 = bf16x3 split precision [default], 1 = plain bf16; parity experiments only),
- * "fuse_encoder" (1 = positional encoding of the samples inside the shading kernel: no [M, P + V]-sized tile buffer;
- *   0 = separate kernel [default]),
+ * "fuse_encoder" (1 = positional encoding of the samples inside the shading kernel, a tile ahead of its MLP: no
+ *   [M, P + V]-sized tile buffer and no separate stage-3 launch [default]; NDC scenes always take the separate kernel;
+ *   0 = separate kernel; both render the same bits),
  * "sample_budget" (B > 0 = every adaptive render -- rays, aux, camera, rgba8, surface, *_host -- takes its `thr` as a floor
  *   and renders with the smallest threshold t* >= thr whose total sample count M over the whole call is <= B, chosen on
  *   the device with no host synchronisation; the picture is exactly that of a fixed-threshold call at t*.  Fails with
