@@ -33,6 +33,10 @@ class AuxOutputs(C.Structure):   # adn_aux_outputs: device pointers, any may be 
                 ("d_acc_map", C.c_void_p), ("d_disp_map", C.c_void_p), ("d_depth_est", C.c_void_p)]
 
 
+# adn_budget_reduce_fn: (user, uint64 d_words, n_words, stream) -> 0 on success
+BUDGET_REDUCE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p)
+
+
 class Stats(C.Structure):
     _fields_ = [("n_rays", C.c_int64), ("n_samples", C.c_int64), ("ms_stage", C.c_float * 6),
                 ("kernel_launches", C.c_int64)]
@@ -41,7 +45,7 @@ class Stats(C.Structure):
 # every symbol include/adanerf_b200.h declares (tests/test_abi.py checks the .so exports all of them)
 SYMBOLS = [
     "adn_create", "adn_destroy", "adn_strerror", "adn_last_error", "adn_version", "adn_set_weights",
-    "adn_create_from_export_dir", "adn_probe_export_dir", "adn_render_camera_surface", "adn_register_host_buffer", "adn_unregister_host_buffer", "adn_net_dims", "adn_net_shape", "adn_set_option", "adn_get_stats", "adn_last_threshold", "adn_render_rays", "adn_render_rays_aux", "adn_render_camera",
+    "adn_create_from_export_dir", "adn_probe_export_dir", "adn_render_camera_surface", "adn_register_host_buffer", "adn_unregister_host_buffer", "adn_net_dims", "adn_net_shape", "adn_set_option", "adn_get_stats", "adn_last_threshold", "adn_set_budget_group", "adn_render_rays", "adn_render_rays_aux", "adn_render_camera",
     "adn_render_camera_rgba8", "adn_render_rays_host", "adn_render_camera_host", "adn_stage0_features",
     "adn_generate_ray_directions", "adn_mlp0_forward", "adn_stage2_sample", "adn_budget_threshold", "adn_stage3_encode",
     "adn_mlp1_forward", "adn_stage5_composite", "adn_stage5_composite_aux", "adn_image_metrics",
@@ -79,6 +83,7 @@ def load_library():
     lib.adn_net_shape.argtypes = [vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.adn_get_stats.argtypes = [vp, C.POINTER(Stats)]
     lib.adn_last_threshold.argtypes = [vp, fp]
+    lib.adn_set_budget_group.argtypes = [vp, BUDGET_REDUCE_FN, vp]
     lib.adn_render_rays.argtypes = [vp, fp, fp, f32p, i64, C.c_float, C.c_int, f32p, i32p, f32p, vp]
     lib.adn_render_rays_aux.argtypes = [vp, fp, fp, f32p, i64, C.c_float, C.c_int, f32p, i32p, f32p, C.POINTER(AuxOutputs), vp]
     lib.adn_render_camera.argtypes = [vp, fp, fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, f32p, i32p, vp]

@@ -78,6 +78,7 @@ struct adn_ctx {
   Buf tiles0, raw0, ray_o, ray_d, count, offset, rayidx, zbuf, zpbuf, tiles1, raw1, s2scratch, rgba, metric;
   Buf dirs, rgb, nsamples;        // device side of the *_host entry points
   Buf budget_keys, budget_work, budget_thr;   // sample budget: candidate keys, histograms + select state, t*
+  BudgetGroup group;              // adn_set_budget_group: the reducer that sums the selection's histograms across members
   Buf total;                      // long long: samples of the last stage 2
   Buf watchdog{Buf::kPinned};     // int flag in mapped pinned host memory: still readable after a device trap
   int* d_err = nullptr;           // device view of watchdog
@@ -108,6 +109,13 @@ adn_status fail(adn_ctx* ctx, adn_status s, const std::string& msg) {
 }
 adn_status cuda_fail(adn_ctx* ctx, cudaError_t e, const char* where) {
   return fail(ctx, ADN_ERR_CUDA, std::string(where) + ": " + cudaGetErrorString(e));
+}
+// A budgeted call on a context in a budget group takes part in the group's reductions even when it has no rays.
+bool joins_group(const adn_ctx* ctx) { return ctx && ctx->sample_budget > 0 && ctx->group.fn; }
+// The status of a selection whose group reduction failed (launch_budget_threshold stopped enqueueing).
+adn_status group_fail(adn_ctx* ctx, const char* who) {
+  return fail(ctx, ADN_ERR_CUDA, std::string(who) + ": the budget group's reducer returned " + std::to_string(ctx->group.status) +
+                                     " in select round " + std::to_string(ctx->group.failed_round));
 }
 #define ADN_CUDA(ctx, call)                                   \
   do {                                                        \
@@ -657,7 +665,8 @@ adn_status render(adn_ctx* ctx, const RenderCall& call) {
   const int64_t n_rays = call.n_rays;
   const float thr = call.thr;
   const int K = call.K;
-  if (!ctx || !call.pose || !call.rot || n_rays < 0 || (!call.d_rgb && !call.d_rgba8))
+  const bool joins = joins_group(ctx);   // an empty call still joins the selection's reductions
+  if (!ctx || !call.pose || !call.rot || n_rays < 0 || (!call.d_rgb && !call.d_rgba8 && !(joins && n_rays == 0)))
     return fail(ctx, ADN_ERR_INVALID, "render: bad arguments");
   if (!ctx->net[0].ready || !ctx->net[1].ready) return fail(ctx, ADN_ERR_NO_WEIGHTS, "render: set both networks first");
   if (ctx->net[0].n_in != ctx->n_feat0 || ctx->net[0].n_out != 128)
@@ -674,8 +683,8 @@ adn_status render(adn_ctx* ctx, const RenderCall& call) {
     return fail(ctx, ADN_ERR_INVALID, "render: sample_budget supports at most 2^32 - 1 candidate samples (N * (K - 1)) per call");
   if (budget > 0 && (reinterpret_cast<uintptr_t>(call.d_oracle_w) & 15u))
     return fail(ctx, ADN_ERR_INVALID, "render: sample_budget needs 16-byte aligned d_oracle_weights rows");
-  if (n_rays == 0) return ADN_OK;
-  if (ctx->scene.use_ndc) {
+  if (n_rays == 0 && !joins) return ADN_OK;
+  if (ctx->scene.use_ndc && n_rays > 0) {
     // image size behind ndc_rays: the frame being rendered (viewer, featureset.cpp:83-84) or the dataset's (features.py:350-351,430)
     if (call.cam) set_ndc_projection(ctx, call.cam->W, call.cam->H, 0.0f);
     else if (ctx->scene.ndc_w > 0 && ctx->scene.ndc_h > 0) set_ndc_projection(ctx, ctx->scene.ndc_w, ctx->scene.ndc_h, ctx->scene.ndc_focal);
@@ -718,8 +727,10 @@ adn_status render(adn_ctx* ctx, const RenderCall& call) {
   if (ctx->profile) cudaEventRecord(ctx->ev[7], call.st);   // the selection is timed with stage 2 of the first chunk
   int launches = 0;
   ADN_CUDA(ctx, launch_budget_threshold(call.d_oracle_w ? call.d_oracle_w : ctx->raw0.as<float>(), n_rays, thr, K, budget,
-                                        ctx->budget_keys.as<uint32_t>(), ctx->budget_work.p, d_thr, ctx->num_sms, call.st, &launches));
+                                        ctx->budget_keys.as<uint32_t>(), ctx->budget_work.p, d_thr, ctx->num_sms, call.st, &launches,
+                                        &ctx->group));
   ctx->stats.kernel_launches += launches;
+  if (ctx->group.failed_round >= 0) return group_fail(ctx, "render");
   for (int64_t r0 = 0; r0 < n_rays; r0 += chunk)
     if ((s = run_stages_2_5(ctx, chunk_of(call, r0, chunk), r0, d_thr, ctx->profile && r0 == 0)) != ADN_OK) return s;
   return ADN_OK;
@@ -930,6 +941,13 @@ adn_status adn_set_option(adn_ctx* ctx, const char* name, int64_t value) {
   return fail(ctx, ADN_ERR_INVALID, "unknown option " + n);
 }
 
+adn_status adn_set_budget_group(adn_ctx* ctx, adn_budget_reduce_fn fn, void* user) {
+  if (!ctx) return ADN_ERR_INVALID;
+  ctx->group.fn = fn;
+  ctx->group.user = fn ? user : nullptr;
+  return ADN_OK;
+}
+
 adn_status adn_get_stats(adn_ctx* ctx, adn_stats* out) {
   if (!ctx || !out) return ADN_ERR_INVALID;
   ADN_CUDA(ctx, cudaSetDevice(ctx->device));
@@ -962,16 +980,16 @@ adn_status adn_last_threshold(adn_ctx* ctx, float* thr_out) {
 
 adn_status adn_render_rays(adn_ctx* ctx, const float* pose, const float* rot, const float* d_dirs, int64_t n_rays, float thr,
                            int K, float* d_rgb, int32_t* d_nsamples, float* d_oracle_weights, void* stream) {
-  if (ctx && n_rays == 0) return ADN_OK;   // empty batch: nothing to read or write
-  if (!d_dirs) return fail(ctx, ADN_ERR_INVALID, "render_rays: d_dirs is null");
+  if (ctx && n_rays == 0 && !joins_group(ctx)) return ADN_OK;   // empty batch: nothing to read or write
+  if (!d_dirs && n_rays != 0) return fail(ctx, ADN_ERR_INVALID, "render_rays: d_dirs is null");
   return adn_render_rays_aux(ctx, pose, rot, d_dirs, n_rays, thr, K, d_rgb, d_nsamples, d_oracle_weights, nullptr, stream);
 }
 
 adn_status adn_render_rays_aux(adn_ctx* ctx, const float* pose, const float* rot, const float* d_dirs, int64_t n_rays, float thr,
                                int K, float* d_rgb, int32_t* d_nsamples, float* d_oracle_weights, const adn_aux_outputs* aux,
                                void* stream) {
-  if (ctx && n_rays == 0) return ADN_OK;
-  if (!d_dirs) return fail(ctx, ADN_ERR_INVALID, "render_rays_aux: d_dirs is null");
+  if (ctx && n_rays == 0 && !joins_group(ctx)) return ADN_OK;
+  if (!d_dirs && n_rays != 0) return fail(ctx, ADN_ERR_INVALID, "render_rays_aux: d_dirs is null");
   RenderCall c(pose, rot, n_rays, thr, K, stream);
   c.d_dirs = d_dirs;
   c.d_rgb = d_rgb;
@@ -1010,7 +1028,7 @@ adn_status adn_render_camera_surface(adn_ctx* ctx, const float* pose, const floa
   adn_status s = order.begin("render_camera_surface");
   if (s != ADN_OK || (s = ensure(ctx, ctx->rgba, size_t(rows) * W * 4)) != ADN_OK) return s;
   c.d_rgba8 = ctx->rgba.as<uint8_t>();
-  if ((s = render(ctx, c)) != ADN_OK) return s;
+  if ((s = render(ctx, c)) != ADN_OK || rows == 0) return s;
   ADN_CUDA(ctx, launch_rgba_to_surface(c.d_rgba8, W, row0, rows, surface, c.st));
   ctx->stats.kernel_launches++;
   return ADN_OK;
@@ -1060,7 +1078,7 @@ adn_status adn_net_shape(adn_ctx* ctx, int net_id, int* depth, int* width, int* 
 adn_status adn_render_rays_host(adn_ctx* ctx, const float* pose, const float* rot, const float* h_dirs, int64_t n_rays,
                                 float thr, int K, float* h_rgb, int32_t* h_nsamples) {
   if (!ctx || !h_dirs || !h_rgb || n_rays < 0) return fail(ctx, ADN_ERR_INVALID, "render_rays_host: bad arguments");
-  if (n_rays == 0) return ADN_OK;
+  if (n_rays == 0 && !joins_group(ctx)) return ADN_OK;
   return render_host(ctx, RenderCall(pose, rot, n_rays, thr, K, nullptr), h_dirs, h_rgb, h_nsamples);
 }
 
@@ -1069,7 +1087,7 @@ adn_status adn_render_camera_host(adn_ctx* ctx, const float* pose, const float* 
   RenderCall c(pose, rot, int64_t(rows) * W, thr, K, nullptr);
   c.cam = camera_rays(ctx, W, H, row0, rows);
   if (!c.cam || !h_rgb) return fail(ctx, ADN_ERR_INVALID, "render_camera_host: bad arguments");
-  if (c.n_rays == 0) return ADN_OK;
+  if (c.n_rays == 0 && !joins_group(ctx)) return ADN_OK;
   return render_host(ctx, c, nullptr, h_rgb, h_nsamples);
 }
 
@@ -1144,9 +1162,10 @@ adn_status adn_budget_threshold(adn_ctx* ctx, const float* d_raw0, int64_t n_ray
     return s;
   int launches = 0;
   ADN_CUDA(ctx, launch_budget_threshold(d_raw0, n_rays, thr_min, K, max_samples, static_cast<uint32_t*>(ctx->budget_keys.p),
-                                        ctx->budget_work.p, d_thr, ctx->num_sms, static_cast<cudaStream_t>(stream), &launches));
+                                        ctx->budget_work.p, d_thr, ctx->num_sms, static_cast<cudaStream_t>(stream), &launches,
+                                        &ctx->group));
   ctx->stats.kernel_launches += launches;
-  return ADN_OK;
+  return ctx->group.failed_round >= 0 ? group_fail(ctx, "budget_threshold") : ADN_OK;
 }
 
 adn_status adn_stage3_encode(adn_ctx* ctx, const float* d_ray_o, const float* d_ray_d, const int32_t* d_ray, const float* d_z,

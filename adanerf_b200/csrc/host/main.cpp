@@ -40,14 +40,16 @@ int main(int argc, char** argv) {
   adn_host::Config config;
   if (!config.load(model)) { std::fprintf(stderr, "couldn't read export directory %s\n", model.c_str()); return 1; }
   std::printf("model %s: K = %d, adaptiveSamplingThreshold = %g\n", model.c_str(), config.numRaymarchSamples, config.adaptiveSamplingThreshold);
-  if (gpus > 1 && budget > 0) { std::fprintf(stderr, "--budget renders on one device (each row band would choose its own threshold)\n"); return 2; }
   if (gpus > 1) {
     // Row bands over `gpus` devices of this node + one NCCL gather per frame (include/adanerf_b200_multi.h); two frames
-    // in flight, so the gather of a frame overlaps the next frame's sampling MLP.
+    // in flight, so the gather of a frame overlaps the next frame's sampling MLP.  --budget: one frame budget, every band at
+    // the frame's threshold; frames are then rendered one at a time so that each one's threshold and M can be printed.
     adn_multi* m = nullptr;
     float thr = 0.f;
     int K = 0;
     if (adn_multi_create_from_export_dir(&m, model.c_str(), nullptr, gpus, &thr, &K) != ADN_OK) { std::fprintf(stderr, "multi-GPU load failed\n"); return 1; }
+    if (budget > 0 && adn_multi_set_option(m, "sample_budget", budget) != ADN_OK) { std::fprintf(stderr, "sample budget: %s\n", adn_multi_last_error(m)); return 1; }
+    std::vector<int64_t> band_m(size_t(gpus), 0);
     adn_host::Camera cam;
     cam.width = W;
     cam.height = H;
@@ -64,14 +66,24 @@ int main(int argc, char** argv) {
     std::chrono::steady_clock::time_point t0;
     for (int f = 0; f < frames + 2; ++f) {
       if (f == 2) {   // two warm-up frames (allocation, NCCL channel setup): drain, then time a full pipeline
-        if (adn_multi_wait_frame(m, nullptr, nullptr) != ADN_OK) { std::fprintf(stderr, "%s\n", adn_multi_last_error(m)); return 1; }
+        if (budget == 0 && adn_multi_wait_frame(m, nullptr, nullptr) != ADN_OK) { std::fprintf(stderr, "%s\n", adn_multi_last_error(m)); return 1; }
         t0 = std::chrono::steady_clock::now();
       }
       pose_at(f);
       if (adn_multi_render_camera(m, cam.pos, rot, W, H, thr, K) != ADN_OK) { std::fprintf(stderr, "%s\n", adn_multi_last_error(m)); return 1; }
+      if (budget > 0) {
+        if (adn_multi_wait_frame(m, nullptr, f == frames + 1 ? rgb.data() : nullptr) != ADN_OK) { std::fprintf(stderr, "%s\n", adn_multi_last_error(m)); return 1; }
+        if (f < 2) continue;
+        float t = 0.f;
+        if (adn_multi_last_threshold(m, &t) != ADN_OK || adn_multi_last_samples(m, band_m.data()) != ADN_OK) { std::fprintf(stderr, "%s\n", adn_multi_last_error(m)); return 1; }
+        long long total = 0;
+        for (int64_t b : band_m) total += b;
+        std::printf("frame %d: threshold %.7g, %lld samples (budget %lld)\n", f - 2, double(t), total, budget);
+        continue;
+      }
       if (f >= 1 && f != 2 && adn_multi_wait_frame(m, nullptr, nullptr) != ADN_OK) { std::fprintf(stderr, "%s\n", adn_multi_last_error(m)); return 1; }
     }
-    if (adn_multi_wait_frame(m, nullptr, rgb.data()) != ADN_OK) { std::fprintf(stderr, "%s\n", adn_multi_last_error(m)); return 1; }
+    if (budget == 0 && adn_multi_wait_frame(m, nullptr, rgb.data()) != ADN_OK) { std::fprintf(stderr, "%s\n", adn_multi_last_error(m)); return 1; }
     const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
     const size_t ng = size_t(gpus);
     std::vector<float> r_ms(ng, 0.f), g_ms(ng, 0.f);

@@ -4,6 +4,7 @@
 
 #include <cstdio>
 #include <string>
+#include <thread>
 #include <vector>
 
 #include "../../include/adanerf_b200_multi.h"
@@ -17,6 +18,7 @@ struct Dev {
   ncclComm_t comm = nullptr;
   cudaStream_t render = nullptr, comm_s = nullptr;
   float* band[2] = {nullptr, nullptr};
+  int32_t* ns[2] = {nullptr, nullptr};      // the band's per-ray sample counts
   size_t band_cap = 0;                      // floats per buffer
   cudaEvent_t start[2] = {}, rendered[2] = {}, gathered[2] = {};
 };
@@ -29,6 +31,7 @@ struct adn_multi {
   size_t frame_cap = 0;
   long long issued = 0, waited = 0;         // frames enqueued / handed out
   int W[2] = {0, 0}, H[2] = {0, 0};
+  int64_t budget = 0;                       // option "sample_budget": samples per frame, over all bands
   std::string err;
 };
 
@@ -53,6 +56,12 @@ adn_status fail(adn_multi* m, adn_status s, const std::string& msg) {
     adn_status s__ = (call);                                                                      \
     if (s__ != ADN_OK) return fail(m, s__, std::string(#call) + ": " + adn_last_error((d).ctx));  \
   } while (0)
+
+// adn_budget_reduce_fn of a device's context: sums a select round's histogram words over all devices' bands.
+int all_reduce_u64(void* user, uint64_t* d_words, int64_t n_words, void* stream) {
+  const Dev* d = static_cast<const Dev*>(user);
+  return ncclAllReduce(d_words, d_words, size_t(n_words), ncclUint64, ncclSum, d->comm, static_cast<cudaStream_t>(stream)) == ncclSuccess ? 0 : 1;
+}
 
 void band_of(int G, int H, int rank, int* row0, int* rows) {
   const int base = H / G, extra = H % G;
@@ -135,6 +144,7 @@ void adn_multi_destroy(adn_multi* m) {
     if (d.comm) ncclCommDestroy(d.comm);
     for (int k = 0; k < 2; ++k) {
       if (d.band[k]) cudaFree(d.band[k]);
+      if (d.ns[k]) cudaFree(d.ns[k]);
       if (d.start[k]) cudaEventDestroy(d.start[k]);
       if (d.rendered[k]) cudaEventDestroy(d.rendered[k]);
       if (d.gathered[k]) cudaEventDestroy(d.gathered[k]);
@@ -161,8 +171,14 @@ adn_status adn_multi_set_weights(adn_multi* m, int net_id, const adn_tensor_desc
 }
 
 adn_status adn_multi_set_option(adn_multi* m, const char* name, int64_t value) {
-  if (!m) return ADN_ERR_INVALID;
+  if (!m || !name) return ADN_ERR_INVALID;
   for (Dev& d : m->devs) MADN(m, d, adn_set_option(d.ctx, name, value));
+  if (std::string(name) == "sample_budget") {
+    // B holds for the frame: on several devices every band's selection sums its histograms with the other bands' (NCCL)
+    m->budget = value;
+    const bool group = value > 0 && m->devs.size() > 1;
+    for (Dev& d : m->devs) MADN(m, d, adn_set_budget_group(d.ctx, group ? all_reduce_u64 : nullptr, &d));
+  }
   return ADN_OK;
 }
 
@@ -179,6 +195,17 @@ adn_status adn_multi_render_camera(adn_multi* m, const float* pose, const float*
   const int G = int(m->devs.size());
   const int slot = int(m->issued & 1);
   const size_t frame_floats = size_t(W) * H * 3;
+  const int64_t n_rays = int64_t(W) * H;
+  // what a band cannot see for itself is refused here, before any device enqueues: a band that failed before its first
+  // reduction would leave the others waiting in theirs
+  if (m->budget > 0 && thr == 0.0f)
+    return fail(m, ADN_ERR_INVALID, "multi_render_camera: sample_budget needs the adaptive path (thr > 0), not dense mode");
+  if (m->budget > 0 && m->budget < n_rays)
+    return fail(m, ADN_ERR_INVALID, "multi_render_camera: sample_budget " + std::to_string(m->budget) + " is below the " +
+                                        std::to_string(n_rays) + " rays of the frame (every ray keeps at least one sample)");
+  if (m->budget > 0 && n_rays * (K - 1) >= (int64_t(1) << 32))
+    return fail(m, ADN_ERR_INVALID, "multi_render_camera: sample_budget supports at most 2^32 - 1 candidate samples (W * H * (K - 1)) per frame");
+  const bool grouped = m->budget > 0 && G > 1;
   Dev& d0 = m->devs[0];
   if (frame_floats > m->frame_cap) {   // (re)allocate both frame buffers: only when idle
     if (m->issued != m->waited) return fail(m, ADN_ERR_INVALID, "multi_render_camera: frame size changed with a frame in flight");
@@ -190,7 +217,6 @@ adn_status adn_multi_render_camera(adn_multi* m, const float* pose, const float*
     }
     m->frame_cap = frame_floats;
   }
-  // every device renders its band (its own rays from pose / rot / row window: no input scatter)
   for (int r = 0; r < G; ++r) {
     Dev& d = m->devs[size_t(r)];
     int row0, rows;
@@ -201,18 +227,58 @@ adn_status adn_multi_render_camera(adn_multi* m, const float* pose, const float*
       if (m->issued != m->waited) return fail(m, ADN_ERR_INVALID, "multi_render_camera: frame size changed with a frame in flight");
       for (int k = 0; k < 2; ++k) {
         if (d.band[k]) MCUDA(m, cudaFree(d.band[k]));
+        if (d.ns[k]) MCUDA(m, cudaFree(d.ns[k]));
         d.band[k] = nullptr;
+        d.ns[k] = nullptr;
         MCUDA(m, cudaMalloc(&d.band[k], n * sizeof(float)));
+        MCUDA(m, cudaMalloc(&d.ns[k], n / 3 * sizeof(int32_t)));
       }
       d.band_cap = n;
     }
-    // the band buffer of this slot was the source of the gather two frames ago
-    MCUDA(m, cudaStreamWaitEvent(d.render, d.gathered[slot], 0));
-    MCUDA(m, cudaEventRecord(d.start[slot], d.render));
-    if (rows > 0) MADN(m, d, adn_render_camera(d.ctx, pose, rot, W, H, row0, rows, thr, K, d.band[slot], nullptr, d.render));
-    MCUDA(m, cudaEventRecord(d.rendered[slot], d.render));
-    MCUDA(m, cudaStreamWaitEvent(d.comm_s, d.rendered[slot], 0));
   }
+  // every device renders its band (its own rays from pose / rot / row window: no input scatter), enqueued from a host
+  // thread of its own: a band's budget selection issues NCCL collectives, which one thread cannot issue for several
+  // devices outside a group call.  Under a budget a device with no rows still makes its empty call, to take part.
+  struct Enqueued {
+    adn_status s = ADN_OK;
+    std::string msg;
+  };
+  std::vector<Enqueued> res(static_cast<size_t>(G));
+  auto enqueue = [&](int r) {
+    Dev& d = m->devs[size_t(r)];
+    Enqueued& out = res[size_t(r)];
+    auto cuda = [&](cudaError_t e, const char* what) {
+      if (e != cudaSuccess) {
+        out.s = ADN_ERR_CUDA;
+        out.msg = std::string(what) + ": " + cudaGetErrorString(e);
+      }
+      return e == cudaSuccess;
+    };
+    int row0, rows;
+    band_of(G, H, r, &row0, &rows);
+    // the band buffer of this slot was the source of the gather two frames ago
+    if (!cuda(cudaSetDevice(d.device), "cudaSetDevice") || !cuda(cudaStreamWaitEvent(d.render, d.gathered[slot], 0), "cudaStreamWaitEvent") ||
+        !cuda(cudaEventRecord(d.start[slot], d.render), "cudaEventRecord"))
+      return;
+    if (rows > 0 || grouped) {
+      out.s = adn_render_camera(d.ctx, pose, rot, W, H, row0, rows, thr, K, d.band[slot], d.ns[slot], d.render);
+      if (out.s != ADN_OK) {
+        out.msg = std::string("adn_render_camera on device ") + std::to_string(d.device) + ": " + adn_last_error(d.ctx);
+        return;
+      }
+    }
+    if (cuda(cudaEventRecord(d.rendered[slot], d.render), "cudaEventRecord"))
+      cuda(cudaStreamWaitEvent(d.comm_s, d.rendered[slot], 0), "cudaStreamWaitEvent");
+  };
+  if (G == 1) {
+    enqueue(0);
+  } else {
+    std::vector<std::thread> threads;
+    for (int r = 0; r < G; ++r) threads.emplace_back(enqueue, r);
+    for (std::thread& t : threads) t.join();
+  }
+  for (const Enqueued& e : res)
+    if (e.s != ADN_OK) return fail(m, e.s, e.msg);
   // ONE gather of the RGB tiles on the first device: grouped send / recv over NVLink; the first device's own band is a
   // device-to-device copy on its communication stream
   {
@@ -263,6 +329,32 @@ adn_status adn_multi_wait_frame(adn_multi* m, const float** d_frame, float* h_rg
   if (h_rgb) {
     MCUDA(m, cudaSetDevice(m->devs[0].device));
     MCUDA(m, cudaMemcpy(h_rgb, m->frame[slot], size_t(m->W[slot]) * m->H[slot] * 3 * sizeof(float), cudaMemcpyDeviceToHost));
+  }
+  return ADN_OK;
+}
+
+adn_status adn_multi_last_threshold(adn_multi* m, float* thr_out) {
+  if (!m || !thr_out || m->issued == 0) return fail(m, ADN_ERR_INVALID, "multi_last_threshold: no frame enqueued");
+  Dev& d = m->devs[0];   // every band of a budgeted frame rendered at the same t*; the first band is never empty
+  MADN(m, d, adn_last_threshold(d.ctx, thr_out));
+  return ADN_OK;
+}
+
+adn_status adn_multi_last_samples(adn_multi* m, int64_t* band_samples) {
+  if (!m || !band_samples || m->issued == 0) return fail(m, ADN_ERR_INVALID, "multi_last_samples: no frame enqueued");
+  const int slot = int((m->issued - 1) & 1), G = int(m->devs.size());
+  std::vector<int32_t> ns;
+  for (int r = 0; r < G; ++r) {
+    Dev& d = m->devs[size_t(r)];
+    int row0, rows;
+    band_of(G, m->H[slot], r, &row0, &rows);
+    ns.resize(size_t(rows) * m->W[slot]);
+    MCUDA(m, cudaSetDevice(d.device));
+    MCUDA(m, cudaEventSynchronize(d.rendered[slot]));
+    if (!ns.empty()) MCUDA(m, cudaMemcpy(ns.data(), d.ns[slot], ns.size() * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    int64_t sum = 0;
+    for (int32_t c : ns) sum += c;
+    band_samples[r] = sum;
   }
   return ADN_OK;
 }

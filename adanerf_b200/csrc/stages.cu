@@ -662,17 +662,26 @@ cudaError_t launch_stage2(const float* d_raw0, long long n_rays, float thr, int 
 // S is positive, so float order is uint32 bit order: S is written as keys (0 = no entry) and the (Q+1)-th largest key is
 // found by a radix select over bits [31:21], [20:10], [9:0]; the first histogram is folded into the extraction pass.
 // Histograms use integer atomics (order independent), so t* is deterministic.
+//
+// The global histograms are uint64 words, and round 0 carries one more word, the call's ray count N (q = B - N is formed
+// on the device from it).  Integer sums do not depend on order, so members of a budget group (BudgetGroup) that add each
+// round's words across all members before its select all narrow to the same prefix: the t* of one call over every
+// member's rays.  Work layout: round 0 [kBudgetBins bins | N], round 1 [kBudgetBins], round 2 [kBudgetBins], BudgetState.
 constexpr int kBudgetBins = 2048;
+constexpr int kBudgetWords0 = kBudgetBins + 1;
 struct BudgetState {
   unsigned long long k;   // rank still sought inside the current prefix (1 = largest)
   uint32_t prefix;        // key bits fixed so far
   uint32_t done;          // 1: |S| <= Q, t* = thr_min
 };
-size_t budget_work_bytes() { return size_t(3 * kBudgetBins) * 4 + sizeof(BudgetState); }
+__host__ __device__ constexpr int budget_round_offset(int round) { return round == 0 ? 0 : kBudgetWords0 + (round - 1) * kBudgetBins; }
+size_t budget_work_bytes() { return size_t(budget_round_offset(3)) * 8 + sizeof(BudgetState); }
 
-__device__ __forceinline__ void budget_flush_hist(const uint32_t* s_hist, uint32_t* __restrict__ hist) {
+// Adds the CTA's histogram into the global one; CTA 0 also stores the call's ray count (the round-0 histogram's last word).
+__device__ __forceinline__ void budget_flush_hist(const uint32_t* s_hist, unsigned long long* __restrict__ hist, long long n_rays = -1) {
   for (int b = threadIdx.x; b < kBudgetBins; b += blockDim.x)
-    if (s_hist[b]) atomicAdd(hist + b, s_hist[b]);
+    if (s_hist[b]) atomicAdd(hist + b, (unsigned long long)s_hist[b]);
+  if (n_rays >= 0 && blockIdx.x == 0 && threadIdx.x == 0) hist[kBudgetBins] = (unsigned long long)n_rays;
 }
 
 // K <= 16: thread per ray, the group-maximum pop rounds of stage2_thread_kernel; pops 1..K-1 that are >= thr_min are the
@@ -680,7 +689,7 @@ __device__ __forceinline__ void budget_flush_hist(const uint32_t* s_hist, uint32
 // flushed once per CTA.
 __global__ void __launch_bounds__(kS2Rays)
 budget_keys_thread_kernel(const float* __restrict__ raw0, long long n_rays, float thr_min, int K, uint32_t* __restrict__ keys,
-                          uint32_t* __restrict__ hist) {
+                          unsigned long long* __restrict__ hist) {
   __shared__ __align__(16) uint8_t rows[kS2Rays * kS2tRowBytes];
   __shared__ uint32_t s_hist[kBudgetBins];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -721,14 +730,14 @@ budget_keys_thread_kernel(const float* __restrict__ raw0, long long n_rays, floa
     for (int i = tid; i < n_out; i += kS2Rays) keys[ray0 * KM1 + i] = st[i];
   }
   __syncthreads();
-  budget_flush_hist(s_hist, hist);
+  budget_flush_hist(s_hist, hist, n_rays);
 }
 
 // 16 < K <= 128: warp per ray with stage 2's select_cells; the selected cells minus one instance of
 // the largest value are the ray's keys (none when no cell reaches thr_min).
 __global__ void __launch_bounds__(kS2Threads)
 budget_keys_warp_kernel(const float* __restrict__ raw0, long long n_rays, float thr_min, int K, uint32_t* __restrict__ keys,
-                        uint32_t* __restrict__ hist) {
+                        unsigned long long* __restrict__ hist) {
   __shared__ uint32_t s_hist[kBudgetBins];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   for (int b = threadIdx.x; b < kBudgetBins; b += kS2Threads) s_hist[b] = 0;
@@ -772,13 +781,13 @@ budget_keys_warp_kernel(const float* __restrict__ raw0, long long n_rays, float 
     for (int p = n_keys + lane; p < KM1; p += 32) keys[r * KM1 + p] = 0u;
   }
   __syncthreads();
-  budget_flush_hist(s_hist, hist);
+  budget_flush_hist(s_hist, hist, n_rays);
 }
 
 // Rounds 1 and 2 of the select: histogram of the next key bits over the keys that carry the current prefix.
 __global__ void __launch_bounds__(256)
 budget_hist_kernel(const uint32_t* __restrict__ keys, long long n_keys, const BudgetState* __restrict__ st, int round,
-                   uint32_t* __restrict__ hist) {
+                   unsigned long long* __restrict__ hist) {
   __shared__ uint32_t s_hist[kBudgetBins];
   if (st->done) return;   // uniform
   const uint32_t prefix = st->prefix;
@@ -804,15 +813,16 @@ budget_hist_kernel(const uint32_t* __restrict__ keys, long long n_keys, const Bu
 }
 
 // One CTA: finds the bin of the k-th largest key (descending scan over the bins) and narrows the prefix.  Round 0 also
-// decides |S| <= Q; round 2 fixes the last bits and writes t*.
+// decides |S| <= Q, Q = max(B - N, 0) with N the ray count word; round 2 fixes the last bits and writes t*.
 __global__ void __launch_bounds__(1024)
-budget_select_kernel(const uint32_t* __restrict__ hist_all, BudgetState* __restrict__ st, int round, unsigned long long q,
-                     float thr_min, float* __restrict__ d_thr) {
+budget_select_kernel(const unsigned long long* __restrict__ hist_all, BudgetState* __restrict__ st, int round,
+                     unsigned long long max_samples, float thr_min, float* __restrict__ d_thr) {
   __shared__ unsigned long long s_warp[32];
   if (round > 0 && st->done) return;   // uniform
-  const uint32_t* hist = hist_all + round * kBudgetBins;
+  const unsigned long long* hist = hist_all + budget_round_offset(round);
   const int nb = round == 2 ? 1024 : 2048, per = nb / 1024;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const unsigned long long n = hist_all[kBudgetBins], q = max_samples > n ? max_samples - n : 0ull;
   const unsigned long long k = round == 0 ? q + 1 : st->k;
   unsigned long long s = 0;
   for (int u = 0; u < per; ++u) s += hist[nb - 1 - (tid * per + u)];   // thread 0 owns the highest bins
@@ -861,33 +871,53 @@ budget_select_kernel(const uint32_t* __restrict__ hist_all, BudgetState* __restr
 }
 
 cudaError_t launch_budget_threshold(const float* d_raw0, long long n_rays, float thr_min, int K, long long max_samples,
-                                    uint32_t* d_keys, void* d_work, float* d_thr, int num_sms, cudaStream_t s, int* launches) {
-  uint32_t* hist = static_cast<uint32_t*>(d_work);
-  BudgetState* st = reinterpret_cast<BudgetState*>(hist + 3 * kBudgetBins);
+                                    uint32_t* d_keys, void* d_work, float* d_thr, int num_sms, cudaStream_t s, int* launches,
+                                    BudgetGroup* group) {
+  unsigned long long* hist = static_cast<unsigned long long*>(d_work);
+  BudgetState* st = reinterpret_cast<BudgetState*>(hist + budget_round_offset(3));
+  const bool grouped = group && group->fn;
+  if (group) group->failed_round = -1;
   cudaError_t e = cudaMemsetAsync(d_work, 0, budget_work_bytes(), s);
   if (e != cudaSuccess) return e;
-  const unsigned long long q = (unsigned long long)(max_samples - n_rays);
+  // every round's words summed across the group, in place, ordered on s
+  auto reduce = [&](int round) {
+    if (!grouped) return true;
+    if ((e = cudaGetLastError()) != cudaSuccess) return false;
+    group->status = group->fn(group->user, reinterpret_cast<uint64_t*>(hist + budget_round_offset(round)), round == 0 ? kBudgetWords0 : kBudgetBins, s);
+    if (group->status != 0) group->failed_round = round;
+    return group->status == 0;
+  };
   const long long n_keys = n_rays * (K - 1);
+  // a group member runs every kernel and every reduction even without candidates: the others wait for its words
+  const bool select_all = n_keys > 0 || grouped;
   int n = 0;
-  if (n_keys > 0) {
+  if (select_all) {
     if (K <= 16) {
       const long long n_tiles = (n_rays + kS2Rays - 1) / kS2Rays;
-      budget_keys_thread_kernel<<<unsigned(std::min<long long>(n_tiles, 5ll * num_sms)), kS2Rays, 0, s>>>(d_raw0, n_rays, thr_min, K,
-                                                                                                         d_keys, hist);
+      budget_keys_thread_kernel<<<unsigned(std::max(1ll, std::min<long long>(n_tiles, 5ll * num_sms))), kS2Rays, 0, s>>>(
+          d_raw0, n_rays, thr_min, K, d_keys, hist);
     } else {
       const long long blocks = (n_rays + kS2Threads / 32 - 1) / (kS2Threads / 32);
-      budget_keys_warp_kernel<<<unsigned(std::min<long long>(blocks, 8ll * num_sms)), kS2Threads, 0, s>>>(d_raw0, n_rays, thr_min, K,
-                                                                                                         d_keys, hist);
+      budget_keys_warp_kernel<<<unsigned(std::max(1ll, std::min<long long>(blocks, 8ll * num_sms))), kS2Threads, 0, s>>>(
+          d_raw0, n_rays, thr_min, K, d_keys, hist);
     }
     ++n;
   }
-  budget_select_kernel<<<1, 1024, 0, s>>>(hist, st, 0, q, thr_min, d_thr);
+  if (!reduce(0)) {
+    if (launches) *launches += n;
+    return e;
+  }
+  budget_select_kernel<<<1, 1024, 0, s>>>(hist, st, 0, (unsigned long long)max_samples, thr_min, d_thr);
   ++n;
-  if (n_keys > 0) {
+  if (select_all) {
     const unsigned grid = unsigned(std::max<long long>(1, std::min<long long>((n_keys / 4 + 255) / 256, 4ll * num_sms)));
     for (int round = 1; round <= 2; ++round) {
-      budget_hist_kernel<<<grid, 256, 0, s>>>(d_keys, n_keys, st, round, hist + round * kBudgetBins);
-      budget_select_kernel<<<1, 1024, 0, s>>>(hist, st, round, q, thr_min, d_thr);
+      budget_hist_kernel<<<grid, 256, 0, s>>>(d_keys, n_keys, st, round, hist + budget_round_offset(round));
+      if (!reduce(round)) {
+        if (launches) *launches += n + 1;
+        return e;
+      }
+      budget_select_kernel<<<1, 1024, 0, s>>>(hist, st, round, (unsigned long long)max_samples, thr_min, d_thr);
       n += 2;
     }
   }

@@ -51,9 +51,23 @@ cudaError_t launch_stage2(const float* d_raw0, long long n_rays, float thr, int 
 // Sample budget: writes to *d_thr the smallest threshold t >= thr_min (> 0) at which stage 2 over raw0 [n_rays, 128] with K
 // samples per ray yields at most max_samples (>= n_rays) samples in all.  d_raw0 must be 16-byte aligned.
 // d_keys: [n_rays * (K - 1)] uint32 scratch; d_work: budget_work_bytes() of scratch.  Stream ordered, no host synchronisation; adds its kernel count to *launches.
+//
+// group (may be null, or have a null fn): the call is one member of a budget group.  fn is called on the host once per select
+// round, after the kernel that filled that round's histogram (2049 uint64 words in round 0: 2048 bins and the ray count,
+// 2048 in rounds 1 and 2), and must sum the words in place across all members, ordered on the stream it is given.  Every
+// member then selects the t* of all members' rays together (max_samples is the group's budget), and runs all three rounds
+// even with no rays or no candidates.  When fn returns non-zero the launcher stops enqueueing and records the status and
+// the round; *d_thr is then not written.
+struct BudgetGroup {
+  int (*fn)(void* user, uint64_t* d_words, int64_t n_words, void* stream) = nullptr;
+  void* user = nullptr;
+  int status = 0;          // fn's last return value
+  int failed_round = -1;   // the round whose reduction failed, -1 = none
+};
 size_t budget_work_bytes();
 cudaError_t launch_budget_threshold(const float* d_raw0, long long n_rays, float thr_min, int K, long long max_samples,
-                                    uint32_t* d_keys, void* d_work, float* d_thr, int num_sms, cudaStream_t s, int* launches);
+                                    uint32_t* d_keys, void* d_work, float* d_thr, int num_sms, cudaStream_t s, int* launches,
+                                    BudgetGroup* group = nullptr);
 // Dense (thr == 0): count = K, offset = ray*K, total = N*K; no index arrays are materialised.
 cudaError_t launch_stage2_dense(long long n_rays, int K, int32_t* d_count, int32_t* d_offset, long long* d_total,
                                 cudaStream_t s);

@@ -8,13 +8,13 @@ import torch
 
 from . import _lib
 from ._lib import AdnError, Scene, TensorDesc
-from .renderer import _fptr, _state_dict_of, make_scene
+from .renderer import _device_tensor, _fptr, _state_dict_of, make_scene
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 MULTI_LIB_PATH = os.environ.get("ADN_MULTI_LIB_PATH") or os.path.join(_HERE, "libadanerf_b200_multi.so")
 SYMBOLS = ["adn_multi_create", "adn_multi_create_from_export_dir", "adn_multi_destroy", "adn_multi_last_error", "adn_multi_devices",
            "adn_multi_set_weights", "adn_multi_set_option", "adn_multi_band", "adn_multi_render_camera", "adn_multi_wait_frame",
-           "adn_multi_last_times"]
+           "adn_multi_last_times", "adn_multi_last_threshold", "adn_multi_last_samples"]
 _multi = None
 
 
@@ -39,6 +39,8 @@ def load_multi_library():
         lib.adn_multi_render_camera.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_float, C.c_int]
         lib.adn_multi_wait_frame.argtypes = [vp, C.POINTER(vp), vp]
         lib.adn_multi_last_times.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_float)]
+        lib.adn_multi_last_threshold.argtypes = [vp, C.POINTER(C.c_float)]
+        lib.adn_multi_last_samples.argtypes = [vp, C.POINTER(C.c_int64)]
         _multi = lib
     return _multi
 
@@ -80,6 +82,7 @@ class MultiRenderer:
         self._check(self.lib.adn_multi_set_weights(self.handle, int(net_id), descs, len(sd)))
 
     def set_option(self, name, value):
+        """See adn_multi_set_option: "sample_budget" is the budget of the whole frame, one threshold for every band."""
         self._check(self.lib.adn_multi_set_option(self.handle, name.encode(), int(value)))
 
     def band(self, H, rank):
@@ -103,13 +106,25 @@ class MultiRenderer:
         self._waited += 1
         if host_out is not None:
             return host_out
-        return _device_tensor(ptr.value, shape, self.devices[0])
+        return _device_tensor(ptr.value, shape, "<f4", torch.device("cuda", self.devices[0]))
 
     def last_times(self):
         g = len(self.devices)
         a, b = (C.c_float * g)(), (C.c_float * g)()
         self._check(self.lib.adn_multi_last_times(self.handle, a, b))
         return list(a), list(b)
+
+    def last_threshold(self):
+        """The threshold the newest frame enqueued rendered at (t* under "sample_budget").  Synchronises."""
+        t = C.c_float()
+        self._check(self.lib.adn_multi_last_threshold(self.handle, C.byref(t)))
+        return t.value
+
+    def last_samples(self):
+        """[M of each band] of the newest frame enqueued; their sum is the frame's M.  Waits for that frame."""
+        out = (C.c_int64 * len(self.devices))()
+        self._check(self.lib.adn_multi_last_samples(self.handle, out))
+        return list(out)
 
     def close(self):
         if getattr(self, "handle", None):
@@ -121,12 +136,3 @@ class MultiRenderer:
             self.close()
         except Exception:
             pass
-
-
-def _device_tensor(ptr, shape, device):
-    """A torch tensor aliasing device memory owned by the library (__cuda_array_interface__)."""
-    class _Holder:
-        pass
-    h = _Holder()
-    h.__cuda_array_interface__ = dict(shape=tuple(shape), typestr="<f4", data=(int(ptr), False), version=3, strides=None)
-    return torch.as_tensor(h, device=torch.device("cuda", device))

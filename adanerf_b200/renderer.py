@@ -63,6 +63,8 @@ class Renderer:
         self.device = int(device)
         self.handle = C.c_void_p()
         self._registered = {}    # address -> numpy array page-locked through register_host_buffer (kept alive here)
+        self._reduce_cb = None    # the budget group's ctypes callback (set_budget_group), kept alive while installed
+        self._reduce_error = None  # the exception the reducer raised in the failing call
         self.n_feat0 = 90        # sampling-net input features (30 with the "2-2" encoding of the NDC configs)
         self.n_feat1 = 90        # shading-net input features: position, then view columns
         if _handle is not None:
@@ -97,7 +99,8 @@ class Renderer:
     def _check(self, st, create=False):
         if st != 0:
             detail = "" if create or not self.handle else (self.lib.adn_last_error(self.handle) or b"").decode()
-            raise AdnError(st, detail)
+            cause, self._reduce_error = self._reduce_error, None
+            raise AdnError(st, detail) from cause
 
     def close(self):
         if getattr(self, "handle", None):
@@ -126,6 +129,34 @@ class Renderer:
 
     def set_option(self, name, value):
         self._check(self.lib.adn_set_option(self.handle, name.encode(), int(value)))
+
+    def set_budget_group(self, fn):
+        """Joins a budget group (adn_set_budget_group): budgeted calls on this renderer and on the other members choose one
+        threshold under one budget, as one renderer would over all their rays.  fn(words) must sum `words` -- an int64
+        tensor on this renderer's device aliasing the library's uint64 histogram words -- in place across all members, on
+        the current stream (the call's), e.g. lambda t: dist.all_reduce(t, group=g).  The counts stay below 2^63, so the
+        signed sum is the unsigned one.  It runs on the thread that makes the call, once per select round.  An exception
+        in fn fails that call (AdnError, raised from the exception).  fn = None leaves the group."""
+        if fn is None:
+            self._check(self.lib.adn_set_budget_group(self.handle, _lib.BUDGET_REDUCE_FN(), None))
+            self._reduce_cb = None
+            return
+        dev = self._dev()
+
+        def reduce(_user, words, n_words, stream):
+            try:
+                t = _device_tensor(words, (n_words,), "<i8", dev)
+                st = torch.cuda.ExternalStream(stream, device=dev) if stream else torch.cuda.default_stream(dev)
+                with torch.cuda.device(dev), torch.cuda.stream(st):
+                    fn(t)
+                return 0
+            except BaseException as e:     # the library sees a failed reduction; _check raises from e
+                self._reduce_error = e
+                return 1
+
+        cb = _lib.BUDGET_REDUCE_FN(reduce)
+        self._check(self.lib.adn_set_budget_group(self.handle, cb, None))
+        self._reduce_cb = cb               # the library calls it until the group is left
 
     def net_dims(self, net_id):
         n_in, n_out = C.c_int(), C.c_int()
@@ -387,6 +418,15 @@ class Renderer:
             for k in ("weights", "depth_map"):
                 out.setdefault(k, None)
         return out
+
+
+def _device_tensor(ptr, shape, typestr, device):
+    """A torch tensor aliasing device memory owned by the library (__cuda_array_interface__)."""
+    class _Holder:
+        pass
+    h = _Holder()
+    h.__cuda_array_interface__ = dict(shape=tuple(shape), typestr=typestr, data=(int(ptr), False), version=3, strides=None)
+    return torch.as_tensor(h, device=device)
 
 
 _RENDERERS = {}

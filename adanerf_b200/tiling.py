@@ -45,9 +45,30 @@ def gather_bands(band, W, H, group=None, dst=None):
     return torch.cat([p[:rows * W] for p, (_, rows) in zip(parts, bands)], 0)
 
 
-def render_frame_distributed(renderer, pose, rot, W, H, thr, K, group=None, dst=None):
-    """Each rank renders its row band (adn_render_camera with row0/rows) and the tiles are gathered."""
+def render_frame_distributed(renderer, pose, rot, W, H, thr, K, group=None, dst=None, sample_budget=None):
+    """Each rank renders its row band (adn_render_camera with row0/rows) and the tiles are gathered.
+
+    sample_budget=B: at most B samples in the whole frame, every band at the one threshold a single renderer would choose
+    for the frame (the gathered frame equals its budgeted frame bit for bit).  The ranks' renderers form a budget group
+    whose reducer is dist.all_reduce(SUM) over `group`, for this call; afterwards the renderer has no budget and no group.
+    Every rank checks the budget against the frame before anything is enqueued, so all ranks refuse the same frames."""
     rank = dist.get_rank(group)
     row0, rows = row_bands(H, dist.get_world_size(group))[rank]
-    band = renderer.render_camera(pose, rot, W, H, thr, K, row0=row0, rows=rows)["rgb"]
+    if sample_budget is None:
+        band = renderer.render_camera(pose, rot, W, H, thr, K, row0=row0, rows=rows)["rgb"]
+        return gather_bands(band, W, H, group=group, dst=dst)
+    B = int(sample_budget)
+    if not thr > 0:
+        raise ValueError("render_frame_distributed: sample_budget needs the adaptive path (thr > 0), not dense mode")
+    if B < W * H:
+        raise ValueError(f"render_frame_distributed: sample_budget {B} is below the {W * H} rays of the frame")
+    if W * H * (K - 1) >= 1 << 32:
+        raise ValueError("render_frame_distributed: sample_budget supports at most 2^32 - 1 candidate samples (W * H * (K - 1))")
+    renderer.set_option("sample_budget", B)
+    renderer.set_budget_group(lambda words: dist.all_reduce(words, op=dist.ReduceOp.SUM, group=group))
+    try:
+        band = renderer.render_camera(pose, rot, W, H, thr, K, row0=row0, rows=rows)["rgb"]
+    finally:
+        renderer.set_budget_group(None)
+        renderer.set_option("sample_budget", 0)
     return gather_bands(band, W, H, group=group, dst=dst)

@@ -140,8 +140,31 @@ adn_status adn_probe_export_dir(const char* dir, adn_scene* scene_out, float* th
  *   ADN_ERR_INVALID in dense mode (thr == 0) and when B < n_rays.  The stage-2 slot of ms_stage includes the selection.
  *   Calls of more than one chunk keep raw0 and the ray origins / directions of the whole call (536 B per ray: the caller's
  *   d_oracle_weights when given, else context scratch).  0 = off [default]).
- *   The frame cost follows M, so B is a frame-time knob; row bands (multi-GPU) each choose their own t*. */
+ *   The frame cost follows M, so B is a frame-time knob.  Row bands of one frame share one t* and one B through a budget
+ *   group (adn_set_budget_group below); without one each call chooses its own. */
 adn_status adn_set_option(adn_ctx* ctx, const char* name, int64_t value);
+
+/* Budget group: several contexts (one per row band, on one device or several) whose budgeted calls choose ONE threshold, the
+ * t* a single context would choose over all their rays together, under ONE budget B.  The threshold selection is an exact
+ * radix select over integer histograms, so it is enough that every member sums its histograms with the others' before each
+ * of its three select rounds.  The context calls `fn` on the host, from the thread that makes the call, while it enqueues:
+ * once per round (after the candidate extraction, then after each histogram kernel).  `fn` must add d_words[0 .. n_words)
+ * (uint64 device memory; 2049 words in round 0 -- 2048 bins and the member's ray count --, 2048 in rounds 1 and 2) in place
+ * across all members, ordered on `stream` (the call's stream, a cudaStream_t; NULL = legacy default stream), and return 0,
+ * e.g. ncclAllReduce(d_words, d_words, n_words, ncclUint64, ncclSum, comm, stream).  Counts stay below 2^63, so a signed
+ * 64-bit sum gives the same words.  Q = B - sum N is formed on the device, 0 when sum N > B.
+ * Every budgeted call honours the group -- rays, aux, camera, rgba8, surface, *_host -- and so does adn_budget_threshold.
+ * A budgeted call with no rays still runs the selection and every reduction (it renders nothing and may pass NULL outputs).
+ * Contract between the members:
+ *   - every member makes the same sequence of budgeted calls, with the same `thr`, `K` and sample budget B;
+ *   - checks that can differ between members (B >= the rays of all members, the 2^32 - 1 candidate limit over all
+ *     members, dense mode) are made by the caller before any member enqueues: a member refuses a call before its first
+ *     reduction only for what it can see itself;
+ *   - a member whose call fails before its first reduction leaves the others waiting in theirs.
+ * A non-zero return from `fn` fails the call with ADN_ERR_CUDA (adn_last_error names the round) and nothing more of it is
+ * enqueued; the context stays usable.  fn = NULL leaves the group: calls choose their own threshold again. */
+typedef int (*adn_budget_reduce_fn)(void* user, uint64_t* d_words, int64_t n_words, void* stream);
+adn_status adn_set_budget_group(adn_ctx* ctx, adn_budget_reduce_fn fn, void* user);
 adn_status adn_get_stats(adn_ctx* ctx, adn_stats* out);   /* synchronises the context's stream */
 /* The threshold the last render call used: t* under "sample_budget", else its `thr` argument.  Synchronises like
  * adn_get_stats. */

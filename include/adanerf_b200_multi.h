@@ -1,6 +1,7 @@
 /* adanerf_b200 -- multi-GPU frame renderer (libadanerf_b200_multi.so, links NCCL).
  *
- * One host thread drives G devices of one node: one adn_ctx per device (weights replicated), contiguous row bands of the
+ * One host thread drives G devices of one node (each frame's bands are enqueued from one short-lived thread per device
+ * when G > 1): one adn_ctx per device (weights replicated), contiguous row bands of the
  * image per device (ray id = y * W + x, images are rgb.reshape(h, w, 3) with no flip -- src/util/saveimage.py:46 of
  * thomasneff/AdaNeRF), each device generates its own rays from (pose, rot, row0, rows), and ONE NCCL gather per frame
  * (grouped ncclSend / ncclRecv over NVLink) collects the RGB tiles on the first device.  ncclCommInitAll over the
@@ -33,6 +34,13 @@ int adn_multi_devices(const adn_multi* m);
 
 /* Same tensors to every device (see adn_set_weights). */
 adn_status adn_multi_set_weights(adn_multi* m, int net_id, const adn_tensor_desc* tensors, int n_tensors);
+/* The same option on every device (see adn_set_option), except "sample_budget": B > 0 is the budget of the whole frame.
+ * Every device's context joins a budget group (adn_set_budget_group) whose reducer is ncclAllReduce(ncclUint64, ncclSum)
+ * on that device's communicator and the band's stream, so all bands render at the one threshold t* a single device would
+ * choose for the frame (M <= B over all bands; the frame equals the single-GPU budgeted frame bit for bit).  The bands of a
+ * frame are then enqueued from one host thread per device, and a device with no rows still makes its (empty) budgeted
+ * call.  B < W * H, dense mode (thr == 0) and more than 2^32 - 1 candidates (W * H * (K - 1)) are refused for the whole
+ * frame before any device enqueues.  0 = off. */
 adn_status adn_multi_set_option(adn_multi* m, const char* name, int64_t value);
 
 /* Row band of device `rank` for an image of H rows: rows [row0, row0 + rows), whole rows, sizes differ by at most one. */
@@ -48,6 +56,13 @@ adn_status adn_multi_wait_frame(adn_multi* m, const float** d_frame, float* h_rg
 
 /* Device time of the last completed frame on each device: render (band) and gather, in ms; arrays of n_devices. */
 adn_status adn_multi_last_times(adn_multi* m, float* render_ms, float* gather_ms);
+
+/* The threshold the newest frame enqueued rendered at: t* under "sample_budget" (the same on every band), else its `thr`.
+ * Synchronises the first device. */
+adn_status adn_multi_last_threshold(adn_multi* m, float* thr_out);
+/* Samples M of each band of the newest frame enqueued (band_samples: array of n_devices; their sum is the frame's M).
+ * Waits for that frame's bands. */
+adn_status adn_multi_last_samples(adn_multi* m, int64_t* band_samples);
 
 #ifdef __cplusplus
 }
