@@ -48,7 +48,7 @@ SYMBOLS = [
     "adn_create_from_export_dir", "adn_probe_export_dir", "adn_render_camera_surface", "adn_register_host_buffer", "adn_unregister_host_buffer", "adn_net_dims", "adn_net_shape", "adn_set_option", "adn_get_stats", "adn_last_threshold", "adn_set_budget_group", "adn_render_rays", "adn_render_rays_aux", "adn_render_camera",
     "adn_render_camera_rgba8", "adn_render_rays_host", "adn_render_camera_host", "adn_stage0_features",
     "adn_generate_ray_directions", "adn_mlp0_forward", "adn_stage2_sample", "adn_budget_threshold", "adn_stage3_encode",
-    "adn_mlp1_forward", "adn_stage5_composite", "adn_stage5_composite_aux", "adn_image_metrics",
+    "adn_mlp1_forward", "adn_stage5_composite", "adn_stage5_composite_aux", "adn_image_metrics", "adn_sampling_view",
 ]
 
 _lib = None
@@ -96,6 +96,7 @@ def load_library():
     lib.adn_mlp0_forward.argtypes = [vp, f32p, i64, f32p, vp]
     lib.adn_stage2_sample.argtypes = [vp, f32p, i64, C.c_float, C.c_int, i32p, i32p, i32p, i32p, f32p, f32p, vp, vp]
     lib.adn_budget_threshold.argtypes = [vp, f32p, i64, C.c_float, C.c_int, i64, f32p, vp]
+    lib.adn_sampling_view.argtypes = [vp, f32p, i64, f32p, vp]
     lib.adn_stage3_encode.argtypes = [vp, f32p, f32p, i32p, f32p, i64, f32p, vp]
     lib.adn_mlp1_forward.argtypes = [vp, f32p, i64, f32p, vp]
     lib.adn_stage5_composite.argtypes = [vp, f32p, f32p, f32p, i32p, i32p, i64, C.c_int, f32p, f32p, f32p, vp]

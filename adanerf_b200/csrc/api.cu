@@ -74,6 +74,9 @@ struct adn_ctx {
   bool last_budget = false;       // the last render chose its threshold on the device (in budget_thr)
   float last_thr = 0.0f;          // the last render's threshold argument
   bool prof_budget = false;       // the profiled render timed the selection with stage 2 (ev[7] -> ev[3])
+  bool sampling_view = false;     // adn_set_option "sampling_view": renders draw the sampling net's view (stages 0-1 + view)
+  bool last_view = false;         // the last render drew the view (it counts no samples)
+  bool prof_view = false;         // the profiled render drew the view (slots 2-4 unused, the view kernel in slot 5)
   // scratch
   Buf tiles0, raw0, ray_o, ray_d, count, offset, rayidx, zbuf, zpbuf, tiles1, raw1, s2scratch, rgba, metric;
   Buf dirs, rgb, nsamples;        // device side of the *_host entry points
@@ -659,8 +662,21 @@ adn_status run_stages_2_5(adn_ctx* ctx, const RenderCall& c, int64_t w, const fl
   return ADN_OK;
 }
 
+// The sampling net's view of one chunk in place of stages 2-5 (option "sampling_view"): reads what run_stages_0_1 wrote
+// for the same chunk.  The view counts no samples: d_nsamples is zeroed.  timing: record ev[5..6].
+adn_status run_view(adn_ctx* ctx, const RenderCall& c, bool timing) {
+  const float* raw0 = c.d_oracle_w ? c.d_oracle_w : ctx->raw0.as<float>();
+  if (c.d_nsamples) ADN_CUDA(ctx, cudaMemsetAsync(c.d_nsamples, 0, size_t(c.n_rays) * 4, c.st));
+  if (timing) cudaEventRecord(ctx->ev[5], c.st);
+  ADN_CUDA(ctx, launch_sampling_view(raw0, c.n_rays, c.d_rgb, c.d_rgba8, c.st));
+  ctx->stats.kernel_launches++;
+  if (timing) cudaEventRecord(ctx->ev[6], c.st);
+  return ADN_OK;
+}
+
 // The hot path for every render entry point: stream ordered, no host synchronisation.  The call runs in chunks of rays;
 // with a sample budget, stages 0-1 of every chunk, then one threshold for the whole call, then stages 2-5 of every chunk.
+// With option "sampling_view", stages 0-1 and the view of every chunk, and no sample budget.
 adn_status render(adn_ctx* ctx, const RenderCall& call) {
   const int64_t n_rays = call.n_rays;
   const float thr = call.thr;
@@ -673,7 +689,15 @@ adn_status render(adn_ctx* ctx, const RenderCall& call) {
     return fail(ctx, ADN_ERR_INVALID, "render: sampling net must be " + std::to_string(ctx->n_feat0) + " -> 128 for this scene's encoding");
   if (K < 1 || K > 128 || thr < 0.0f) return fail(ctx, ADN_ERR_INVALID, "render: need 1 <= K <= 128 and thr >= 0");
   if (thr == 0.0f && K != 128) return fail(ctx, ADN_ERR_INVALID, "render: dense mode (thr == 0) needs K == 128 (one sample per depth cell)");
-  const int64_t budget = ctx->sample_budget;
+  const bool view = ctx->sampling_view;
+  if (view) {
+    const adn_aux_outputs& a = call.aux;
+    if (a.d_weights || a.d_alpha || a.d_z_vals || a.d_depth_map || a.d_acc_map || a.d_disp_map || a.d_depth_est)
+      return fail(ctx, ADN_ERR_INVALID, "render: option sampling_view draws no auxiliary outputs (pass none)");
+    if (reinterpret_cast<uintptr_t>(call.d_oracle_w) & 15u)
+      return fail(ctx, ADN_ERR_INVALID, "render: option sampling_view needs 16-byte aligned d_oracle_weights rows");
+  }
+  const int64_t budget = view ? 0 : ctx->sample_budget;   // the view selects no samples
   if (budget > 0 && thr == 0.0f)
     return fail(ctx, ADN_ERR_INVALID, "render: sample_budget needs the adaptive path (thr > 0 is the floor threshold), not dense mode");
   if (budget > 0 && budget < n_rays)
@@ -703,7 +727,9 @@ adn_status render(adn_ctx* ctx, const RenderCall& call) {
   ctx->stats.n_rays = n_rays;
   ctx->last_budget = budget > 0;
   ctx->last_thr = thr;
+  ctx->last_view = view;
   if (ctx->profile) ctx->prof_budget = budget > 0;
+  if (ctx->profile) ctx->prof_view = view;
   // raw0 / ray_o / ray_d: one chunk's worth, or with a sample budget the whole call's (the threshold is chosen over all of
   // raw0 before any chunk runs stage 2)
   const int64_t span = budget > 0 ? n_rays : std::min(chunk, n_rays);
@@ -714,7 +740,8 @@ adn_status render(adn_ctx* ctx, const RenderCall& call) {
     for (int64_t r0 = 0; r0 < n_rays; r0 += chunk) {
       const RenderCall c = chunk_of(call, r0, chunk);
       const bool timing = ctx->profile && r0 == 0;
-      if ((s = run_stages_0_1(ctx, c, 0, timing)) != ADN_OK || (s = run_stages_2_5(ctx, c, 0, nullptr, timing)) != ADN_OK) return s;
+      if ((s = run_stages_0_1(ctx, c, 0, timing)) != ADN_OK) return s;
+      if ((s = view ? run_view(ctx, c, timing) : run_stages_2_5(ctx, c, 0, nullptr, timing)) != ADN_OK) return s;
     }
     return ADN_OK;
   }
@@ -924,6 +951,11 @@ adn_status adn_set_option(adn_ctx* ctx, const char* name, int64_t value) {
     ctx->sample_budget = value;
     return ADN_OK;
   }
+  if (n == "sampling_view") {   // 1: renders draw the sampling net's view (the viewer's render-oracle mode); 0 (default): off
+    if (value != 0 && value != 1) return fail(ctx, ADN_ERR_INVALID, "sampling_view must be 0 or 1");
+    ctx->sampling_view = value != 0;
+    return ADN_OK;
+  }
   if (n == "fuse_encoder") {   // 1 (default): positional encoding inside the shading kernel (no tile buffer); 0: stage3_kernel + packed tiles
     ctx->fuse_encoder = value != 0;
     return ADN_OK;
@@ -955,10 +987,14 @@ adn_status adn_get_stats(adn_ctx* ctx, adn_stats* out) {
   if (s != ADN_OK) return s;
   long long total = 0;
   ADN_CUDA(ctx, cudaMemcpy(&total, ctx->total.p, sizeof(total), cudaMemcpyDeviceToHost));
-  ctx->stats.n_samples = total;
+  ctx->stats.n_samples = ctx->last_view ? 0 : total;
   if (ctx->profile) {
     for (int i = 0; i < 6; ++i) {
       float ms = 0;
+      if (ctx->prof_view && i >= 2 && i <= 4) {   // the view runs no stages 2-4
+        ctx->stats.ms_stage[i] = 0.0f;
+        continue;
+      }
       // with a sample budget, stage 2's slot starts at the threshold selection (ev[7])
       const cudaEvent_t from = (i == 2 && ctx->prof_budget) ? ctx->ev[7] : ctx->ev[i];
       if (cudaEventElapsedTime(&ms, from, ctx->ev[i + 1]) == cudaSuccess) ctx->stats.ms_stage[i] = ms;
@@ -1144,6 +1180,23 @@ adn_status adn_stage2_sample(adn_ctx* ctx, const float* d_raw0, int64_t n_rays, 
   ADN_CUDA(ctx, launch_stage2(d_raw0, n_rays, thr, K, ctx->zlut.as<float>(), d_count, d_offset, d_cell, d_ray, d_z, d_zp,
                               reinterpret_cast<long long*>(d_total), ctx->s2scratch.p, &ctx->s2sync, static_cast<cudaStream_t>(stream)));
   ctx->stats.kernel_launches++;
+  return ADN_OK;
+}
+
+adn_status adn_sampling_view(adn_ctx* ctx, const float* d_raw0, int64_t n_rays, float* d_rgb, uint8_t* d_rgba8) {
+  if (!ctx || n_rays < 0 || (n_rays > 0 && (!d_raw0 || (!d_rgb && !d_rgba8))))
+    return fail(ctx, ADN_ERR_INVALID, "sampling_view: bad arguments");
+  if (reinterpret_cast<uintptr_t>(d_raw0) & 15u) return fail(ctx, ADN_ERR_INVALID, "sampling_view: d_raw0 must be 16-byte aligned");
+  if (n_rays == 0) return ADN_OK;
+  ADN_CUDA(ctx, cudaSetDevice(ctx->device));
+  const cudaStream_t st = ctx->own_stream;
+  {
+    CallOrder order(ctx, st);
+    if (adn_status s = order.begin("sampling_view"); s != ADN_OK) return s;
+    ADN_CUDA(ctx, launch_sampling_view(d_raw0, n_rays, d_rgb, d_rgba8, st));
+    ctx->stats.kernel_launches++;
+  }
+  ADN_CUDA(ctx, cudaStreamSynchronize(st));
   return ADN_OK;
 }
 

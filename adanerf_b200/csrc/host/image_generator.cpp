@@ -43,11 +43,20 @@ bool ImageGenerator::load(const Config& config, int device) {
   return true;
 }
 
+bool ImageGenerator::apply_options(int batch_size) {
+  if (batch_size > 0) adn_set_option(ctx_, "chunk_rays", batch_size);
+  if (adn_set_option(ctx_, "sampling_view", render_oracle_ ? 1 : 0) != ADN_OK) {
+    err_ = adn_last_error(ctx_);
+    return false;
+  }
+  return true;
+}
+
 bool ImageGenerator::inference(const Camera& camera, uint8_t* d_rgba8, int batch_size, int num_samples, void* stream) {
   if (!ctx_) return false;
   float rot[9];
   camera.rotation(rot);
-  if (batch_size > 0) adn_set_option(ctx_, "chunk_rays", batch_size);
+  if (!apply_options(batch_size)) return false;
   const adn_status s =
       adn_render_camera_rgba8(ctx_, camera.pos, rot, camera.width, camera.height, 0, camera.height, thr_, num_samples, d_rgba8, stream);
   if (s != ADN_OK) err_ = adn_last_error(ctx_);
@@ -59,7 +68,7 @@ bool ImageGenerator::inference(Camera& camera, unsigned long long output_surf, i
   if (!ctx_) return false;
   float rot[9];
   camera.rotation(rot);
-  if (batch_size > 0) adn_set_option(ctx_, "chunk_rays", batch_size);
+  if (!apply_options(batch_size)) return false;
   const adn_status s = adn_render_camera_surface(ctx_, camera.pos, rot, camera.width, camera.height, 0, camera.height, thr_, num_samples,
                                                  output_surf, nullptr);
   if (s != ADN_OK) err_ = adn_last_error(ctx_);
@@ -70,7 +79,7 @@ bool ImageGenerator::inference_host(const Camera& camera, float* h_rgb, int batc
   if (!ctx_) return false;
   float rot[9];
   camera.rotation(rot);
-  if (batch_size > 0) adn_set_option(ctx_, "chunk_rays", batch_size);
+  if (!apply_options(batch_size)) return false;
   const adn_status s =
       adn_render_camera_host(ctx_, camera.pos, rot, camera.width, camera.height, 0, camera.height, thr_, num_samples, h_rgb, h_nsamples);
   if (s != ADN_OK) err_ = adn_last_error(ctx_);

@@ -65,14 +65,24 @@ class ImageGenerator {
   bool set_sample_budget(int64_t max_samples);
   bool last_threshold(float* thr);
 
+  // ImageGenerator::switchRenderOracle (include/imagegenerator.h:69, the viewer's `O` key): toggles the render-oracle view.
+  // While it is on, every inference overload draws the sampling network's view (adn_set_option "sampling_view") instead
+  // of the rendered frame.
+  void switchRenderOracle() { render_oracle_ = !render_oracle_; }
+  bool renderOracle() const { return render_oracle_; }
+
   const char* last_error() const;
   bool stats(adn_stats* out);
   // The loaded network's shape (adn_net_shape): depth, width and skip layer (-1 = none).
   bool net_shape(int net_id, int* depth, int* width, int* skip);
 
  private:
+  // the per-frame options every inference overload applies before it renders: rays per batch and the render-oracle view
+  bool apply_options(int batch_size);
+
   adn_ctx* ctx_ = nullptr;
   float thr_ = 0.f;
+  bool render_oracle_ = false;
   std::string err_;
 };
 

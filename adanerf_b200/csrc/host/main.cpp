@@ -23,7 +23,7 @@ int main(int argc, char** argv) {
   std::string model = "sample/";
   int W = 800, H = 800, batch = -1, frames = 20, device = 0, gpus = 1;
   long long budget = 0;   // --budget: samples per frame (0 = fixed threshold)
-  bool write = false, surface = false;
+  bool write = false, surface = false, oracle = false;
   for (int i = 1; i < argc; ++i) {
     const std::string a = argv[i];
     if ((a == "-s" || a == "--size") && i + 2 < argc) { W = std::atoi(argv[++i]); H = std::atoi(argv[++i]); }
@@ -34,12 +34,27 @@ int main(int argc, char** argv) {
     else if (a == "--surface") surface = true;   // one frame through ImageGenerator::inference(camera, cudaSurfaceObject_t, ...)
     else if ((a == "-g" || a == "--gpus") && i + 1 < argc) gpus = std::atoi(argv[++i]);
     else if (a == "--budget" && i + 1 < argc) budget = std::atoll(argv[++i]);
+    else if (a == "--oracle") oracle = true;   // the sampling network's view (ImageGenerator::switchRenderOracle, the viewer's O key)
     else if (a[0] != '-') model = a;
-    else { std::fprintf(stderr, "usage: %s modelPath [-s W H] [-bs raysPerBatch] [-f frames] [-dev id] [-g gpus] [--budget samplesPerFrame] [--surface] [-w]\n", argv[0]); return 2; }
+    else { std::fprintf(stderr, "usage: %s modelPath [-s W H] [-bs raysPerBatch] [-f frames] [-dev id] [-g gpus] [--budget samplesPerFrame] [--oracle] [--surface] [-w]\n", argv[0]); return 2; }
   }
   adn_host::Config config;
   if (!config.load(model)) { std::fprintf(stderr, "couldn't read export directory %s\n", model.c_str()); return 1; }
   std::printf("model %s: K = %d, adaptiveSamplingThreshold = %g\n", model.c_str(), config.numRaymarchSamples, config.adaptiveSamplingThreshold);
+  // -w: the last frame as a binary PPM in the model directory, saturate(x) * 255 truncated (the viewer's pixels)
+  auto write_ppm = [&](const std::vector<float>& rgb) {
+    const std::string out = model + "/adn_frame.ppm";
+    FILE* fp = std::fopen(out.c_str(), "wb");
+    if (!fp) { std::fprintf(stderr, "cannot write %s\n", out.c_str()); return false; }
+    std::fprintf(fp, "P6\n%d %d\n255\n", W, H);
+    for (size_t i = 0; i < rgb.size(); ++i) {
+      const float v = rgb[i] > 0.f ? std::fmin(rgb[i], 1.f) : 0.f;
+      std::fputc(int(v * 255.0f), fp);
+    }
+    std::fclose(fp);
+    std::printf("wrote %s\n", out.c_str());
+    return true;
+  };
   if (gpus > 1) {
     // Row bands over `gpus` devices of this node + one NCCL gather per frame (include/adanerf_b200_multi.h); two frames
     // in flight, so the gather of a frame overlaps the next frame's sampling MLP.  --budget: one frame budget, every band at
@@ -49,6 +64,7 @@ int main(int argc, char** argv) {
     int K = 0;
     if (adn_multi_create_from_export_dir(&m, model.c_str(), nullptr, gpus, &thr, &K) != ADN_OK) { std::fprintf(stderr, "multi-GPU load failed\n"); return 1; }
     if (budget > 0 && adn_multi_set_option(m, "sample_budget", budget) != ADN_OK) { std::fprintf(stderr, "sample budget: %s\n", adn_multi_last_error(m)); return 1; }
+    if (oracle && adn_multi_set_option(m, "sampling_view", 1) != ADN_OK) { std::fprintf(stderr, "sampling view: %s\n", adn_multi_last_error(m)); return 1; }
     std::vector<int64_t> band_m(size_t(gpus), 0);
     adn_host::Camera cam;
     cam.width = W;
@@ -96,7 +112,7 @@ int main(int argc, char** argv) {
     for (float v : rgb) sum += v;
     std::printf("checksum %.6f\n", sum);
     adn_multi_destroy(m);
-    return 0;
+    return write && !write_ppm(rgb) ? 1 : 0;
   }
   adn_host::ImageGenerator gen;
   if (!gen.load(config, device)) { std::fprintf(stderr, "load failed: %s\n", gen.last_error()); return 1; }
@@ -112,6 +128,7 @@ int main(int argc, char** argv) {
     std::printf("net %d: %s %d x %d, skip %d, posEnc %s\n", id, id == 0 ? "sampling" : "shading", d, w, sk, enc);
   }
   if (budget > 0 && !gen.set_sample_budget(budget)) { std::fprintf(stderr, "sample budget: %s\n", gen.last_error()); return 1; }
+  if (oracle) gen.switchRenderOracle();
   std::vector<int32_t> ns(budget > 0 ? size_t(W) * H : 0);   // per-ray sample counts, for M under a budget
   adn_host::Camera cam;
   cam.width = W;
@@ -166,7 +183,7 @@ int main(int argc, char** argv) {
       }
       if (px[4 * i + 3] != 255) ++bad;
     }
-    std::printf("surface frame %dx%d: %zu mismatching bytes against the fp32 frame\n", W, H, bad);
+    std::printf("surface frame %dx%d%s: %zu mismatching bytes against the fp32 frame\n", W, H, oracle ? " (sampling view)" : "", bad);
     cudaDestroySurfaceObject(surf);
     cudaFreeArray(arr);
     if (bad) return 1;
@@ -176,17 +193,8 @@ int main(int argc, char** argv) {
   std::printf("%d frames %dx%d: %.3f ms/frame (%.1f fps), last frame %lld samples (%.2f per ray), %lld kernel launches\n", frames, W, H,
               total_ms / frames, 1000.0 * frames / total_ms, (long long)st.n_samples, double(st.n_samples) / (double(W) * H),
               (long long)st.kernel_launches);
-  if (write) {
-    const std::string out = model + "/adn_frame.ppm";
-    FILE* fp = std::fopen(out.c_str(), "wb");
-    if (!fp) { std::fprintf(stderr, "cannot write %s\n", out.c_str()); return 1; }
-    std::fprintf(fp, "P6\n%d %d\n255\n", W, H);
-    for (size_t i = 0; i < rgb.size(); ++i) {
-      const float v = rgb[i] > 0.f ? std::fmin(rgb[i], 1.f) : 0.f;
-      std::fputc(int(v * 255.0f), fp);
-    }
-    std::fclose(fp);
-    std::printf("wrote %s\n", out.c_str());
-  }
-  return 0;
+  double sum = 0;   // the same checksum as the multi-GPU path prints, of the last frame
+  for (float v : rgb) sum += v;
+  std::printf("checksum %.6f\n", sum);
+  return write && !write_ppm(rgb) ? 1 : 0;
 }

@@ -32,6 +32,7 @@ struct adn_multi {
   long long issued = 0, waited = 0;         // frames enqueued / handed out
   int W[2] = {0, 0}, H[2] = {0, 0};
   int64_t budget = 0;                       // option "sample_budget": samples per frame, over all bands
+  bool view = false;                        // option "sampling_view": the bands draw the sampling net's view (no budget)
   std::string err;
 };
 
@@ -179,6 +180,7 @@ adn_status adn_multi_set_option(adn_multi* m, const char* name, int64_t value) {
     const bool group = value > 0 && m->devs.size() > 1;
     for (Dev& d : m->devs) MADN(m, d, adn_set_budget_group(d.ctx, group ? all_reduce_u64 : nullptr, &d));
   }
+  if (std::string(name) == "sampling_view") m->view = value != 0;
   return ADN_OK;
 }
 
@@ -197,15 +199,16 @@ adn_status adn_multi_render_camera(adn_multi* m, const float* pose, const float*
   const size_t frame_floats = size_t(W) * H * 3;
   const int64_t n_rays = int64_t(W) * H;
   // what a band cannot see for itself is refused here, before any device enqueues: a band that failed before its first
-  // reduction would leave the others waiting in theirs
-  if (m->budget > 0 && thr == 0.0f)
+  // reduction would leave the others waiting in theirs.  The sampling net's view applies no budget.
+  const int64_t budget = m->view ? 0 : m->budget;
+  if (budget > 0 && thr == 0.0f)
     return fail(m, ADN_ERR_INVALID, "multi_render_camera: sample_budget needs the adaptive path (thr > 0), not dense mode");
-  if (m->budget > 0 && m->budget < n_rays)
-    return fail(m, ADN_ERR_INVALID, "multi_render_camera: sample_budget " + std::to_string(m->budget) + " is below the " +
+  if (budget > 0 && budget < n_rays)
+    return fail(m, ADN_ERR_INVALID, "multi_render_camera: sample_budget " + std::to_string(budget) + " is below the " +
                                         std::to_string(n_rays) + " rays of the frame (every ray keeps at least one sample)");
-  if (m->budget > 0 && n_rays * (K - 1) >= (int64_t(1) << 32))
+  if (budget > 0 && n_rays * (K - 1) >= (int64_t(1) << 32))
     return fail(m, ADN_ERR_INVALID, "multi_render_camera: sample_budget supports at most 2^32 - 1 candidate samples (W * H * (K - 1)) per frame");
-  const bool grouped = m->budget > 0 && G > 1;
+  const bool grouped = budget > 0 && G > 1;
   Dev& d0 = m->devs[0];
   if (frame_floats > m->frame_cap) {   // (re)allocate both frame buffers: only when idle
     if (m->issued != m->waited) return fail(m, ADN_ERR_INVALID, "multi_render_camera: frame size changed with a frame in flight");

@@ -941,6 +941,95 @@ cudaError_t launch_stage2_dense(long long n_rays, int K, int32_t* d_count, int32
   return cudaGetLastError();
 }
 
+// ------------------------------------------------------------------------------------- sampling-network view
+// The viewer's render-oracle picture (samplesToImage, adanerf_real_time_viewer/src/cuda/base_cuda_kernels.cu:487-528): per
+// ray the three cells c0, c1, c2 that come first when the 128 raw0 values are sorted in descending order by
+// cub::BlockRadixSort (stable), drawn as (c + 0.5) / 128.  Radix order is the order of the twiddled uint32 keys; the CUB of
+// CUDA 12.x ranks -0 as +0 (cub/block/radix_rank_sort_operations.cuh, ProcessFloatMinusZero), so a positive NaN ranks above
+// +inf, a negative NaN below -inf, and equal keys keep the lower cell first.  Nothing is sorted here: one thread per ray
+// (rows staged like stage2_thread_kernel's) runs three pop rounds over the 16 group maxima of its keys.
+__device__ __forceinline__ uint32_t view_key(float v) {
+  const uint32_t b = __float_as_uint(v);
+  const uint32_t k = (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+  return k == 0x7fffffffu ? 0x80000000u : k;   // -0 -> +0
+}
+
+__device__ __forceinline__ void view_group_keys(const uint8_t* row, int q, uint32_t (&x)[8]) {
+  const float4 a = reinterpret_cast<const float4*>(row)[2 * q], b = reinterpret_cast<const float4*>(row)[2 * q + 1];
+  x[0] = view_key(a.x), x[1] = view_key(a.y), x[2] = view_key(a.z), x[3] = view_key(a.w);
+  x[4] = view_key(b.x), x[5] = view_key(b.y), x[6] = view_key(b.z), x[7] = view_key(b.w);
+}
+
+__global__ void __launch_bounds__(kS2Rays)
+sampling_view_kernel(const float* __restrict__ raw0, long long n_rays, float* __restrict__ rgb, uchar4* __restrict__ rgba8) {
+  extern __shared__ __align__(16) uint8_t sv_smem[];
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const long long ray0 = (long long)blockIdx.x * kS2Rays;
+  const long long r = ray0 + tid;
+  s2t_fetch_rows(raw0, n_rays, ray0, sv_smem, warp, lane);
+  asm volatile("cp.async.wait_group 0;" ::: "memory");
+  __syncwarp();
+  if (r >= n_rays) return;
+  const uint8_t* row = sv_smem + tid * kS2tRowBytes;
+
+  uint32_t g[16];   // group maxima of the keys (groups of 8 cells)
+#pragma unroll
+  for (int q = 0; q < 16; ++q) {
+    uint32_t x[8];
+    view_group_keys(row, q, x);
+    g[q] = max(max(max(x[0], x[1]), max(x[2], x[3])), max(max(x[4], x[5]), max(x[6], x[7])));
+  }
+  int cell[3] = {-1, -1, -1};
+#pragma unroll
+  for (int j = 0; j < 3; ++j) {
+    uint32_t m = g[0];
+#pragma unroll
+    for (int q = 1; q < 16; ++q) m = max(m, g[q]);
+    int gi = 0;
+#pragma unroll
+    for (int q = 15; q >= 0; --q) gi = (g[q] == m) ? q : gi;   // first group holding the maximum
+    uint32_t x[8];
+    view_group_keys(row, gi, x);
+    // the first cell of that group holding the maximum that is not taken yet, and the group's maximum without it (at most
+    // two of its eight cells are taken, so it keeps one)
+    bool found = false;
+    int idx = 0;
+    uint32_t nm = 0u;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const int c = 8 * gi + i;
+      const bool taken = (c == cell[0]) || (c == cell[1]);
+      const bool e = !taken && !found && x[i] == m;
+      found = found || e;
+      idx = e ? i : idx;
+      nm = (taken || e) ? nm : max(nm, x[i]);
+    }
+#pragma unroll
+    for (int q = 0; q < 16; ++q) g[q] = (q == gi) ? nm : g[q];
+    cell[j] = 8 * gi + idx;
+  }
+  float v[3];
+#pragma unroll
+  for (int j = 0; j < 3; ++j) v[j] = (0.5f + float(cell[j])) / 128.0f;
+  if (rgb) {
+    rgb[3 * r] = v[0];
+    rgb[3 * r + 1] = v[1];
+    rgb[3 * r + 2] = v[2];
+  }
+  // clamp(v, 0, 1) * 255 converted to unsigned char (truncation), alpha 255: base_cuda_kernels.cu:522-526
+  if (rgba8)
+    rgba8[r] = make_uchar4((unsigned char)(__saturatef(v[0]) * 255.0f), (unsigned char)(__saturatef(v[1]) * 255.0f),
+                           (unsigned char)(__saturatef(v[2]) * 255.0f), 255);
+}
+
+cudaError_t launch_sampling_view(const float* d_raw0, long long n_rays, float* d_rgb, uint8_t* d_rgba8, cudaStream_t s) {
+  if (n_rays <= 0) return cudaSuccess;
+  const long long n_tiles = (n_rays + kS2Rays - 1) / kS2Rays;
+  sampling_view_kernel<<<unsigned(n_tiles), kS2Rays, size_t(kS2Rays) * kS2tRowBytes, s>>>(d_raw0, n_rays, d_rgb,
+                                                                                        reinterpret_cast<uchar4*>(d_rgba8));
+  return cudaGetLastError();
+}
+
 // ------------------------------------------------------------------------------------- stage 3
 // RayMarchFromPoses.batch (src/features.py:458-479): one thread per packed sample.  RT == false: posEnc 10-4 at compile
 // time.  RT == true: sc.n_freq_pos (<= 20) and sc.n_freq_dir (<= 10) bands, the features written one at a time into x1

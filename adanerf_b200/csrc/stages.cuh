@@ -72,6 +72,11 @@ cudaError_t launch_budget_threshold(const float* d_raw0, long long n_rays, float
 cudaError_t launch_stage2_dense(long long n_rays, int K, int32_t* d_count, int32_t* d_offset, long long* d_total,
                                 cudaStream_t s);
 
+// The sampling network's view (the viewer's render-oracle mode): raw0 [n_rays, 128] (16-byte aligned) -> per ray the three
+// cells that lead raw0's stable descending radix order, as (c + 0.5) / 128 into d_rgb [n_rays, 3] and as uchar4 pixels
+// (value * 255 truncated, alpha 255) into d_rgba8 [n_rays]; either output may be null.
+cudaError_t launch_sampling_view(const float* d_raw0, long long n_rays, float* d_rgb, uint8_t* d_rgba8, cudaStream_t s);
+
 // Stage 3.  Adaptive: sample s -> (d_ray[s], d_z[s]).  Dense (d_ray == nullptr): ray = s / K,
 // z = d_zlut_dense[s % K].  n_samples read from d_total when non-null.  d_x1 (fp32 features) and d_tiles1 (the shading
 // net's packed input tiles, shading_tiles in tiles.cuh) may be null (not written).

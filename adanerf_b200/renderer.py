@@ -364,6 +364,26 @@ class Renderer:
                                                   t.data_ptr(), self._stream()))
         return t
 
+    def sampling_view(self, raw0, rgb=True, rgba8=True):
+        """The sampling network's view of raw0 [N,128] (adn_sampling_view, the viewer's render-oracle picture) ->
+        dict(rgb [N,3] float32, rgba8 [N,4] uint8); an output asked for with False is None.  Waits for the current stream
+        first: the call runs on the context's own stream and returns once its outputs are written.  Refused while the
+        current stream captures a CUDA graph (that wait would end the capture)."""
+        if torch.cuda.is_current_stream_capturing():
+            raise AdnError(1, "sampling_view: the current stream is capturing a CUDA graph; the call synchronises and cannot "
+                              "be captured")
+        x = self._f32(raw0)
+        if x.dim() != 2 or x.shape[1] != 128:
+            raise ValueError("sampling_view: raw0 must be [N, 128]")
+        n, dev = x.shape[0], self._dev()
+        out = dict(rgb=torch.empty((n, 3), dtype=torch.float32, device=dev) if rgb else None,
+                   rgba8=torch.empty((n, 4), dtype=torch.uint8, device=dev) if rgba8 else None)
+        ptr = lambda t: t.data_ptr() if t is not None else None
+        with torch.cuda.device(self.device):
+            torch.cuda.current_stream().synchronize()
+            self._check(self.lib.adn_sampling_view(self.handle, x.data_ptr(), n, ptr(out["rgb"]), ptr(out["rgba8"])))
+        return out
+
     def stage3(self, ray_o, ray_d, ray_idx, z):
         ro, rd, zz = self._f32(ray_o), self._f32(ray_d), self._f32(z)
         ri = ray_idx.to(device=self._dev(), dtype=torch.int32).contiguous()

@@ -141,7 +141,17 @@ adn_status adn_probe_export_dir(const char* dir, adn_scene* scene_out, float* th
  *   Calls of more than one chunk keep raw0 and the ray origins / directions of the whole call (536 B per ray: the caller's
  *   d_oracle_weights when given, else context scratch).  0 = off [default]).
  *   The frame cost follows M, so B is a frame-time knob.  Row bands of one frame share one t* and one B through a budget
- *   group (adn_set_budget_group below); without one each call chooses its own. */
+ *   group (adn_set_budget_group below); without one each call chooses its own.
+ * "sampling_view" (1 = every render -- rays, aux, camera, rgba8, surface, *_host -- draws the sampling network's view, the
+ *   C++ viewer's render-oracle mode behind ImageGenerator::switchRenderOracle (imagegenerator.cpp:316-326): stage 0 and the
+ *   sampling MLP run, then per ray the three depth cells c0, c1, c2 that lead the sampling net's output in descending order
+ *   are drawn as (c + 0.5) / 128 into rgb, and as uchar4 (value * 255 truncated, alpha 255) into the RGBA8 / surface
+ *   pixels (samplesToImage, base_cuda_kernels.cu:487-528; see adn_sampling_view for the order); stages 2-5 do not run.
+ *   In this mode `thr` / `K` are validated as before but not used; d_oracle_weights still receives raw0 (its rows must be
+ *   16-byte aligned); d_nsamples receives 0 for every ray; non-NULL auxiliary outputs fail with ADN_ERR_INVALID;
+ *   "sample_budget" is not applied (no selection runs, a budget group makes no reductions, adn_last_threshold returns
+ *   `thr`); adn_get_stats reports n_samples = 0 and, profiled, stages 0-1 in ms_stage[0..1], the view in ms_stage[5] and 0
+ *   in ms_stage[2..4].  0 = off [default]: renders are exactly as without the option). */
 adn_status adn_set_option(adn_ctx* ctx, const char* name, int64_t value);
 
 /* Budget group: several contexts (one per row band, on one device or several) whose budgeted calls choose ONE threshold, the
@@ -156,7 +166,8 @@ adn_status adn_set_option(adn_ctx* ctx, const char* name, int64_t value);
  * Every budgeted call honours the group -- rays, aux, camera, rgba8, surface, *_host -- and so does adn_budget_threshold.
  * A budgeted call with no rays still runs the selection and every reduction (it renders nothing and may pass NULL outputs).
  * Contract between the members:
- *   - every member makes the same sequence of budgeted calls, with the same `thr`, `K` and sample budget B;
+ *   - every member makes the same sequence of budgeted calls, with the same `thr`, `K` and sample budget B, and the same
+ *     value of option "sampling_view" (a member drawing the view makes no reductions);
  *   - checks that can differ between members (B >= the rays of all members, the 2^32 - 1 candidate limit over all
  *     members, dense mode) are made by the caller before any member enqueues: a member refuses a call before its first
  *     reduction only for what it can see itself;
@@ -260,6 +271,17 @@ adn_status adn_stage2_sample(adn_ctx* ctx, const float* d_raw0, int64_t n_rays, 
  * rank-2..K values. */
 adn_status adn_budget_threshold(adn_ctx* ctx, const float* d_raw0, int64_t n_rays, float thr_min, int K, int64_t max_samples,
                                 float* d_thr, void* stream);
+/* The sampling network's view of raw0 alone (what option "sampling_view" draws after the sampling MLP), the viewer's
+ * samplesToImage (adanerf_real_time_viewer/src/cuda/base_cuda_kernels.cu:487-528): d_raw0 [N,128] fp32, 16-byte aligned ->
+ * d_rgb [N,3] fp32 (c0, c1, c2 as (c + 0.5) / 128) and d_rgba8 [N] uchar4 (each value * 255 truncated, alpha 255); either
+ * output may be NULL.  c0, c1, c2 are the first three cells of the stable descending order that cub::BlockRadixSort gives
+ * (CUDA 12.x CUB): keys compare as the twiddled bit patterns, with -0 equal to +0, so a positive NaN ranks above +inf and
+ * a negative NaN below -inf, and equal keys keep the lower cell first.
+ * Unlike the other stage entries it takes no stream: it is an inspection entry for a raw0 the caller already has (the
+ * stream-ordered path is option "sampling_view" on the render entries).  It runs on the context's own stream, after the
+ * context's earlier calls, like the *_host entries, and returns once its outputs are written (it synchronises that
+ * stream); d_raw0 must be complete when the call is made. */
+adn_status adn_sampling_view(adn_ctx* ctx, const float* d_raw0, int64_t n_rays, float* d_rgb, uint8_t* d_rgba8);
 /* stage 3: RayMarchFromPoses.batch encode (src/features.py:458-479). d_x1 [M, P + V] fp32 (pos block first; adn_net_dims). */
 adn_status adn_stage3_encode(adn_ctx* ctx, const float* d_ray_o, const float* d_ray_d, const int32_t* d_ray,
                              const float* d_z, int64_t n_samples, float* d_x1, void* stream);

@@ -40,7 +40,8 @@ adn_status adn_multi_set_weights(adn_multi* m, int net_id, const adn_tensor_desc
  * choose for the frame (M <= B over all bands; the frame equals the single-GPU budgeted frame bit for bit).  The bands of a
  * frame are then enqueued from one host thread per device, and a device with no rows still makes its (empty) budgeted
  * call.  B < W * H, dense mode (thr == 0) and more than 2^32 - 1 candidates (W * H * (K - 1)) are refused for the whole
- * frame before any device enqueues.  0 = off. */
+ * frame before any device enqueues.  0 = off.  With "sampling_view" = 1 the frame is the sampling net's view on every band
+ * and no budget is applied (nor its checks made), as on one device. */
 adn_status adn_multi_set_option(adn_multi* m, const char* name, int64_t value);
 
 /* Row band of device `rank` for an image of H rows: rows [row0, row0 + rows), whole rows, sizes differ by at most one. */
