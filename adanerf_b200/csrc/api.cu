@@ -13,6 +13,7 @@
 
 #include "../../include/adanerf_b200.h"
 #include "export_loader.h"
+#include "flip.cuh"
 #include "mlp.cuh"
 #include "ptx.cuh"
 #include "stages.cuh"
@@ -78,7 +79,7 @@ struct adn_ctx {
   bool last_view = false;         // the last render drew the view (it counts no samples)
   bool prof_view = false;         // the profiled render drew the view (slots 2-4 unused, the view kernel in slot 5)
   // scratch
-  Buf tiles0, raw0, ray_o, ray_d, count, offset, rayidx, zbuf, zpbuf, tiles1, raw1, s2scratch, rgba, metric;
+  Buf tiles0, raw0, ray_o, ray_d, count, offset, rayidx, zbuf, zpbuf, tiles1, raw1, s2scratch, rgba, metric, flip;
   Buf dirs, rgb, nsamples;        // device side of the *_host entry points
   Buf budget_keys, budget_work, budget_thr;   // sample budget: candidate keys, histograms + select state, t*
   BudgetGroup group;              // adn_set_budget_group: the reducer that sums the selection's histograms across members
@@ -1295,6 +1296,30 @@ adn_status adn_image_metrics(adn_ctx* ctx, const float* d_image, const float* d_
   const double mse = sum / double(n_values);                       // calculate_mse, src/evaluate.py:49-50
   if (mse_out) *mse_out = mse;
   if (psnr_out) *psnr_out = 10.0 * std::log10(1.0 / mse);         // calculate_psnr, src/evaluate.py:53-54
+  return ADN_OK;
+}
+
+adn_status adn_image_flip(adn_ctx* ctx, const float* d_image, const float* d_reference, int W, int H, double pixels_per_degree,
+                          float* d_flip_map, double* mean_out) {
+  if (!ctx || !d_image || !d_reference || (!d_flip_map && !mean_out) || W < 1 || H < 1 || int64_t(W) * H > INT32_MAX)
+    return fail(ctx, ADN_ERR_INVALID, "image_flip: bad arguments");
+  if (!std::isfinite(pixels_per_degree) || !(pixels_per_degree > 0.0) || pixels_per_degree > kFlipMaxPpd)
+    return fail(ctx, ADN_ERR_INVALID, "image_flip: need 0 < pixels_per_degree <= " + std::to_string(kFlipMaxPpd));
+  FlipConsts c;
+  flip_consts(pixels_per_degree, &c);
+  ADN_CUDA(ctx, cudaSetDevice(ctx->device));
+  const cudaStream_t st = ctx->own_stream;
+  double sum = 0.0;
+  {
+    CallOrder order(ctx, st);
+    adn_status s = order.begin("image_flip");
+    if (s != ADN_OK || (s = ensure(ctx, ctx->flip, flip_scratch_bytes(W, H))) != ADN_OK) return s;
+    ADN_CUDA(ctx, launch_flip(d_image, d_reference, W, H, c, ctx->flip.p, d_flip_map, st));
+    ctx->stats.kernel_launches += 3;
+    ADN_CUDA(ctx, cudaMemcpyAsync(&sum, ctx->flip.p, sizeof(double), cudaMemcpyDeviceToHost, st));
+  }
+  ADN_CUDA(ctx, cudaStreamSynchronize(st));
+  if (mean_out) *mean_out = sum / (double(W) * double(H));
   return ADN_OK;
 }
 

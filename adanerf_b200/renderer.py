@@ -43,6 +43,10 @@ def make_scene(view_cell_center, view_cell_size, depth_range, max_depth, fov, z_
     return s
 
 
+# the observer src/evaluate.py:123-126 evaluates FLIP for: 0.7 m from a 0.7 m wide 3840-pixel screen, in pixels per degree
+EVALUATE_PPD = 0.7 * (3840 / 0.7) * (np.pi / 180)
+
+
 def _fptr(a):
     return a.ctypes.data_as(C.POINTER(C.c_float))
 
@@ -310,6 +314,30 @@ class Renderer:
             self._check(self.lib.adn_image_metrics(self.handle, a.data_ptr(), b.data_ptr(), a.numel(), int(bool(clamp01)),
                                                    C.byref(mse), C.byref(psnr), self._stream()))
         return dict(mse=mse.value, psnr=psnr.value)
+
+    def flip(self, image, reference, W, H, pixels_per_degree=EVALUATE_PPD, want_map=True):
+        """FLIP of two W x H sRGB images (adn_image_flip, src/evaluate.py:119-161): image and reference are [H*W, 3] or
+        [H, W, 3] -> dict(mean=float, map=[H, W] float32 on the device, or None when want_map is False).  Waits for the
+        current stream first: the call runs on the context's own stream and returns once its results are written.  Refused
+        while the current stream captures a CUDA graph (that wait would end the capture)."""
+        if torch.cuda.is_current_stream_capturing():
+            raise AdnError(1, "flip: the current stream is capturing a CUDA graph; the call synchronises and cannot be captured")
+        W, H = int(W), int(H)
+        if W < 1 or H < 1:
+            raise ValueError("flip: W and H must be >= 1")
+        for name, t in (("image", image), ("reference", reference)):
+            if tuple(t.shape) not in ((H * W, 3), (H, W, 3)):
+                raise ValueError(f"flip: {name} must be [H*W, 3] or [H, W, 3] with W={W}, H={H}, got {tuple(t.shape)}")
+        if tuple(image.shape) != tuple(reference.shape):
+            raise ValueError("flip: image and reference shapes differ")
+        a, b = self._f32(image), self._f32(reference)
+        fmap = torch.empty((H, W), dtype=torch.float32, device=self._dev()) if want_map else None
+        mean = C.c_double()
+        with torch.cuda.device(self.device):
+            torch.cuda.current_stream().synchronize()
+            self._check(self.lib.adn_image_flip(self.handle, a.data_ptr(), b.data_ptr(), W, H, float(pixels_per_degree),
+                                                fmap.data_ptr() if fmap is not None else None, C.byref(mean)))
+        return dict(mean=mean.value, map=fmap)
 
     def generate_ray_directions(self, W, H, row0=0, rows=None):
         rows = H - row0 if rows is None else rows

@@ -307,6 +307,18 @@ adn_status adn_stage5_composite_aux(adn_ctx* ctx, const float* d_raw1, const flo
  * clamp01 != 0 clips d_image to [0,1] first (src/evaluate.py:257-258).  Synchronises the stream; results on the host. */
 adn_status adn_image_metrics(adn_ctx* ctx, const float* d_image, const float* d_reference, int64_t n_values, int clamp01,
                              double* mse_out, double* psnr_out, void* stream);
+/* FLIP (Andersson et al., HPG 2020) of two device images, as src/evaluate.py:119-161 computes it through
+ * src/util/flip_loss.py: d_image and d_reference are W x H sRGB pixels, [H*W, 3] fp32 row-major (no alignment needed);
+ * d_flip_map [H*W] receives the per-pixel FLIP and *mean_out its mean (double accumulation, deterministic).  Either output
+ * may be NULL, not both.  pixels_per_degree is the observer's (evaluate.py uses 0.7 * 3840 / 0.7 * pi / 180 = 67.02...);
+ * it must be finite with 0 < ppd <= 200, the largest the kernels' filter radius (28 px) covers.  W, H >= 1, W * H < 2^31.
+ * Inputs are clamped to [0,1] by the metric itself; a NaN input pixel makes the map NaN within the filter radius (10 px at
+ * the default ppd) and the mean NaN, as the reference does.  The map is symmetric in the two images, bit for bit.
+ * Like adn_sampling_view it takes no stream: it runs on the context's own stream after the context's earlier calls and
+ * returns once the map is written and the mean is on the host (the inputs must be complete when the call is made).
+ * Scratch: 56 B per pixel, kept by the context. */
+adn_status adn_image_flip(adn_ctx* ctx, const float* d_image, const float* d_reference, int W, int H, double pixels_per_degree,
+                          float* d_flip_map, double* mean_out);
 
 #ifdef __cplusplus
 }
