@@ -49,7 +49,7 @@ SYMBOLS = [
     "adn_render_camera_rgba8", "adn_render_rays_host", "adn_render_camera_host", "adn_stage0_features",
     "adn_generate_ray_directions", "adn_mlp0_forward", "adn_stage2_sample", "adn_budget_threshold", "adn_stage3_encode",
     "adn_mlp1_forward", "adn_stage5_composite", "adn_stage5_composite_aux", "adn_image_metrics", "adn_sampling_view",
-    "adn_image_flip",
+    "adn_image_flip", "adn_image_iwssim",
 ]
 
 _lib = None
@@ -105,6 +105,7 @@ def load_library():
                                              C.POINTER(AuxOutputs), vp]
     lib.adn_image_metrics.argtypes = [vp, f32p, f32p, i64, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double), vp]
     lib.adn_image_flip.argtypes = [vp, f32p, f32p, C.c_int, C.c_int, C.c_double, f32p, C.POINTER(C.c_double)]
+    lib.adn_image_iwssim.argtypes = [vp, f32p, f32p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double)]
     for name in SYMBOLS:
         fn = getattr(lib, name)
         if fn.restype is C.c_int and name not in ("adn_destroy", "adn_strerror", "adn_last_error", "adn_version"):

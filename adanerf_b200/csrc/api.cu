@@ -14,6 +14,7 @@
 #include "../../include/adanerf_b200.h"
 #include "export_loader.h"
 #include "flip.cuh"
+#include "iwssim.cuh"
 #include "mlp.cuh"
 #include "ptx.cuh"
 #include "stages.cuh"
@@ -79,7 +80,7 @@ struct adn_ctx {
   bool last_view = false;         // the last render drew the view (it counts no samples)
   bool prof_view = false;         // the profiled render drew the view (slots 2-4 unused, the view kernel in slot 5)
   // scratch
-  Buf tiles0, raw0, ray_o, ray_d, count, offset, rayidx, zbuf, zpbuf, tiles1, raw1, s2scratch, rgba, metric, flip;
+  Buf tiles0, raw0, ray_o, ray_d, count, offset, rayidx, zbuf, zpbuf, tiles1, raw1, s2scratch, rgba, metric, flip, iwssim;
   Buf dirs, rgb, nsamples;        // device side of the *_host entry points
   Buf budget_keys, budget_work, budget_thr;   // sample budget: candidate keys, histograms + select state, t*
   BudgetGroup group;              // adn_set_budget_group: the reducer that sums the selection's histograms across members
@@ -1320,6 +1321,32 @@ adn_status adn_image_flip(adn_ctx* ctx, const float* d_image, const float* d_ref
   }
   ADN_CUDA(ctx, cudaStreamSynchronize(st));
   if (mean_out) *mean_out = sum / (double(W) * double(H));
+  return ADN_OK;
+}
+
+adn_status adn_image_iwssim(adn_ctx* ctx, const float* d_image, const float* d_reference, int W, int H, int layout,
+                            double* score_out, double* scale_out) {
+  if (!ctx || !d_image || !d_reference || !score_out || W < kIwMinSize || H < kIwMinSize || int64_t(W) * H > INT32_MAX)
+    return fail(ctx, ADN_ERR_INVALID, "image_iwssim: bad arguments (W, H >= " + std::to_string(kIwMinSize) + ", W * H < 2^31)");
+  if (layout != ADN_IWSSIM_GRAY && layout != ADN_IWSSIM_EVALUATE_RGB)
+    return fail(ctx, ADN_ERR_INVALID, "image_iwssim: unknown layout " + std::to_string(layout));
+  // the metric's image: H rows of W for gray planes; evaluate.py views its [H*W, 3] buffer as [W, H]
+  const IwPlan plan = layout == ADN_IWSSIM_GRAY ? iwssim_plan(H, W) : iwssim_plan(W, H);
+  ADN_CUDA(ctx, cudaSetDevice(ctx->device));
+  const cudaStream_t st = ctx->own_stream;
+  double res[1 + kIwNsc];
+  {
+    CallOrder order(ctx, st);
+    adn_status s = order.begin("image_iwssim");
+    if (s != ADN_OK || (s = ensure(ctx, ctx->iwssim, plan.bytes)) != ADN_OK) return s;
+    ADN_CUDA(ctx, launch_iwssim(d_image, d_reference, layout == ADN_IWSSIM_GRAY ? kIwGray : kIwEvaluateRgb, plan, ctx->iwssim.p, st));
+    ctx->stats.kernel_launches += 10;
+    ADN_CUDA(ctx, cudaMemcpyAsync(res, static_cast<char*>(ctx->iwssim.p) + plan.off_out, sizeof(res), cudaMemcpyDeviceToHost, st));
+  }
+  ADN_CUDA(ctx, cudaStreamSynchronize(st));
+  *score_out = res[0];
+  if (scale_out)
+    for (int k = 0; k < kIwNsc; ++k) scale_out[k] = res[1 + k];
   return ADN_OK;
 }
 

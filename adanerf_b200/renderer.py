@@ -46,6 +46,10 @@ def make_scene(view_cell_center, view_cell_size, depth_range, max_depth, fov, z_
 # the observer src/evaluate.py:123-126 evaluates FLIP for: 0.7 m from a 0.7 m wide 3840-pixel screen, in pixels per degree
 EVALUATE_PPD = 0.7 * (3840 / 0.7) * (np.pi / 180)
 
+# adn_image_iwssim's layouts (ADN_IWSSIM_EVALUATE_RGB, ADN_IWSSIM_GRAY) and its smallest frame side
+IWSSIM_LAYOUTS = {"gray": 0, "evaluate": 1}
+IWSSIM_MIN_SIZE = 161
+
 
 def _fptr(a):
     return a.ctypes.data_as(C.POINTER(C.c_float))
@@ -338,6 +342,35 @@ class Renderer:
             self._check(self.lib.adn_image_flip(self.handle, a.data_ptr(), b.data_ptr(), W, H, float(pixels_per_degree),
                                                 fmap.data_ptr() if fmap is not None else None, C.byref(mean)))
         return dict(mean=mean.value, map=fmap)
+
+    def iw_ssim(self, image, reference, W, H, layout="evaluate"):
+        """IW-SSIM of image (distorted) against reference (original) (adn_image_iwssim, src/evaluate.py:81-88) ->
+        dict(score=float, scales=[wmcs of scales 1..5]).  layout "evaluate": [H*W, 3] or [H, W, 3] fp32 as evaluate.py holds
+        its images, converted by its rgb2gray(x.view(W, H, -1)); layout "gray": [H*W] or [H, W] planes on the metric's 0-255
+        scale.  W, H >= 161.  Waits for the current stream first: the call runs on the context's own stream and returns
+        once its results are on the host.  Refused while the current stream captures a CUDA graph."""
+        W, H = int(W), int(H)
+        if layout not in IWSSIM_LAYOUTS:
+            raise ValueError(f"iw_ssim: layout must be one of {sorted(IWSSIM_LAYOUTS)}, got {layout!r}")
+        if W < IWSSIM_MIN_SIZE or H < IWSSIM_MIN_SIZE:
+            raise ValueError(f"iw_ssim: W and H must be >= {IWSSIM_MIN_SIZE}, got W={W}, H={H}")
+        shapes = ((H * W, 3), (H, W, 3)) if layout == "evaluate" else ((H * W,), (H, W))
+        for name, t in (("image", image), ("reference", reference)):
+            if tuple(t.shape) not in shapes:
+                raise ValueError(f"iw_ssim: {name} must be {' or '.join(map(str, shapes))} for layout {layout!r} with "
+                                 f"W={W}, H={H}, got {tuple(t.shape)}")
+        if tuple(image.shape) != tuple(reference.shape):
+            raise ValueError("iw_ssim: image and reference shapes differ")
+        if torch.cuda.is_current_stream_capturing():
+            raise AdnError(1, "iw_ssim: the current stream is capturing a CUDA graph; the call synchronises and cannot be "
+                              "captured")
+        a, b = self._f32(image), self._f32(reference)
+        score, scales = C.c_double(), (C.c_double * 5)()
+        with torch.cuda.device(self.device):
+            torch.cuda.current_stream().synchronize()
+            self._check(self.lib.adn_image_iwssim(self.handle, a.data_ptr(), b.data_ptr(), W, H, IWSSIM_LAYOUTS[layout],
+                                                  C.byref(score), scales))
+        return dict(score=score.value, scales=list(scales))
 
     def generate_ray_directions(self, W, H, row0=0, rows=None):
         rows = H - row0 if rows is None else rows

@@ -319,6 +319,29 @@ adn_status adn_image_metrics(adn_ctx* ctx, const float* d_image, const float* d_
  * Scratch: 56 B per pixel, kept by the context. */
 adn_status adn_image_flip(adn_ctx* ctx, const float* d_image, const float* d_reference, int W, int H, double pixels_per_degree,
                           float* d_flip_map, double* mean_out);
+/* Information-weighted multi-scale SSIM (IW-SSIM, Wang & Li 2011) of two device images, as src/evaluate.py:81-88 computes
+ * it through src/util/IW_SSIM_PyTorch.py with its defaults (5 scales, 3 x 3 neighbourhoods with the parent band,
+ * sigma_nsq 0.4, K = (0.01, 0.03), L = 255, an 11 x 11 Gaussian of sigma 1.5).  d_reference is the metric's original: its
+ * bands weight the scales and supply the parent band, so the metric is not symmetric.  Layouts:
+ *   ADN_IWSSIM_GRAY          [H*W] fp32 planes, H rows of W, used as given (the metric's constants assume values 0..255);
+ *   ADN_IWSSIM_EVALUATE_RGB  [H*W, 3] fp32 as evaluate.py holds its images: each becomes rgb2gray(x.view(W, H, -1)), that is
+ *                            round-half-even(0.2989 r + 0.5870 g + 0.1140 b) in fp32, an image of W rows of H pixels (for
+ *                            W != H a reshuffle of the frame, not its transpose).  Images in [0, 1] become 0s and 1s, as
+ *                            in evaluate.py, so scores stay close to 1.
+ * *score_out receives the score and scale_out[5] (may be NULL) wmcs of scales 1..5; the score is the product of |wmcs_s|
+ * raised to (0.0448, 0.2856, 0.3001, 0.2363, 0.1333).  Pyramid in fp64, bands rounded to fp32 once, everything after them
+ * in fp64; deterministic (a repeated call returns the same bits).
+ * W, H >= 161 (the coarsest band must hold one 11 x 11 window) and W * H < 2^31; NULL inputs or score_out, or an unknown
+ * layout, fail with ADN_ERR_INVALID before any launch.  A scale whose rebuilt covariance cannot be inverted (all its
+ * adjusted eigenvalues 0, or a zero pivot) is NaN and so is the score, with ADN_OK: an all-zero reference (every band 0,
+ * where the reference's torch.linalg.inv raises) and a NaN input pixel do this.
+ * Like adn_image_flip it takes no stream: it runs on the context's own stream after the context's earlier calls and returns
+ * with the results on the host (the inputs must be complete when the call is made).  Scratch, kept by the context: about
+ * 16 B per pixel of the metric's image for both pyramids. */
+#define ADN_IWSSIM_GRAY          0
+#define ADN_IWSSIM_EVALUATE_RGB  1
+adn_status adn_image_iwssim(adn_ctx* ctx, const float* d_image, const float* d_reference, int W, int H, int layout,
+                            double* score_out, double* scale_out);
 
 #ifdef __cplusplus
 }
