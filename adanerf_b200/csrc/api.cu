@@ -209,25 +209,39 @@ struct Seg {
 };
 
 // Packs one layer's weights W [n_out, k_in] into the ring-stage stream, in the order the MLP kernel consumes it: for each
-// 128-row N half, for each K block (Seg): a [128 x 64] K-major SWIZZLE_128B bf16 tile (hi), followed by the lo tile when
-// nsplit == 2.
-void pack_layer(const float* W, int n_out, int k_in, const std::vector<Seg>& segs, int nsplit, std::vector<uint8_t>& blob) {
+// 128-row N half, for each K block (Seg):
+//   nsplit == 1: a [128 x 64] K-major SWIZZLE_128B bf16 tile;
+//   nsplit == 2: for each pair of K steps that holds one (L.k_cnt), a [128 x 32] K-major SWIZZLE_64B tile of the hi
+//   terms followed by the same tile of the lo terms (16 KB a stage).  A K block with no K step gets no stage, e.g. the
+//   sampling net's second input block at 30 inputs; at 90 inputs it gets one.
+// layer_stages(L, nsplit) stages in all.
+void pack_layer(const float* W, int n_out, int k_in, const std::vector<Seg>& segs, int nsplit, const MlpLayer& L,
+                std::vector<uint8_t>& blob) {
   const int n_half = (n_out + 127) / 128;
+  const int cols = nsplit == 2 ? 16 * stage_k_steps(nsplit) : 64;   // K columns of one stage
+  const uint32_t half = kBlkBytes / 2;                                // one [128 x 32] tile (nsplit == 2)
   for (int nh = 0; nh < n_half; ++nh) {
-    for (const Seg& sg : segs) {
-      const size_t base = blob.size();
-      blob.resize(base + size_t(nsplit) * kBlkBytes, 0);
-      for (int n = 0; n < 128; ++n) {
-        const int row = nh * 128 + n;
-        for (int kk = 0; kk < 64; ++kk) {
-          float w = 0.0f;
-          if (row < n_out && kk < sg.valid && sg.col0 + kk < k_in) w = W[size_t(row) * k_in + sg.col0 + kk];
-          const uint16_t hi = f2bf(w);
-          const uint32_t off = sw128_offset(uint32_t(n), uint32_t(kk));
-          std::memcpy(&blob[base + off], &hi, 2);
-          if (nsplit == 2) {
-            const uint16_t lo = f2bf(w - bf2f(hi));
-            std::memcpy(&blob[base + kBlkBytes + off], &lo, 2);
+    for (size_t b = 0; b < segs.size(); ++b) {
+      const Seg& sg = segs[b];
+      const int n_st = nsplit == 2 ? (L.k_cnt[b] + stage_k_steps(nsplit) - 1) / stage_k_steps(nsplit) : 1;
+      for (int s = 0; s < n_st; ++s) {
+        const size_t base = blob.size();
+        blob.resize(base + size_t(nsplit) * (nsplit == 2 ? half : kBlkBytes), 0);
+        for (int n = 0; n < 128; ++n) {
+          const int row = nh * 128 + n;
+          for (int kk = 0; kk < cols; ++kk) {
+            const int c = s * cols + kk;   // column inside the K block
+            float w = 0.0f;
+            if (row < n_out && c < sg.valid && sg.col0 + c < k_in) w = W[size_t(row) * k_in + sg.col0 + c];
+            const uint16_t hi = f2bf(w);
+            if (nsplit == 2) {
+              const uint32_t off = sw64_offset(uint32_t(n), uint32_t(kk));
+              const uint16_t lo = f2bf(w - bf2f(hi));
+              std::memcpy(&blob[base + off], &hi, 2);
+              std::memcpy(&blob[base + half + off], &lo, 2);
+            } else {
+              std::memcpy(&blob[base + sw128_offset(uint32_t(n), uint32_t(kk))], &hi, 2);
+            }
           }
         }
       }
@@ -317,7 +331,7 @@ adn_status build_net0(adn_ctx* ctx) {
     L.n_half = uint8_t(n_out / 128);
     L.flags = last ? uint8_t(LF_FINAL_RAW) : uint8_t(LF_RELU | LF_OUT_ACT);
     L.w_off = uint32_t(wblob.size());
-    pack_layer(W->data.data(), n_out, k_in, segs, nsplit, wblob);
+    pack_layer(W->data.data(), n_out, k_in, segs, nsplit, L, wblob);
     L.bias_off = uint32_t(push_floats(fblob, B->data.data(), B->data.size()));
     if (last) {
       net.n_out = n_out;
@@ -446,7 +460,7 @@ adn_status build_net1(adn_ctx* ctx) {
     L.n_kb = uint8_t(segs.size());
     for (size_t i = 0; i < segs.size(); ++i) L.k_cnt[i] = uint8_t((segs[i].valid + 15) / 16);
     L.w_off = uint32_t(wblob.size());
-    pack_layer(Wt->data.data(), int(Wt->rows), int(Wt->cols), segs, 1, wblob);
+    pack_layer(Wt->data.data(), int(Wt->rows), int(Wt->cols), segs, 1, L, wblob);
     std::vector<float> bias(size_t(L.n_half) * 128, 0.0f);   // zero rows past the view layer's W/2 outputs
     std::copy(B->data.begin(), B->data.end(), bias.begin());
     L.bias_off = uint32_t(push_floats(fblob, bias.data(), bias.size()));

@@ -23,14 +23,17 @@ struct MlpCfg {
   // layer reads first (the sampling net's two, the shading net's one or two P blocks); the hidden activations stay in
   // registers and the inputs sit in kInSlots slots of one packed tile each.
   static constexpr int kNB = (NSPLIT == 2) ? 4 : 2;
-  static constexpr int kStageBytes = NSPLIT * kBlkBytes;              // one [128 x 64] weight block (+ its lo part)
+  // One ring stage, 16 KB either way: a [128 x 64] weight block (SWIZZLE_128B), or for the split net a [128 x 32] hi
+  // block and its lo block (SWIZZLE_64B, stage_k_steps(2) = 2 K steps).
+  static constexpr int kStageBytes = kBlkBytes;
   // As many ring stages as fit next to the inputs and the side parameters (227 KB per block): two slots of a three-block
-  // tile (P > 64 columns) take two stages' room.
-  __host__ __device__ static constexpr int stages(int n_blk) { return NSPLIT == 2 ? 2 : (n_blk > 2 ? 6 : 8); }
+  // tile (P > 64 columns) take two stages' room; the split net's 128 KB of activations leave room for five.
+  __host__ __device__ static constexpr int stages(int n_blk) { return NSPLIT == 2 ? 5 : (n_blk > 2 ? 6 : 8); }
   __host__ __device__ static constexpr size_t in_bytes(int n_blk) {
     return NSPLIT == 2 ? size_t(NSPLIT) * kNB * kBlkBytes : size_t(kInSlots) * n_blk * kBlkBytes;
   }
-  __host__ __device__ static constexpr int n_bars(int n_blk) { return 2 * stages(n_blk) + (NSPLIT == 1 ? 2 * kInSlots : 0); }
+  // full / empty per ring stage, and per input slot (NSPLIT == 1) or an input-landed barrier per consumer warpgroup
+  __host__ __device__ static constexpr int n_bars(int n_blk) { return 2 * stages(n_blk) + (NSPLIT == 1 ? 2 * kInSlots : 2); }
   __host__ __device__ static constexpr size_t smem_bytes(int n_blk) {
     return in_bytes(n_blk) + size_t(stages(n_blk)) * kStageBytes + size_t(kSideFloats) * 4 + size_t(n_bars(n_blk)) * 8 +
            1024 /*alignment slack*/;
@@ -66,19 +69,6 @@ __device__ __forceinline__ void encode_row(const EncodeParams& enc, long long i,
   }
 }
 
-// This warpgroup's 64 rows (the first or second 8 KB) of `nblk` consecutive packed blocks, global -> shared.
-__device__ __forceinline__ void copy_rows(const uint8_t* __restrict__ src, uint32_t dst, int nblk, int wg, int tw) {
-  for (int b = 0; b < nblk; ++b) {
-    const uint4* s = reinterpret_cast<const uint4*>(src + size_t(b) * kBlkBytes + size_t(wg) * (kBlkBytes / 2));
-    const uint32_t d = dst + uint32_t(b) * kBlkBytes + uint32_t(wg) * (kBlkBytes / 2);
-    uint4 v[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) v[j] = __ldg(s + tw + 128 * j);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) st_shared_v4(d + uint32_t(tw + 128 * j) * 16u, v[j].x, v[j].y, v[j].z, v[j].w);
-  }
-}
-
 template <int NSPLIT, bool ENC>
 __global__ void __launch_bounds__(kMlpThreads, 1)
 mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ wblob, const uint8_t* __restrict__ in_tiles,
@@ -89,6 +79,7 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
   constexpr int NB = Cfg::kNB;
   const int STAGES = Cfg::stages(prog.in.n_blk);   // a constant for NSPLIT == 2
   constexpr int STAGE_BYTES = Cfg::kStageBytes;
+  constexpr int STAGE_K = stage_k_steps(NSPLIT);   // K steps per ring stage
   constexpr int kConsumerWarps = 8, kProducerWarp = 8;
   constexpr int kEncThreads = 96;   // ENC: producer warps 9-11 encode the inputs
   // The launch gives every thread 168 registers (__launch_bounds__(384, 1)); setmaxnreg only moves them between
@@ -107,7 +98,8 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
   float* side = reinterpret_cast<float*>(ring + size_t(STAGES) * STAGE_BYTES);
   uint64_t* w_full = reinterpret_cast<uint64_t*>(side + kSideFloats);   // [STAGES] the stage has landed
   uint64_t* w_empty = w_full + STAGES;                                   // [STAGES] every consumer warp's MMAs on it retired
-  uint64_t* in_full = w_empty + STAGES;                                  // NSPLIT == 1, [kInSlots]: the slot holds its tile
+  // NSPLIT == 1, [kInSlots]: the slot holds its tile.  NSPLIT == 2, [2]: consumer warpgroup wg's rows of the tile landed
+  uint64_t* in_full = w_empty + STAGES;
   uint64_t* in_empty = in_full + kInSlots;                               // [kInSlots] every consumer warp is done with it
 
   const int warp = __shfl_sync(0xffffffffu, int(threadIdx.x >> 5), 0);
@@ -127,6 +119,8 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
         mbar_init(&in_full[s], ENC ? kEncThreads : 1);
         mbar_init(&in_empty[s], kConsumerWarps);
       }
+    } else {
+      for (int g = 0; g < 2; ++g) mbar_init(&in_full[g], 1);
     }
     mbar_fence_init();
   }
@@ -166,15 +160,15 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
       return;
     }
     // -------------------------------------------------------------------- weight producer
-    // Stage i of a layer is [128 N rows x 64 K] (hi, then lo when NSPLIT == 2), N half outermost: the order the
-    // consumers walk them in.  It never waits on an input slot.
+    // Stage i of a layer is [128 N rows x 64 K], or [128 x 32] hi then lo when NSPLIT == 2 (pack_layer), N half
+    // outermost: the order the consumers walk them in.  It never waits on an input slot.
     if (warp == kProducerWarp && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) {
         for (int l = 0; l < prog.n_layers; ++l) {
           const MlpLayer& L = prog.layers[l];
-          const int n_st = int(L.n_kb) * int(L.n_half);
+          const int n_st = layer_stages(L, NSPLIT);
           for (int i = 0; i < n_st; ++i) {
             mbar_wait(&w_empty[stage], phase ^ 1, err_flag, 1);
             mbar_arrive_expect_tx(&w_full[stage], STAGE_BYTES);
@@ -204,6 +198,8 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
   auto blk_addr = [&](int term, int blk) -> uint32_t { return in_s + uint32_t(term * NB + blk) * kBlkBytes; };
   const uint64_t desc_hi = make_desc_sw128(0) & ~uint64_t(0x3FFF);
   auto desc = [&](uint32_t addr) -> uint64_t { return desc_hi | uint64_t((addr & 0x3FFFF) >> 4); };
+  const uint64_t desc64_hi = make_desc_sw64(0) & ~uint64_t(0x3FFF);   // the split net's weight stages
+  auto desc64 = [&](uint32_t addr) -> uint64_t { return desc64_hi | uint64_t((addr & 0x3FFFF) >> 4); };
 
   // Shading net: the bf16 output of the last LF_OUT_ACT layer as register-A fragments, [K block][K step][register]
   // (hidden column 64 kb + 16 k + ...).  Indexed with compile-time constants only, so it stays in registers.
@@ -224,14 +220,14 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
   int stage = 0;
   uint32_t phase = 0;
   int prev = -1;   // ring stage whose MMAs may still be running
-  // One K block = one ring stage: wait for it, issue up to 4 K steps through mma(k, B stage address, accumulate), and hand
-  // the previous stage back to the producer once its MMAs have retired.
+  // One ring stage: wait for it, issue up to STAGE_K K steps through mma(k, B stage address, accumulate), and hand the
+  // previous stage back to the producer once its MMAs have retired.
   auto k_block = [&](bool first, int nk, auto mma) {
     mbar_wait(&w_full[stage], phase, err_flag, 2);
     wgmma_fence();
     const uint32_t b = ring_s + uint32_t(stage) * STAGE_BYTES;
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
+    for (int k = 0; k < STAGE_K; ++k) {
       if (k < nk) mma(k, b, (first && k == 0) ? 0u : 1u);   // zero-padded tail columns of an input block are not multiplied
     }
     wgmma_commit();
@@ -244,16 +240,24 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
     }
   };
 
+  // NSPLIT == 2: one thread of the warpgroup bulk-copies the warpgroup's 64 rows of tile tt's input blocks (8 KB of each
+  // block of each term) into its rows of activation blocks 0 .. in_nblk0 - 1 of both terms, completing on in_full[wg].
+  auto fetch_input = [&](long long tt) {
+    if (tw != 0) return;
+    const uint8_t* src = in_tiles + size_t(tt) * prog.in.tile_bytes() + wg_off;
+    mbar_arrive_expect_tx(&in_full[wg], uint32_t(NSPLIT * prog.in_nblk0) * (kBlkBytes / 2));
+    for (int term = 0; term < NSPLIT; ++term)
+      for (int b = 0; b < prog.in_nblk0; ++b)
+        bulk_g2s(act + size_t(term * NB + b) * kBlkBytes + wg_off, src + prog.in.blk_off(term, b), kBlkBytes / 2, &in_full[wg]);
+  };
+  if (NSPLIT == 2 && blockIdx.x < n_tiles) fetch_input(blockIdx.x);
+
   int in_slot = 0;
   uint32_t in_phase = 0;
   for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) {
     if constexpr (NSPLIT == 2) {
-      // tile input (the previous tile's last MMAs retired before its epilogue: the blocks are free)
-#pragma unroll
-      for (int term = 0; term < NSPLIT; ++term)
-        copy_rows(in_tiles + size_t(t) * prog.in.tile_bytes() + prog.in.blk_off(term, 0), blk_addr(term, 0), prog.in_nblk0, wg, tw);
-      fence_proxy_async_smem();
-      named_bar_sync(bar_id, 128);
+      mbar_wait(&in_full[wg], in_phase, err_flag, 4);   // this warpgroup's rows of the tile's inputs have landed
+      in_phase ^= 1;
     } else {
       mbar_wait(&in_full[in_slot], in_phase, err_flag, 4);   // the producer has filled this tile's slot
       in_s = act_s + uint32_t(in_slot) * prog.in.tile_bytes();
@@ -267,15 +271,18 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
       for (int nh = 0; nh < 2; ++nh) {
         if (nh >= L.n_half) break;
         if (NSPLIT == 2) {
+          // K block kb in stages of STAGE_K K steps, [128 x 32] hi then lo (SWIZZLE_64B); K steps past k_cnt have none
           for (int kb = 0; kb < L.n_kb; ++kb) {
-            const uint32_t a_hi = blk_addr(0, kb) + wg_off;
-            const uint32_t a_lo = a_hi + uint32_t(NB) * kBlkBytes;
-            k_block(kb == 0, L.k_cnt[kb], [&](int k, uint32_t b_hi, uint32_t accumulate) {
-              const uint32_t b_lo = b_hi + uint32_t(kBlkBytes);
-              wgmma_m64n128_bf16(acc[nh], desc(a_hi + 32 * k), desc(b_hi + 32 * k), accumulate);
-              wgmma_m64n128_bf16(acc[nh], desc(a_lo + 32 * k), desc(b_hi + 32 * k), 1u);
-              wgmma_m64n128_bf16(acc[nh], desc(a_hi + 32 * k), desc(b_lo + 32 * k), 1u);
-            });
+            for (int k0 = 0; k0 < L.k_cnt[kb]; k0 += STAGE_K) {
+              const uint32_t a_hi = blk_addr(0, kb) + wg_off + 32 * k0;
+              const uint32_t a_lo = a_hi + uint32_t(NB) * kBlkBytes;
+              k_block(kb == 0 && k0 == 0, L.k_cnt[kb] - k0, [&](int k, uint32_t b_hi, uint32_t accumulate) {
+                const uint32_t b_lo = b_hi + uint32_t(kBlkBytes / 2);
+                wgmma_m64n128_bf16(acc[nh], desc(a_hi + 32 * k), desc64(b_hi + 32 * k), accumulate);
+                wgmma_m64n128_bf16(acc[nh], desc(a_lo + 32 * k), desc64(b_hi + 32 * k), 1u);
+                wgmma_m64n128_bf16(acc[nh], desc(a_hi + 32 * k), desc64(b_lo + 32 * k), 1u);
+              });
+            }
           }
         } else {
           auto from_smem = [&](int blk) {
@@ -302,9 +309,18 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
       wgmma_wait<0>();
       if (lane == 0) mbar_arrive(&w_empty[prev]);
       prev = -1;
+      // NSPLIT == 2: the tile's last layer fetches the next tile's inputs, before its epilogue when that writes no
+      // activations (the sampling net's LF_FINAL_RAW layer), else after it
+      const bool fetch_next = l + 1 == prog.n_layers && t + gridDim.x < n_tiles;
+      const bool fetch_early = fetch_next && !(L.flags & LF_OUT_ACT);
       if constexpr (NSPLIT == 2) {
         // all of the warpgroup's MMAs retired: the A blocks in shared memory may be overwritten in place
         named_bar_sync(bar_id, 128);
+        // The bulk copy (async proxy) overwrites this warpgroup's rows of the input blocks.  The wgmma reads of them (async
+        // proxy) retired: wait_group 0 in every warp, then the barrier.  The generic-proxy stores of earlier epilogues
+        // that wrote them were each followed by fence.proxy.async and the barrier after that epilogue, so they are
+        // ordered before the copy.  This layer's epilogue writes only global memory and registers.
+        if (fetch_early) fetch_input(t + gridDim.x);
       } else {
         // the tile's last MMAs retired: its slot goes back to the input producer
         if (l + 1 == prog.n_layers && lane == 0) mbar_arrive(&in_empty[in_slot]);
@@ -396,6 +412,7 @@ mlp_kernel(const __grid_constant__ MlpProgram prog, const uint8_t* __restrict__ 
       if constexpr (NSPLIT == 2) {
         fence_proxy_async_smem();        // generic-proxy stores -> visible to the next layer's wgmma reads
         named_bar_sync(bar_id, 128);
+        if (fetch_next && !fetch_early) fetch_input(t + gridDim.x);   // its activation stores are fenced: as above
       }
     }
     if (NSPLIT == 1 && ++in_slot == kInSlots) {

@@ -2,7 +2,8 @@
 //
 // One persistent CTA per SM walks 128-row tiles of the batch through ALL layers of the network:
 //   * weights stream layer by layer from L2 into a shared-memory ring with 1-D bulk async copies
-//     (TMA engine), pre-packed on the host as K-major SWIZZLE_128B tiles in consumption order,
+//     (TMA engine), pre-packed on the host as K-major SWIZZLE_128B tiles (the split net: [128 x 32] SWIZZLE_64B hi + lo
+//     tiles) in consumption order,
 //   * activations never leave the SM: two consumer warpgroups each own 64 rows of the tile, accumulate
 //     a layer in registers (wgmma m64n128k16, one 64-register accumulator per 128-column N half), add
 //     bias / ReLU, round to bf16 and keep the result as the next layer's A operand: in registers for plain
@@ -46,7 +47,7 @@ enum : uint8_t {
 // split-precision sampling net (NSPLIT == 2) keeps them as activation blocks 0 .. n_hid - 1, which each epilogue
 // overwrites in place, so there K block kb reads activation block kb.
 struct MlpLayer {
-  uint32_t w_off;     // byte offset of this layer's packed weight stages (N half outermost, then K block)
+  uint32_t w_off;     // byte offset of this layer's packed weight stages (N half outermost, then K block; layer_stages)
   uint32_t bias_off;  // float offset of the fp32 bias vector in MlpProgram::side
   uint8_t n_kb;       // number of 64-wide K blocks
   uint8_t in_first, n_hid, in_last;   // 0-2, 0 or W / 64, 0 / 1
@@ -56,6 +57,20 @@ struct MlpLayer {
   // padding, e.g. 90 input features -> blocks of 4 and 2 steps; 30 features -> 2 and 0).
   uint8_t k_cnt[6];
 };
+
+// 16-wide K steps per weight ring stage: a [128 x 64] block for plain bf16; for the split net a [128 x 32] hi block and
+// its lo block (SWIZZLE_64B), so that its ring holds more, smaller stages next to its activation blocks.
+__host__ __device__ constexpr int stage_k_steps(int nsplit) { return nsplit == 2 ? 2 : 4; }
+
+// Ring stages of layer L, one per N half and K block's group of stage_k_steps K steps that holds a K step (a K block
+// with k_cnt 0 has none; with nsplit == 1 every K block has a stage).  pack_layer packs this many, the kernel's weight
+// producer streams and its consumers take this many.
+__host__ __device__ inline int layer_stages(const MlpLayer& L, int nsplit) {
+  if (nsplit == 1) return int(L.n_kb) * int(L.n_half);
+  int s = 0;
+  for (int kb = 0; kb < L.n_kb; ++kb) s += (L.k_cnt[kb] + stage_k_steps(nsplit) - 1) / stage_k_steps(nsplit);
+  return s * int(L.n_half);
+}
 
 struct MlpProgram {
   int32_t n_layers;

@@ -185,10 +185,28 @@ __device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr_bytes) {
   return d;
 }
 
+// The same descriptor for the 64-byte swizzle: rows are 64 B (32 elements) apart, groups of 8 rows 512 B apart (SBO), the
+// 16-byte chunk index is XORed with (row % 8) / 2.  Tile base 512-byte aligned; a K step of 16 elements advances the
+// start address by 32 bytes.  Layout type (bits [62,64)) 2 = SWIZZLE_64B.
+__device__ __forceinline__ uint64_t make_desc_sw64(uint32_t smem_addr_bytes) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr_bytes & 0x3FFFF) >> 4);
+  d |= static_cast<uint64_t>(1) << 16;
+  d |= static_cast<uint64_t>(512 >> 4) << 32;
+  d |= static_cast<uint64_t>(2) << 62;
+  return d;
+}
+
 // Byte offset of element (row, col) inside one [rows x 64] bf16 K-major SWIZZLE_128B block.
 __host__ __device__ __forceinline__ uint32_t sw128_offset(uint32_t row, uint32_t col) {
   const uint32_t chunk = (col >> 3) ^ (row & 7);
   return (row >> 3) * 1024u + (row & 7) * 128u + chunk * 16u + (col & 7) * 2u;
+}
+
+// Byte offset of element (row, col) inside one [rows x 32] bf16 K-major SWIZZLE_64B block.
+__host__ __device__ __forceinline__ uint32_t sw64_offset(uint32_t row, uint32_t col) {
+  const uint32_t chunk = (col >> 3) ^ ((row >> 1) & 3);
+  return (row >> 3) * 512u + (row & 7) * 64u + chunk * 16u + (col & 7) * 2u;
 }
 
 }  // namespace adn
