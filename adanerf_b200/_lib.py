@@ -49,7 +49,7 @@ SYMBOLS = [
     "adn_render_camera_rgba8", "adn_render_rays_host", "adn_render_camera_host", "adn_stage0_features",
     "adn_generate_ray_directions", "adn_mlp0_forward", "adn_stage2_sample", "adn_budget_threshold", "adn_stage3_encode",
     "adn_mlp1_forward", "adn_stage5_composite", "adn_stage5_composite_aux", "adn_image_metrics", "adn_sampling_view",
-    "adn_image_flip", "adn_image_iwssim",
+    "adn_image_flip", "adn_image_iwssim", "adn_pdf_sample", "adn_stage5_density_composite",
 ]
 
 _lib = None
@@ -98,6 +98,8 @@ def load_library():
     lib.adn_stage2_sample.argtypes = [vp, f32p, i64, C.c_float, C.c_int, i32p, i32p, i32p, i32p, f32p, f32p, vp, vp]
     lib.adn_budget_threshold.argtypes = [vp, f32p, i64, C.c_float, C.c_int, i64, f32p, vp]
     lib.adn_sampling_view.argtypes = [vp, f32p, i64, f32p, vp]
+    lib.adn_pdf_sample.argtypes = [vp, f32p, i64, C.c_int, C.c_int, i32p, i32p, i32p, f32p]
+    lib.adn_stage5_density_composite.argtypes = [vp, f32p, f32p, f32p, i64, C.c_int, f32p, vp, C.POINTER(AuxOutputs)]
     lib.adn_stage3_encode.argtypes = [vp, f32p, f32p, i32p, f32p, i64, f32p, vp]
     lib.adn_mlp1_forward.argtypes = [vp, f32p, i64, f32p, vp]
     lib.adn_stage5_composite.argtypes = [vp, f32p, f32p, f32p, i32p, i32p, i64, C.c_int, f32p, f32p, f32p, vp]

@@ -8,11 +8,16 @@ existing TrainConfig).  Only the entries those callers read are produced:
     outs[-1][:, :3]                          rgb                                (evaluate.py:228)
     dicts[-1]["AdaptiveSamplePositions"]     samples per ray / K                 (evaluate.py:223-224)
     dicts[1]["OracleWeights"]                raw sampling-net output, thr == 0   (evaluate.py:279-280)
+
+With rayMarchSampler FromClassifiedDepth (sampler=1, the DONeRF baseline) the reference's shading-net dict has neither
+AdaptiveSamplePositions (the feature set is not adaptive, features.py:561-563) nor OracleWeights (its losses[0] is the
+sampler's transform loss, not NeRFWeightMultiplicationLoss, features.py:503-504), and neither has this one's.
     dicts[i]["PostProcessedNetworkOutput"]   = outs[i]                           (util/helper.py:79-130)
 
 The batch keys are the reference's DatasetKeyConstants (src/datasets.py:24-38)."""
 import torch
 
+from .onnx_weights import PDF_TRANSFORMS
 from .renderer import Renderer
 
 # src/datasets.py:29-35 and src/features.py:20-40
@@ -28,11 +33,18 @@ class B200Inference:
     FeatureSet.initialize reads from DatasetInfo (src/features.py:343-360, :747-767)."""
 
     def __init__(self, scene, sampling_net, shading_net, threshold, num_samples, device=0, want_oracle_weights=None,
-                 want_aux=False):
+                 want_aux=False, sampler=0, pdf_transform=1):
+        """sampler / pdf_transform: the renderer options of the same names (0 = the adaptive sampler; 1 = FromClassifiedDepth
+        with transform 1 = sigmoid or 2 = softmax; threshold is then not used)."""
         self.renderer = Renderer(scene, device=device, sampling_net=sampling_net, shading_net=shading_net)
         self.threshold = float(threshold)
         self.K = int(num_samples)
-        self.want_oracle_weights = (self.threshold == 0.0) if want_oracle_weights is None else bool(want_oracle_weights)
+        self.sampler = int(sampler)
+        if self.sampler:
+            self.renderer.set_option("sampler", self.sampler)
+            self.renderer.set_option("pdf_transform", int(pdf_transform))
+        default_ow = self.threshold == 0.0 and not self.sampler
+        self.want_oracle_weights = default_ow if want_oracle_weights is None else bool(want_oracle_weights)
         # plots.render_all_imgs / the depth export read NeRFWeightsOutput, NeRFAlphaOutput, NeRFOutputDepth (src/plots.py:272-306)
         self.want_aux = bool(want_aux)
 
@@ -54,13 +66,27 @@ class B200Inference:
             if hasattr(f, "enc_type"):
                 p, d = (-1, -1) if f.enc_type == "none" else (int(f.n_freq_pos), int(f.n_freq_dir))
                 scene.update({kp: p if p > 0 else min(p, zero), kd: d if d > 0 else min(d, zero)})
-        return scene, [train_config.models[0], train_config.models[1]], float(f1.z_sampler.threshold), int(f1.n_ray_samples)
+        thr = float(getattr(f1.z_sampler, "threshold", 0.0))   # FromClassifiedDepth has none
+        return scene, [train_config.models[0], train_config.models[1]], thr, int(f1.n_ray_samples)
+
+    @staticmethod
+    def sampler_from_train_config(train_config):
+        """(sampler, pdf_transform) of the shading net's rayMarchSampler and losses[0] (src/nerf_raymarch_common.py:625-637):
+        (1, 1 or 2) for FromClassifiedDepth, else (0, 1): the adaptive path.  Raises ValueError for a FromClassifiedDepth run
+        whose losses[0] selects no transform."""
+        if type(train_config.f_in[1].z_sampler).__name__ != "FromClassifiedDepth":
+            return 0, 1
+        loss0 = train_config.config_file.losses[0]
+        if loss0 not in PDF_TRANSFORMS:
+            raise ValueError(f"FromClassifiedDepth with losses[0] = {loss0} applies no transform to raw0 (not supported)")
+        return 1, PDF_TRANSFORMS[loss0]
 
     @classmethod
     def from_train_config(cls, train_config, device=0):
         """Builds the renderer from an initialised reference TrainConfig (models, feature sets, dataset_info)."""
         scene, models, thr, k = cls.args_from_train_config(train_config)
-        return cls(scene, models[0], models[1], thr, k, device=device)
+        sampler, transform = cls.sampler_from_train_config(train_config)
+        return cls(scene, models[0], models[1], thr, k, device=device, sampler=sampler, pdf_transform=transform)
 
     def inference(self, batch_idx, gradient=False, **kwargs):
         if gradient:
@@ -76,9 +102,9 @@ class B200Inference:
         raw0 = out["oracle_weights"]
         d0 = {KEY_POST: raw0, KEY_NET_OUT: raw0}
         d1 = {KEY_POST: rgb}
-        if self.threshold > 0.0:
+        if self.threshold > 0.0 and not self.sampler:
             d1[KEY_ASP] = out["n_samples"].to(torch.float32) / self.K
-        if raw0 is not None:
+        if raw0 is not None and not self.sampler:
             d1[KEY_ORACLE] = raw0
         if self.want_aux:
             d1[KEY_WEIGHTS], d1[KEY_ALPHA], d1[KEY_ZVALS] = out["weights"], out["alpha"], out["z_vals"]

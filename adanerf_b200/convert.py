@@ -9,7 +9,7 @@ without instantiating the reference's classes, so trained checkpoints run throug
 
     python -m adanerf_b200.convert --weights0 Net0_opt.weights --weights1 Net1_opt.weights \
         --dataset-info dataset_info.txt --threshold 0.2 --samples 8 --out export_dir \
-        [--pos-enc nerf,nerf --pos-enc-args 10-4,10-4]
+        [--pos-enc nerf,nerf --pos-enc-args 10-4,10-4] [--sampler FromClassifiedDepth --sampling-loss BCEWithLogitsLoss]
 
 The run's posEnc / posEncArgs (sampling net, shading net) go on the command line: the sampling net's split into position
 and direction bands cannot be read from the width of layers.0.
@@ -20,7 +20,7 @@ from collections import OrderedDict
 
 import torch
 
-from .onnx_weights import net_shapes, write_export_dir
+from .onnx_weights import PDF_TRANSFORMS, net_shapes, write_export_dir
 from .renderer import enc_columns
 
 SAMPLING_KEYS = ("layers.0.weight", "layers.0.bias")
@@ -146,15 +146,17 @@ def read_dataset_info(path):
     return {k: vals[k] for k in need}
 
 
-def weights_to_export_dir(weights0, weights1, out_dir, scene, threshold, num_samples, allow_pickle=False, encoding=None):
-    """encoding: parse_encoding's band counts; None keeps the scene's (posEncArgs [10-4, 10-4] unless it says otherwise)."""
+def weights_to_export_dir(weights0, weights1, out_dir, scene, threshold, num_samples, allow_pickle=False, encoding=None,
+                          sampler="FromClassifiedDepthAdaptive", sampling_loss="BCEWithLogitsLoss"):
+    """encoding: parse_encoding's band counts; None keeps the scene's (posEncArgs [10-4, 10-4] unless it says otherwise).
+    sampler / sampling_loss: rayMarchSampler and losses[0] of the run (onnx_weights.write_export_dir)."""
     sd0, sd1 = load_weights_file(weights0, allow_pickle), load_weights_file(weights1, allow_pickle)
     if encoding is not None:
         (p0, d0), (p, d) = encoding
         # the sampling net's 0 means "the shading net's count" in the scene: zero bands are -1 there
         scene = dict(scene, n_freq_pos=p, n_freq_dir=d, n_freq_pos0=p0 if p0 > 0 else -1, n_freq_dir0=d0 if d0 > 0 else -1)
     check_state_dicts(sd0, sd1, encoding)
-    write_export_dir(out_dir, scene, sd0, sd1, float(threshold), int(num_samples))
+    write_export_dir(out_dir, scene, sd0, sd1, float(threshold), int(num_samples), sampler=sampler, sampling_loss=sampling_loss)
     return sd0, sd1
 
 
@@ -170,13 +172,17 @@ def main(argv=None):
                     help="also read checkpoints that hold a pickled nn.Module (executes code from the file: trusted files only)")
     ap.add_argument("--pos-enc", default=None, help="posEnc of the run, sampling net then shading net: nerf,nerf (default) or none")
     ap.add_argument("--pos-enc-args", default=None, help="posEncArgs of the run, e.g. 10-4,10-4 (default) or 16-4,6-2")
+    ap.add_argument("--sampler", default="FromClassifiedDepthAdaptive", choices=("FromClassifiedDepthAdaptive", "FromClassifiedDepth"),
+                    help="rayMarchSampler of the shading net: the adaptive sampler (default) or DONeRF's fixed-K FromClassifiedDepth")
+    ap.add_argument("--sampling-loss", default="BCEWithLogitsLoss", choices=tuple(PDF_TRANSFORMS),
+                    help="losses[0] of a FromClassifiedDepth run: sigmoid (BCEWithLogitsLoss) or softmax (the CrossEntropy losses)")
     a = ap.parse_args(argv)
     encoding = None
     if a.pos_enc is not None or a.pos_enc_args is not None:
         split = lambda v, d: tuple(x.strip() for x in (v or d).strip("[]").split(","))
         encoding = parse_encoding(split(a.pos_enc, "nerf,nerf"), split(a.pos_enc_args, "10-4,10-4"))
     weights_to_export_dir(a.weights0, a.weights1, a.out, read_dataset_info(a.dataset_info), a.threshold, a.samples, a.allow_pickle,
-                          encoding)
+                          encoding, sampler=a.sampler, sampling_loss=a.sampling_loss)
     print(f"wrote {a.out}")
 
 

@@ -79,6 +79,8 @@ struct adn_ctx {
   bool sampling_view = false;     // adn_set_option "sampling_view": renders draw the sampling net's view (stages 0-1 + view)
   bool last_view = false;         // the last render drew the view (it counts no samples)
   bool prof_view = false;         // the profiled render drew the view (slots 2-4 unused, the view kernel in slot 5)
+  int sampler = 0;                // adn_set_option "sampler": 0 = FromClassifiedDepthAdaptive, 1 = FromClassifiedDepth (fixed K)
+  int pdf_transform = kPdfSigmoid;   // adn_set_option "pdf_transform": what FromClassifiedDepth applies to raw0 first
   // scratch
   Buf tiles0, raw0, ray_o, ray_d, count, offset, rayidx, zbuf, zpbuf, tiles1, raw1, s2scratch, rgba, metric, flip, iwssim;
   Buf dirs, rgb, nsamples;        // device side of the *_host entry points
@@ -596,6 +598,9 @@ Stage5Aux stage5_aux(const adn_ctx* ctx, const adn_aux_outputs& a) {
           sc.depth_range[0], float(std::log(double(sc.depth_range[1]) - double(sc.depth_range[0]) + 1.0))};
 }
 
+// depth_range[1] - depth_range[0] + 1 in double: the base of LogTransform.to_world (the z tables and the fixed-K sampler).
+double depth_base(const adn_ctx* ctx) { return double(ctx->scene.depth_range[1]) - double(ctx->scene.depth_range[0]) + 1.0; }
+
 // Stage 0 + the sampling MLP of one chunk, stream ordered.  Writes the chunk's raw0 [n, 128] (the caller's
 // d_oracle_weights when given, else the context's scratch from ray w on) and its ray origins / directions (scratch from ray
 // w on).  w is 0 unless a sample budget keeps the whole call's rows.  timing: record ev[0..2].
@@ -622,7 +627,8 @@ adn_status run_stages_0_1(adn_ctx* ctx, const RenderCall& c, int64_t w, bool tim
 adn_status run_stages_2_5(adn_ctx* ctx, const RenderCall& c, int64_t w, const float* d_thr, bool timing) {
   const int64_t n = c.n_rays;
   const int K = c.K;
-  const bool dense = (c.thr == 0.0f);
+  const bool fixed_k = ctx->sampler == 1;   // FromClassifiedDepth: the inverse-CDF sampler and the density composite
+  const bool dense = !fixed_k && c.thr == 0.0f;
   const int64_t cap = n * K;
   adn_status s;
   if ((s = ensure(ctx, ctx->count, size_t(n) * 4)) != ADN_OK) return s;
@@ -630,6 +636,8 @@ adn_status run_stages_2_5(adn_ctx* ctx, const RenderCall& c, int64_t w, const fl
   if (!dense) {
     if ((s = ensure(ctx, ctx->rayidx, size_t(cap) * 4)) != ADN_OK) return s;
     if ((s = ensure(ctx, ctx->zbuf, size_t(cap) * 4)) != ADN_OK) return s;
+  }
+  if (!dense && !fixed_k) {
     if ((s = ensure(ctx, ctx->zpbuf, size_t(cap) * 4)) != ADN_OK) return s;
     if ((s = ensure(ctx, ctx->s2scratch, stage2_scratch_bytes(n))) != ADN_OK) return s;
   }
@@ -651,7 +659,10 @@ adn_status run_stages_2_5(adn_ctx* ctx, const RenderCall& c, int64_t w, const fl
   long long* total = ctx->total.as<long long>();
 
   // stage 2
-  if (dense) {
+  if (fixed_k) {
+    ADN_CUDA(ctx, launch_pdf_sample(raw0, n, K, ctx->pdf_transform, depth_base(ctx), ctx->scene.depth_range[0], count, offset,
+                                    rayidx, z, total, c.st));
+  } else if (dense) {
     ADN_CUDA(ctx, launch_stage2_dense(n, K, count, offset, total, c.st));
   } else {
     ADN_CUDA(ctx, launch_stage2(raw0, n, c.thr, K, ctx->zlut.as<float>(), count, offset, nullptr, rayidx, z,
@@ -672,7 +683,7 @@ adn_status run_stages_2_5(adn_ctx* ctx, const RenderCall& c, int64_t w, const fl
   if (timing) cudaEventRecord(ctx->ev[5], c.st);
   // stage 5
   ADN_CUDA(ctx, launch_stage5(raw1, dense ? raw0 : ctx->zpbuf.as<float>(), z, ctx->zlut_dense.as<float>(), offset, count, n, K,
-                              dense ? 1 : 0, c.d_rgb, c.d_rgba8, stage5_aux(ctx, c.aux), c.st));
+                              dense ? 1 : 0, c.d_rgb, c.d_rgba8, stage5_aux(ctx, c.aux), c.st, fixed_k ? ray_d : nullptr));
   ctx->stats.kernel_launches++;
   if (timing) cudaEventRecord(ctx->ev[6], c.st);
   return ADN_OK;
@@ -703,8 +714,10 @@ adn_status render(adn_ctx* ctx, const RenderCall& call) {
   if (!ctx->net[0].ready || !ctx->net[1].ready) return fail(ctx, ADN_ERR_NO_WEIGHTS, "render: set both networks first");
   if (ctx->net[0].n_in != ctx->n_feat0 || ctx->net[0].n_out != 128)
     return fail(ctx, ADN_ERR_INVALID, "render: sampling net must be " + std::to_string(ctx->n_feat0) + " -> 128 for this scene's encoding");
-  if (K < 1 || K > 128 || thr < 0.0f) return fail(ctx, ADN_ERR_INVALID, "render: need 1 <= K <= 128 and thr >= 0");
-  if (thr == 0.0f && K != 128) return fail(ctx, ADN_ERR_INVALID, "render: dense mode (thr == 0) needs K == 128 (one sample per depth cell)");
+  const bool fixed_k = ctx->sampler == 1;   // FromClassifiedDepth ignores thr
+  if (K < 1 || K > 128 || (!fixed_k && thr < 0.0f)) return fail(ctx, ADN_ERR_INVALID, "render: need 1 <= K <= 128 and thr >= 0");
+  if (!fixed_k && thr == 0.0f && K != 128)
+    return fail(ctx, ADN_ERR_INVALID, "render: dense mode (thr == 0) needs K == 128 (one sample per depth cell)");
   const bool view = ctx->sampling_view;
   if (view) {
     const adn_aux_outputs& a = call.aux;
@@ -714,6 +727,10 @@ adn_status render(adn_ctx* ctx, const RenderCall& call) {
       return fail(ctx, ADN_ERR_INVALID, "render: option sampling_view needs 16-byte aligned d_oracle_weights rows");
   }
   const int64_t budget = view ? 0 : ctx->sample_budget;   // the view selects no samples
+  if (fixed_k && budget > 0)
+    return fail(ctx, ADN_ERR_INVALID, "render: sampler 1 (FromClassifiedDepth) places K samples on every ray; it takes no sample_budget");
+  if (fixed_k && ctx->scene.use_ndc)
+    return fail(ctx, ADN_ERR_INVALID, "render: sampler 1 (FromClassifiedDepth) is not supported on NDC scenes");
   if (budget > 0 && thr == 0.0f)
     return fail(ctx, ADN_ERR_INVALID, "render: sample_budget needs the adaptive path (thr > 0 is the floor threshold), not dense mode");
   if (budget > 0 && budget < n_rays)
@@ -732,7 +749,7 @@ adn_status render(adn_ctx* ctx, const RenderCall& call) {
   }
   ADN_CUDA(ctx, cudaSetDevice(ctx->device));
   adn_status s;
-  if (thr == 0.0f && (s = ensure_dense_lut(ctx, K)) != ADN_OK) return s;
+  if (!fixed_k && thr == 0.0f && (s = ensure_dense_lut(ctx, K)) != ADN_OK) return s;
   int64_t chunk = ctx->chunk_rays;
   if (chunk <= 0) {
     chunk = (int64_t(8) << 20) / K;     // ~8 Mi samples of scratch per chunk
@@ -972,6 +989,18 @@ adn_status adn_set_option(adn_ctx* ctx, const char* name, int64_t value) {
     ctx->sampling_view = value != 0;
     return ADN_OK;
   }
+  if (n == "sampler") {   // 0 (default): FromClassifiedDepthAdaptive; 1: FromClassifiedDepth (DONeRF's fixed K samples per ray)
+    if (value != 0 && value != 1) return fail(ctx, ADN_ERR_INVALID, "sampler must be 0 (adaptive) or 1 (FromClassifiedDepth)");
+    ctx->sampler = int(value);
+    return ADN_OK;
+  }
+  if (n == "pdf_transform") {   // FromClassifiedDepth's transform of raw0: 1 (default) sigmoid, 2 softmax
+    if (value != kPdfSigmoid && value != kPdfSoftmax)
+      return fail(ctx, ADN_ERR_INVALID, "pdf_transform must be 1 (sigmoid, BCEWithLogitsLoss) or 2 (softmax, CrossEntropyLoss); "
+                                        "0 (no transform) is not supported");
+    ctx->pdf_transform = int(value);
+    return ADN_OK;
+  }
   if (n == "fuse_encoder") {   // 1 (default): positional encoding inside the shading kernel (no tile buffer); 0: stage3_kernel + packed tiles
     ctx->fuse_encoder = value != 0;
     return ADN_OK;
@@ -1199,6 +1228,27 @@ adn_status adn_stage2_sample(adn_ctx* ctx, const float* d_raw0, int64_t n_rays, 
   return ADN_OK;
 }
 
+adn_status adn_pdf_sample(adn_ctx* ctx, const float* d_raw0, int64_t n_rays, int K, int transform, int32_t* d_count,
+                          int32_t* d_offset, int32_t* d_ray, float* d_z) {
+  if (!ctx || n_rays < 0 || K < 1 || K > 128 || (n_rays > 0 && (!d_raw0 || !d_z)))
+    return fail(ctx, ADN_ERR_INVALID, "pdf_sample: bad arguments (need 1 <= K <= 128, d_raw0 and d_z)");
+  if (transform != kPdfSigmoid && transform != kPdfSoftmax)
+    return fail(ctx, ADN_ERR_INVALID, "pdf_sample: transform must be 1 (sigmoid) or 2 (softmax)");
+  if (n_rays * K > INT32_MAX) return fail(ctx, ADN_ERR_INVALID, "pdf_sample: N * K must stay below 2^31 (int32 offsets)");
+  if (n_rays == 0) return ADN_OK;
+  ADN_CUDA(ctx, cudaSetDevice(ctx->device));
+  const cudaStream_t st = ctx->own_stream;
+  {
+    CallOrder order(ctx, st);
+    if (adn_status s = order.begin("pdf_sample"); s != ADN_OK) return s;
+    ADN_CUDA(ctx, launch_pdf_sample(d_raw0, n_rays, K, transform, depth_base(ctx), ctx->scene.depth_range[0], d_count, d_offset,
+                                    d_ray, d_z, nullptr, st));
+    ctx->stats.kernel_launches++;
+  }
+  ADN_CUDA(ctx, cudaStreamSynchronize(st));
+  return ADN_OK;
+}
+
 adn_status adn_sampling_view(adn_ctx* ctx, const float* d_raw0, int64_t n_rays, float* d_rgb, uint8_t* d_rgba8) {
   if (!ctx || n_rays < 0 || (n_rays > 0 && (!d_raw0 || (!d_rgb && !d_rgba8))))
     return fail(ctx, ADN_ERR_INVALID, "sampling_view: bad arguments");
@@ -1280,6 +1330,24 @@ adn_status adn_stage5_composite_aux(adn_ctx* ctx, const float* d_raw1, const flo
   ADN_CUDA(ctx, launch_stage5(d_raw1, d_zp, dense ? nullptr : d_z, ctx->zlut_dense.as<float>(), dense ? nullptr : d_offset,
                               d_count, n_rays, K, dense, d_rgb, d_rgba8, stage5_aux(ctx, a), static_cast<cudaStream_t>(stream)));
   ctx->stats.kernel_launches++;
+  return ADN_OK;
+}
+
+adn_status adn_stage5_density_composite(adn_ctx* ctx, const float* d_raw1, const float* d_z, const float* d_ray_d, int64_t n_rays,
+                                        int K, float* d_rgb, uint8_t* d_rgba8, const adn_aux_outputs* aux) {
+  if (!ctx || n_rays < 0 || K < 1 || K > 128 || (n_rays > 0 && (!d_raw1 || !d_z || !d_ray_d)))
+    return fail(ctx, ADN_ERR_INVALID, "stage5_density: bad arguments (need 1 <= K <= 128, d_raw1, d_z and d_ray_d)");
+  if (n_rays == 0) return ADN_OK;
+  ADN_CUDA(ctx, cudaSetDevice(ctx->device));
+  const cudaStream_t st = ctx->own_stream;
+  {
+    CallOrder order(ctx, st);
+    if (adn_status s = order.begin("stage5_density"); s != ADN_OK) return s;
+    ADN_CUDA(ctx, launch_stage5(d_raw1, nullptr, d_z, nullptr, nullptr, nullptr, n_rays, K, 0, d_rgb, d_rgba8,
+                                stage5_aux(ctx, aux ? *aux : adn_aux_outputs{}), st, d_ray_d));
+    ctx->stats.kernel_launches++;
+  }
+  ADN_CUDA(ctx, cudaStreamSynchronize(st));
   return ADN_OK;
 }
 
@@ -1403,6 +1471,12 @@ adn_status adn_create_from_export_dir(adn_ctx** out, const char* dir, int device
       adn_destroy(ctx);
       return s;
     }
+  }
+  if (ex.sampler == 1 && ((s = adn_set_option(ctx, "sampler", 1)) != ADN_OK ||
+                          (s = adn_set_option(ctx, "pdf_transform", ex.pdf_transform)) != ADN_OK)) {
+    std::fprintf(stderr, "adanerf_b200: %s\n", ctx->last_error.c_str());
+    adn_destroy(ctx);
+    return s;
   }
   if (thr_out) *thr_out = ex.threshold;
   if (k_out) *k_out = ex.num_samples;

@@ -258,7 +258,31 @@ bool load_export_dir(const std::string& dir_in, ExportDir& out, std::string& err
     const auto items = list_items(it->second);
     return items.empty() || items.back() == want;
   };
-  if (s.use_ndc) {
+  auto sm = cfg.find("rayMarchSampler");
+  const auto sitems = sm == cfg.end() ? std::vector<std::string>{} : list_items(sm->second);
+  if (!sitems.empty() && sitems.back() == "FromClassifiedDepth") {
+    // FromClassifiedDepth (the DONeRF sampler, src/nerf_raymarch_common.py:606-660) returns z only, so the composite is
+    // nerf_raw2outputs without OracleWeights and accumulationMult does not apply; its transform of raw0 is chosen by
+    // losses[0] (:625-637)
+    if (s.use_ndc || !check("rayMarchNormalization", "InverseSqrtDistCentered") || !check("depthTransform", "log")) {
+      err = "config.ini: FromClassifiedDepth exports must use InverseSqrtDistCentered / log and no NDC";
+      return false;
+    }
+    auto lo = cfg.find("losses");
+    const auto litems = lo == cfg.end() ? std::vector<std::string>{} : list_items(lo->second);
+    const std::string loss0 = litems.empty() ? std::string("") : litems.front();
+    if (loss0 == "BCEWithLogitsLoss") {
+      out.pdf_transform = 1;
+    } else if (loss0 == "CrossEntropyLoss" || loss0 == "CrossEntropyLossWeighted") {
+      out.pdf_transform = 2;
+    } else {
+      err = "config.ini: FromClassifiedDepth with losses[0] = " + (loss0.empty() ? std::string("(missing)") : loss0) +
+            " applies no transform to the sampling net's output (pdf_transform 0), which is not supported; "
+            "BCEWithLogitsLoss (sigmoid) and CrossEntropyLoss / CrossEntropyLossWeighted (softmax) are";
+      return false;
+    }
+    out.sampler = 1;
+  } else if (s.use_ndc) {
     if (!check("rayMarchSampler", "FromClassifiedDepthAdaptiveNoDepthRange") || !check("rayMarchNormalization", "None") ||
         !check("accumulationMult", "alpha")) {
       err = "config.ini: NDC exports must use FromClassifiedDepthAdaptiveNoDepthRange / rayMarchNormalization None / alpha";

@@ -21,6 +21,8 @@ struct ExportDir {
   adn_scene scene{};
   float threshold = 0.0f;  // adaptiveSamplingThreshold
   int num_samples = 0;     // numRaymarchSamples[1]
+  int sampler = 0;         // rayMarchSampler[1]: 0 = FromClassifiedDepthAdaptive(NoDepthRange), 1 = FromClassifiedDepth
+  int pdf_transform = 0;   // sampler 1: 1 = sigmoid, 2 = softmax (from losses[0])
   std::vector<NamedTensor> nets[2];
 };
 

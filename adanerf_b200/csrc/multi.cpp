@@ -129,6 +129,14 @@ adn_status adn_multi_create_from_export_dir(adn_multi** out, const char* dir, co
       return s;
     }
   }
+  // a FromClassifiedDepth export: every band renders with the fixed-K sampler and the export's transform
+  if (ex.sampler == 1 && ((s = adn_multi_set_option(*out, "sampler", 1)) != ADN_OK ||
+                          (s = adn_multi_set_option(*out, "pdf_transform", ex.pdf_transform)) != ADN_OK)) {
+    std::fprintf(stderr, "adanerf_b200: %s\n", (*out)->err.c_str());
+    adn_multi_destroy(*out);
+    *out = nullptr;
+    return s;
+  }
   if (thr_out) *thr_out = ex.threshold;
   if (k_out) *k_out = ex.num_samples;
   return ADN_OK;

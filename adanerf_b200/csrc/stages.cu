@@ -1158,35 +1158,58 @@ __device__ __forceinline__ void s5_write_ray_aux(const Stage5Aux& aux, long long
   }
 }
 
-// One thread per ray, samples visited in order: the same sequential cumprod / sum order as torch.
+// alpha of nerf_raw2outputs (src/nerf_raymarch_common.py:35-46): dist = (z1 - z0, or 1e10 for the last sample) * |rays_d|,
+// 1 - exp(-relu(a) * dist).  torch.relu keeps a NaN, fmaxf would not.
+__device__ __forceinline__ float nerf_alpha(float a, float z0, float z1, bool last, float norm) {
+  const float dist = __fmul_rn(last ? 1e10f : __fsub_rn(z1, z0), norm);
+  const float ra = isnan(a) ? a : fmaxf(a, 0.0f);
+  return __fsub_rn(1.0f, expf(__fmul_rn(-ra, dist)));
+}
+
+// torch.norm(rays_d[r], dim=-1) in fp32 (the density composite); 0 when there is no ray_d (the adaptive composite).
+__device__ __forceinline__ float ray_norm(const float* __restrict__ ray_d, long long r) {
+  if (!ray_d) return 0.0f;
+  const float x = __ldg(ray_d + 3 * r), y = __ldg(ray_d + 3 * r + 1), z = __ldg(ray_d + 3 * r + 2);
+  return __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)), __fmul_rn(z, z)));
+}
+
+// One thread per ray, samples visited in order: the same sequential cumprod / sum order as torch.  NERF: the density
+// composite over K samples at offset r K (launch_stage5).
+template <bool NERF>
 __global__ void __launch_bounds__(128)
 stage5_thread_kernel(const float4* __restrict__ raw1, const float* __restrict__ zp, const float* __restrict__ z,
                      const int32_t* __restrict__ offset, const int32_t* __restrict__ count, long long n_rays, int K,
-                     float* __restrict__ rgb, uint32_t* __restrict__ rgba8, const Stage5Aux aux) {
+                     float* __restrict__ rgb, uint32_t* __restrict__ rgba8, const Stage5Aux aux, const float* __restrict__ ray_d) {
   const long long r = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (r >= n_rays) return;
-  const long long off = offset[r];
-  const int n = count[r];
-  const bool want_z = aux.depth_map || aux.disp_map || aux.depth_est || aux.z_vals;
+  constexpr bool nerf = NERF;
+  const long long off = nerf ? r * K : (long long)offset[r];
+  const int n = nerf ? K : count[r];
+  const float norm = ray_norm(ray_d, r);
+  const bool want_z = nerf || aux.depth_map || aux.disp_map || aux.depth_est || aux.z_vals;
   float T = 1.0f, cr = 0.0f, cg = 0.0f, cb = 0.0f, dm = 0.0f, acc = 0.0f;
   for (int j0 = 0; j0 < n; j0 += 4) {
     // four samples' loads are issued before the (sequential) transmittance chain consumes them
     float4 q4[4];
-    float zp4[4], z4[4];
+    float zp4[4], z4[4], zn4[4];
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
       const bool live = j0 + u < n;
       q4[u] = live ? __ldg(raw1 + off + j0 + u) : make_float4(0.f, 0.f, 0.f, 0.f);
-      zp4[u] = live ? __ldg(zp + off + j0 + u) : 0.0f;
+      zp4[u] = (live && !nerf) ? __ldg(zp + off + j0 + u) : 0.0f;
       z4[u] = (live && want_z) ? __ldg(z + off + j0 + u) : 0.0f;
+      zn4[u] = (nerf && j0 + u + 1 < n) ? __ldg(z + off + j0 + u + 1) : 0.0f;
     }
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
       const int j = j0 + u;
       if (j >= n) break;
       const float4 q = q4[u];
-      const float sr = sigmoidf_acc(q.x), sg = sigmoidf_acc(q.y), sb = sigmoidf_acc(q.z), sa = sigmoidf_acc(q.w);
-      const float alpha = __fmul_rn(sa, zp4[u]);                                    // :123-125
+      const float sr = sigmoidf_acc(q.x), sg = sigmoidf_acc(q.y), sb = sigmoidf_acc(q.z);
+      // K == 1: nerf_raw2outputs' dists is [N, 0] (the 1e10 column is expanded to the shape of an empty slice, :36-37), so
+      // its alpha and weights are empty and the ray composites to nothing
+      const float alpha = nerf ? (n == 1 ? 0.0f : nerf_alpha(q.w, z4[u], zn4[u], j + 1 == n, norm))
+                               : __fmul_rn(sigmoidf_acc(q.w), zp4[u]);              // :123-125
       const float w = __fmul_rn(alpha, T);                                          // :128-129
       T = __fmul_rn(T, __fadd_rn(__fsub_rn(1.0f, alpha), 1e-10f));
       cr = __fadd_rn(cr, __fmul_rn(w, sr));                                         // :135
@@ -1195,7 +1218,7 @@ stage5_thread_kernel(const float4* __restrict__ raw1, const float* __restrict__ 
       acc = __fadd_rn(acc, w);                                                      // :139
       if (want_z) {
         dm = __fadd_rn(dm, __fmul_rn(w, z4[u]));                                    // :137
-        if (aux.z_vals) aux.z_vals[r * K + j] = s5_z_val(z4[u]);
+        if (aux.z_vals) aux.z_vals[r * K + j] = nerf ? z4[u] : s5_z_val(z4[u]);
       }
       if (aux.weights) aux.weights[r * K + j] = w;
       if (aux.alpha) aux.alpha[r * K + j] = alpha;
@@ -1216,18 +1239,21 @@ stage5_thread_kernel(const float4* __restrict__ raw1, const float* __restrict__ 
 }
 
 // One warp per ray (dense 128 samples / large K): lanes own consecutive samples, transmittance by a
-// warp-wide product scan with a running carry.
+// warp-wide product scan with a running carry.  NERF: the density composite (launch_stage5).
+template <bool NERF>
 __global__ void __launch_bounds__(256)
 stage5_warp_kernel(const float4* __restrict__ raw1, const float* __restrict__ zp, const float* __restrict__ z,
                    const float* __restrict__ zlut_dense, const int32_t* __restrict__ offset,
                    const int32_t* __restrict__ count, long long n_rays, int K, int dense, float* __restrict__ rgb,
-                   uint32_t* __restrict__ rgba8, const Stage5Aux aux) {
+                   uint32_t* __restrict__ rgba8, const Stage5Aux aux, const float* __restrict__ ray_d) {
   const long long r = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (r >= n_rays) return;
-  const long long off = dense ? r * K : (long long)offset[r];
-  const int n = dense ? K : count[r];
-  const bool want_z = aux.depth_map || aux.disp_map || aux.depth_est || aux.z_vals;
+  constexpr bool nerf = NERF;
+  const long long off = (dense || nerf) ? r * K : (long long)offset[r];
+  const int n = (dense || nerf) ? K : count[r];
+  const float norm = ray_norm(ray_d, r);
+  const bool want_z = nerf || aux.depth_map || aux.disp_map || aux.depth_est || aux.z_vals;
   float carry = 1.0f, cr = 0.0f, cg = 0.0f, cb = 0.0f, dm = 0.0f, acc = 0.0f;
   for (int j0 = 0; j0 < n; j0 += 32) {
     const int j = j0 + lane;
@@ -1237,8 +1263,14 @@ stage5_warp_kernel(const float4* __restrict__ raw1, const float* __restrict__ zp
       sr = sigmoidf_acc(q.x);
       sg = sigmoidf_acc(q.y);
       sb = sigmoidf_acc(q.z);
-      alpha = __fmul_rn(sigmoidf_acc(q.w), __ldg(zp + off + j));
-      if (want_z) zz = dense ? __ldg(zlut_dense + j) : __ldg(z + off + j);
+      if (nerf) {
+        zz = __ldg(z + off + j);
+        const float zn = j + 1 < n ? __ldg(z + off + j + 1) : 0.0f;
+        alpha = nerf_alpha(q.w, zz, zn, j + 1 == n, norm);
+      } else {
+        alpha = __fmul_rn(sigmoidf_acc(q.w), __ldg(zp + off + j));
+        if (want_z) zz = dense ? __ldg(zlut_dense + j) : __ldg(z + off + j);
+      }
     }
     float f = __fadd_rn(__fsub_rn(1.0f, alpha), 1e-10f);
     // inclusive product scan
@@ -1262,7 +1294,7 @@ stage5_warp_kernel(const float4* __restrict__ raw1, const float* __restrict__ zp
       const bool live = j < n;
       if (aux.weights) aux.weights[r * K + j] = live ? w : 0.0f;
       if (aux.alpha) aux.alpha[r * K + j] = live ? alpha : 0.0f;
-      if (aux.z_vals) aux.z_vals[r * K + j] = !live ? __int_as_float(0x7fc00000) : dense ? zz : s5_z_val(zz);
+      if (aux.z_vals) aux.z_vals[r * K + j] = !live ? __int_as_float(0x7fc00000) : (dense || nerf) ? zz : s5_z_val(zz);
     }
   }
   for (int j = ((n + 31) & ~31) + lane; j < K; j += 32) {
@@ -1291,18 +1323,141 @@ stage5_warp_kernel(const float4* __restrict__ raw1, const float* __restrict__ zp
 
 cudaError_t launch_stage5(const float* d_raw1, const float* d_zp, const float* d_z, const float* d_zlut_dense,
                           const int32_t* d_offset, const int32_t* d_count, long long n_rays, int K, int dense, float* d_rgb,
-                          uint8_t* d_rgba8, const Stage5Aux& aux, cudaStream_t s) {
+                          uint8_t* d_rgba8, const Stage5Aux& aux, cudaStream_t s, const float* d_ray_d) {
   if (n_rays <= 0) return cudaSuccess;
   const float4* raw = reinterpret_cast<const float4*>(d_raw1);
   uint32_t* rgba = reinterpret_cast<uint32_t*>(d_rgba8);
-  if (dense || K > 32) {
-    const long long threads = n_rays * 32;
-    stage5_warp_kernel<<<unsigned((threads + 255) / 256), 256, 0, s>>>(raw, d_zp, d_z, d_zlut_dense, d_offset, d_count, n_rays,
-                                                                        K, dense, d_rgb, rgba, aux);
+  const long long threads = n_rays * 32;
+  const unsigned warp_blocks = unsigned((threads + 255) / 256), thread_blocks = unsigned((n_rays + 127) / 128);
+  if (d_ray_d && K > 32) {
+    stage5_warp_kernel<true><<<warp_blocks, 256, 0, s>>>(raw, nullptr, d_z, nullptr, nullptr, nullptr, n_rays, K, 0, d_rgb, rgba,
+                                                         aux, d_ray_d);
+  } else if (d_ray_d) {
+    stage5_thread_kernel<true><<<thread_blocks, 128, 0, s>>>(raw, nullptr, d_z, nullptr, nullptr, n_rays, K, d_rgb, rgba, aux,
+                                                             d_ray_d);
+  } else if (dense || K > 32) {
+    stage5_warp_kernel<false><<<warp_blocks, 256, 0, s>>>(raw, d_zp, d_z, d_zlut_dense, d_offset, d_count, n_rays, K, dense,
+                                                          d_rgb, rgba, aux, nullptr);
   } else {
-    stage5_thread_kernel<<<unsigned((n_rays + 127) / 128), 128, 0, s>>>(raw, d_zp, d_z, d_offset, d_count, n_rays, K, d_rgb,
-                                                                         rgba, aux);
+    stage5_thread_kernel<false><<<thread_blocks, 128, 0, s>>>(raw, d_zp, d_z, d_offset, d_count, n_rays, K, d_rgb, rgba, aux,
+                                                              nullptr);
   }
+  return cudaGetLastError();
+}
+
+// ------------------------------------------------------------------------------------- fixed-K sampler
+// FromClassifiedDepth.generate (src/nerf_raymarch_common.py:606-660): nerf_sample_pdf(mids, w, K + 2, det=True) (:160-192)
+// on mids = linspace(0, 1, 129), samples 1..K kept, then LogTransform.to_world.  One warp per ray, lane l owns cells
+// 4l..4l+3 (one 16-byte load):
+//   * w = transform(raw0) + 1e-5 and pdf = w / sum(w).  The sum is taken in double and rounded once; torch.sum's fp32
+//     order (and the softmax denominator's) is ATen's own, so pdf can differ from the reference's in the last bit;
+//   * cdf = [0, cumsum(pdf)]: ATen's CPU cumsum of fp32 accumulates in double, so the warp scans in double and rounds each
+//     entry once (the association differs, the double sums almost never round differently); staged in shared memory;
+//   * u_j = linspace(0, 1, K + 2)[j] as ATen's CPU kernel forms it: step j below the half, fma(-step, K + 1 - j, 1) above;
+//   * lane t takes j = 1 + t, 33 + t, ... <= K: searchsorted(cdf, u, right=True) by binary search over the staged cdf,
+//     then the interpolation in the reference's separate fp32 operations, then to_world as the z table does it (pow in
+//     double, the rest in fp32).  Stores are coalesced (consecutive j, consecutive lanes).
+constexpr int kPdfWarps = 8;
+constexpr int kPdfStride = 132;   // one warp's staged cdf (129 entries)
+
+__device__ __forceinline__ float linspace01(int j, int steps) {
+  const float step = __fdiv_rn(1.0f, float(steps - 1));
+  return j < steps / 2 ? __fmul_rn(step, float(j)) : __fmaf_rn(-step, float(steps - 1 - j), 1.0f);
+}
+
+__device__ __forceinline__ double warp_sum_f64(double v) {
+#pragma unroll
+  for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+__global__ void __launch_bounds__(32 * kPdfWarps)
+pdf_sample_kernel(const float* __restrict__ raw0, long long n_rays, int K, int transform, double wbase, float dr_min,
+                  bool aligned16, int32_t* __restrict__ count, int32_t* __restrict__ offset, int32_t* __restrict__ ray,
+                  float* __restrict__ zout, long long* __restrict__ total) {
+  __shared__ float s_cdf[kPdfWarps][kPdfStride];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long long r = blockIdx.x * (long long)kPdfWarps + warp;
+  if (r == 0 && lane == 0 && total) *total = n_rays * K;
+  if (r >= n_rays) return;
+  const float4 v4 = ld_row_quad(raw0 + r * 128, lane, aligned16);
+  float w[4] = {v4.x, v4.y, v4.z, v4.w};
+  if (transform == kPdfSoftmax) {   // softmax(dim=-1): exp(x - max) * (1 / sum)
+    float m = fmaxf(fmaxf(w[0], w[1]), fmaxf(w[2], w[3]));
+#pragma unroll
+    for (int o = 16; o; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    double se = 0.0;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      w[k] = expf(__fsub_rn(w[k], m));
+      se += w[k];
+    }
+    const float inv = __fdiv_rn(1.0f, float(warp_sum_f64(se)));   // ATen's vectorised softmax scales by the reciprocal
+#pragma unroll
+    for (int k = 0; k < 4; ++k) w[k] = __fmul_rn(w[k], inv);
+  } else {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) w[k] = sigmoidf_acc(w[k]);
+  }
+  double sw = 0.0;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    w[k] = __fadd_rn(w[k], 1e-5f);                                               // :162
+    sw += w[k];
+  }
+  const float wsum = float(warp_sum_f64(sw));                                      // :163
+  double a[4], run = 0.0;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    run += double(__fdiv_rn(w[k], wsum));
+    a[k] = run;
+  }
+  double inc = run;                                                                // :164 (inclusive warp scan)
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const double y = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += y;
+  }
+  double excl = __shfl_up_sync(0xffffffffu, inc, 1);
+  if (lane == 0) excl = 0.0;
+  float* cdf = s_cdf[warp];
+  if (lane == 0) cdf[0] = 0.0f;                                                    // :165
+#pragma unroll
+  for (int k = 0; k < 4; ++k) cdf[4 * lane + k + 1] = float(excl + a[k]);
+  __syncwarp();
+  const int steps = K + 2;
+  for (int j = 1 + lane; j <= K; j += 32) {
+    const float u = linspace01(j, steps);                                          // :169
+    int lo = 0, hi = 129;                                                          // :177 first cdf entry > u (right=True)
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (cdf[mid] > u) hi = mid;
+      else lo = mid + 1;
+    }
+    const int below = max(0, lo - 1), above = min(128, lo);                       // :178-179
+    const float c0 = cdf[below], c1 = cdf[above];
+    const float b0 = linspace01(below, 129), b1 = linspace01(above, 129);
+    float denom = __fsub_rn(c1, c0);                                               // :188-189
+    if (denom < 1e-5f) denom = 1.0f;
+    const float t = __fdiv_rn(__fsub_rn(u, c0), denom);                            // :190-191
+    const float zs = __fadd_rn(b0, __fmul_rn(t, __fsub_rn(b1, b0)));
+    const float zw = __fadd_rn(__fsub_rn(float(pow(wbase, double(zs))), 1.0f), dr_min);   // depth_transformations.py:44-46
+    const long long o = r * K + (j - 1);
+    zout[o] = zw;
+    if (ray) ray[o] = int32_t(r);
+  }
+  if (lane == 0) {
+    if (count) count[r] = K;
+    if (offset) offset[r] = int32_t(r * K);
+  }
+}
+
+cudaError_t launch_pdf_sample(const float* d_raw0, long long n_rays, int K, int transform, double wbase, float dr_min,
+                              int32_t* d_count, int32_t* d_offset, int32_t* d_ray, float* d_z, long long* d_total, cudaStream_t s) {
+  const long long n = n_rays > 0 ? n_rays : 1;   // an empty call still writes *d_total = 0
+  const bool aligned16 = (reinterpret_cast<uintptr_t>(d_raw0) & 15u) == 0;
+  pdf_sample_kernel<<<unsigned((n + kPdfWarps - 1) / kPdfWarps), 32 * kPdfWarps, 0, s>>>(
+      d_raw0, n_rays, K, transform, wbase, dr_min, aligned16, d_count, d_offset, d_ray, d_z, d_total);
   return cudaGetLastError();
 }
 

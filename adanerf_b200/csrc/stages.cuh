@@ -72,6 +72,15 @@ cudaError_t launch_budget_threshold(const float* d_raw0, long long n_rays, float
 cudaError_t launch_stage2_dense(long long n_rays, int K, int32_t* d_count, int32_t* d_offset, long long* d_total,
                                 cudaStream_t s);
 
+// Fixed-K sampler (rayMarchSampler FromClassifiedDepth, the DONeRF baseline): per ray the inverse CDF of the transformed
+// raw0 [n_rays, 128] at K + 2 evenly spaced u, the first and last dropped, warped to world depth.  transform: 1 = sigmoid,
+// 2 = softmax.  Writes count = K, offset = r K, ray [N K] = r, z [N K] (ascending per ray) and *d_total = N K; any of
+// d_count, d_offset, d_ray, d_total may be null (not written).  wbase = depth_range[1] - depth_range[0] + 1 (double),
+// dr_min = depth_range[0]: LogTransform.to_world as the z table of the adaptive path computes it.
+constexpr int kPdfSigmoid = 1, kPdfSoftmax = 2;
+cudaError_t launch_pdf_sample(const float* d_raw0, long long n_rays, int K, int transform, double wbase, float dr_min,
+                              int32_t* d_count, int32_t* d_offset, int32_t* d_ray, float* d_z, long long* d_total, cudaStream_t s);
+
 // The sampling network's view (the viewer's render-oracle mode): raw0 [n_rays, 128] (16-byte aligned) -> per ray the three
 // cells that lead raw0's stable descending radix order, as (c + 0.5) / 128 into d_rgb [n_rays, 3] and as uchar4 pixels
 // (value * 255 truncated, alpha 255) into d_rgba8 [n_rays]; either output may be null.
@@ -101,9 +110,12 @@ struct Stage5Aux {
 };
 
 // Stage 5.  zp: adaptive -> packed [M]; dense (dense_zp_stride > 0) -> raw0 [N, stride].
+// d_ray_d non-null: the density composite of the fixed-K sampler (nerf_raw2outputs, src/nerf_raymarch_common.py:19-68)
+// over K samples per ray at offset r K: alpha = 1 - exp(-relu(a) dist), dist = (z[k+1] - z[k], last 1e10) * |ray_d [N,3]|;
+// d_zp, d_offset, d_count and dense are not read, and z_vals is z unchanged.
 cudaError_t launch_stage5(const float* d_raw1, const float* d_zp, const float* d_z, const float* d_zlut_dense,
                           const int32_t* d_offset, const int32_t* d_count, long long n_rays, int K, int dense,
-                          float* d_rgb, uint8_t* d_rgba8, const Stage5Aux& aux, cudaStream_t s);
+                          float* d_rgb, uint8_t* d_rgba8, const Stage5Aux& aux, cudaStream_t s, const float* d_ray_d = nullptr);
 
 // Linear RGBA8 pixels [rows * W] -> surf2Dwrite(uchar4, surface, 4 x, row0 + y) (adaptive_cuda_kernels.cu:846-851).
 cudaError_t launch_rgba_to_surface(const uint8_t* d_rgba8, int W, int row0, int rows, unsigned long long surface, cudaStream_t s);

@@ -178,10 +178,40 @@ def _enc_entries(scene):
     return f"[{e0}, {e1}]", f"[{a0}, {a1}]"
 
 
-def write_export_dir(path, scene, sd0, sd1, thr, K):
+# losses[0] of a FromClassifiedDepth run -> the transform its sampler applies to raw0 (src/nerf_raymarch_common.py:625-637),
+# as option "pdf_transform" numbers it
+PDF_TRANSFORMS = {"BCEWithLogitsLoss": 1, "CrossEntropyLoss": 2, "CrossEntropyLossWeighted": 2}
+
+
+def export_sampler(path):
+    """(sampler, pdf_transform) of an export directory's config.ini, as adn_create_from_export_dir sets options "sampler" and
+    "pdf_transform": (0, None) for the adaptive samplers, (1, 1 or 2) for FromClassifiedDepth.  Raises ValueError for a
+    FromClassifiedDepth run whose losses[0] selects no transform."""
+    import os
+    cfg = {}
+    with open(os.path.join(path, "config.ini")) as f:
+        for line in f:
+            if "=" in line and not line.lstrip().startswith(("#", ";")):
+                k, v = line.split("=", 1)
+                cfg[k.strip()] = [x.strip() for x in v.strip().strip("[]").split(",")]
+    if cfg.get("rayMarchSampler", [""])[-1] != "FromClassifiedDepth":
+        return 0, None
+    loss0 = cfg.get("losses", [""])[0]
+    if loss0 not in PDF_TRANSFORMS:
+        raise ValueError(f"{path}: FromClassifiedDepth with losses[0] = {loss0 or '(missing)'} applies no transform (not supported)")
+    return 1, PDF_TRANSFORMS[loss0]
+
+
+def write_export_dir(path, scene, sd0, sd1, thr, K, sampler="FromClassifiedDepthAdaptive", sampling_loss="BCEWithLogitsLoss"):
     """Writes {config.ini, dataset_info.txt, model0.onnx, model1.onnx} in the reference's export format
     (src/export.py:28-93, src/train_data.py:180-195), config.ini with the networks' layers / layerWidth / skips and the
-    scene's posEnc / posEncArgs."""
+    scene's posEnc / posEncArgs.  sampler: rayMarchSampler of the shading net, FromClassifiedDepthAdaptive or
+    FromClassifiedDepth (not with NDC); for FromClassifiedDepth, sampling_loss is losses[0], which picks the transform of
+    the sampling net's output (PDF_TRANSFORMS)."""
+    if sampler not in ("FromClassifiedDepthAdaptive", "FromClassifiedDepth"):
+        raise ValueError(f"write_export_dir: sampler {sampler!r} is not FromClassifiedDepthAdaptive or FromClassifiedDepth")
+    if sampler == "FromClassifiedDepth" and (scene.get("use_ndc") or sampling_loss not in PDF_TRANSFORMS):
+        raise ValueError("write_export_dir: FromClassifiedDepth needs a non-NDC scene and losses[0] in " + ", ".join(PDF_TRANSFORMS))
     import os
     os.makedirs(path, exist_ok=True)
     (d0, w0, _), (d1, w1, skip) = net_shapes(sd0, sd1)
@@ -207,8 +237,10 @@ def write_export_dir(path, scene, sd0, sd1, thr, K):
                     f"adaptiveSamplingThreshold = {thr}\nmultiDepthFeatures = [128, 128]\naccumulationMult = alpha\n")
         else:
             f.write("inFeatures = [SpherePosDir, RayMarchFromPoses]\n"
-                    "outFeatures = [RawSigmoid, RGBARayMarch]\nrayMarchSampler = [none, FromClassifiedDepthAdaptive]\n"
+                    f"outFeatures = [RawSigmoid, RGBARayMarch]\nrayMarchSampler = [none, {sampler}]\n"
                     "rayMarchNormalization = [InverseSqrtDistCentered, InverseSqrtDistCentered]\n"
                     f"numRaymarchSamples = [{K}, {K}]\ndepthTransform = log\nzNear = [0.001, 0.001]\nzFar = [1.0, 1.0]\n"
                     f"adaptiveSamplingThreshold = {thr}\nmultiDepthFeatures = [128, 128]\naccumulationMult = alpha\n")
+            if sampler == "FromClassifiedDepth":
+                f.write(f"losses = [{sampling_loss}, MSE]\n")
         f.write(f"activation = [relu, nerf]\nlayers = [{d0}, {d1}]\nlayerWidth = [{w0}, {w1}]\nskips = [, {_skips_entry(d1, skip)}]\n")

@@ -88,7 +88,9 @@ class Renderer:
 
     @classmethod
     def from_export_dir(cls, path, device=0):
-        """Loads the reference's export directory (src/export.py:28-93). Returns (renderer, thr, K)."""
+        """Loads the reference's export directory (src/export.py:28-93). Returns (renderer, thr, K).  A FromClassifiedDepth
+        export comes back with options "sampler" = 1 and its "pdf_transform" set (export_sampler reads them from
+        config.ini); its thr is not used."""
         lib = _lib.load_library()
         h, thr, k = C.c_void_p(), C.c_float(), C.c_int()
         st = lib.adn_create_from_export_dir(C.byref(h), str(path).encode(), int(device), C.byref(thr), C.byref(k))
@@ -415,6 +417,46 @@ class Renderer:
                                                self._stream()))
         m = int(total.item())
         return dict(count=count, offset=offset, cell=cell[:m], ray=ray[:m], z=z[:m], zp=zp[:m], total=m)
+
+    def pdf_sample(self, raw0, K, transform=1):
+        """FromClassifiedDepth's sample placement alone (adn_pdf_sample): raw0 [N,128] -> dict(count [N], offset [N],
+        ray [N K] int32, z [N K] float32 world depth).  transform: 1 = sigmoid, 2 = softmax (option "pdf_transform").
+        Waits for the current stream first: the call runs on the context's own stream and returns once its outputs are
+        written."""
+        x = self._f32(raw0)
+        n, dev = x.shape[0], self._dev()
+        count = torch.full((n,), -1, dtype=torch.int32, device=dev)
+        offset = torch.full((n,), -1, dtype=torch.int32, device=dev)
+        ray = torch.full((max(n * K, 1),), -1, dtype=torch.int32, device=dev)
+        z = torch.full((max(n * K, 1),), float("nan"), dtype=torch.float32, device=dev)
+        with torch.cuda.device(self.device):
+            torch.cuda.current_stream().synchronize()
+            self._check(self.lib.adn_pdf_sample(self.handle, x.data_ptr(), n, int(K), int(transform), count.data_ptr(),
+                                                offset.data_ptr(), ray.data_ptr(), z.data_ptr()))
+        return dict(count=count, offset=offset, ray=ray[:n * K], z=z[:n * K])
+
+    def stage5_density(self, raw1, z, ray_d, K, aux=True, rgba8=False):
+        """nerf_raw2outputs alone (adn_stage5_density_composite): raw1 [N K, 4], z [N K] and ray_d [N,3] ->
+        dict(rgb [N,3], rgba8 [N,4] uint8 when asked, and the aux outputs: True or an iterable of AUX_KEYS).  Synchronises
+        like pdf_sample."""
+        dev = self._dev()
+        r1, zz, rd = self._f32(raw1), self._f32(z), self._f32(ray_d)
+        n = rd.shape[0]
+        keys = self.AUX_KEYS if aux is True else tuple(aux or ())
+        out = dict(rgb=torch.empty((n, 3), dtype=torch.float32, device=dev),
+                   rgba8=torch.empty((n, 4), dtype=torch.uint8, device=dev) if rgba8 else None)
+        a = AuxOutputs()
+        for k in keys:
+            if k not in self.AUX_KEYS:
+                raise KeyError(f"unknown stage-5 output {k!r}")
+            out[k] = torch.empty((n, int(K)) if k in ("weights", "alpha", "z_vals") else (n,), dtype=torch.float32, device=dev)
+            setattr(a, "d_" + k, out[k].data_ptr())
+        with torch.cuda.device(self.device):
+            torch.cuda.current_stream().synchronize()
+            self._check(self.lib.adn_stage5_density_composite(self.handle, r1.data_ptr(), zz.data_ptr(), rd.data_ptr(), n, int(K),
+                                                              out["rgb"].data_ptr(), out["rgba8"].data_ptr() if rgba8 else None,
+                                                              C.byref(a)))
+        return out
 
     def budget_threshold(self, raw0, thr_min, K, max_samples, out=None):
         """raw0 [N,128] -> [1] float32 device tensor: the smallest threshold >= thr_min at which stage 2 with K samples per

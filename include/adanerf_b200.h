@@ -121,11 +121,14 @@ adn_status adn_net_shape(adn_ctx* ctx, int net_id, int* depth, int* width, int* 
 /* Loads {config.ini, dataset_info.txt, model0.onnx, model1.onnx} as written by src/export.py:28-93
  * (the directory the C++ viewer takes with -mp, adanerf_real_time_viewer/README.md:38-43).
  * Creates the context with the scene from dataset_info.txt; threshold / K from config.ini are
- * returned through thr_out / k_out (may be NULL). */
+ * returned through thr_out / k_out (may be NULL).  A config.ini with rayMarchSampler = [.., FromClassifiedDepth] (the
+ * DONeRF sampler; with InverseSqrtDistCentered and log, not NDC) sets options "sampler" = 1 and "pdf_transform" from
+ * losses[0]: BCEWithLogitsLoss -> 1, CrossEntropyLoss / CrossEntropyLossWeighted -> 2; any other loss is refused. */
 adn_status adn_create_from_export_dir(adn_ctx** out, const char* dir, int device, float* thr_out, int* k_out);
 
 /* Host-only (no GPU needed): parses the export directory like adn_create_from_export_dir and returns the
- * scene, threshold, K and the number of fp32 tensors found in model0.onnx / model1.onnx.  Replaces
+ * scene, threshold, K and the number of fp32 tensors found in model0.onnx / model1.onnx.  It does not report the
+ * sampler: callers that need it read rayMarchSampler / losses from config.ini themselves.  Replaces
  * Config::load + Config::loadDatasetInfo (adanerf_real_time_viewer/src/config.cpp:270-344). */
 adn_status adn_probe_export_dir(const char* dir, adn_scene* scene_out, float* thr_out, int* k_out, int* n_tensors_out /*[2]*/);
 
@@ -151,7 +154,18 @@ adn_status adn_probe_export_dir(const char* dir, adn_scene* scene_out, float* th
  *   16-byte aligned); d_nsamples receives 0 for every ray; non-NULL auxiliary outputs fail with ADN_ERR_INVALID;
  *   "sample_budget" is not applied (no selection runs, a budget group makes no reductions, adn_last_threshold returns
  *   `thr`); adn_get_stats reports n_samples = 0 and, profiled, stages 0-1 in ms_stage[0..1], the view in ms_stage[5] and 0
- *   in ms_stage[2..4].  0 = off [default]: renders are exactly as without the option). */
+ *   in ms_stage[2..4].  0 = off [default]: renders are exactly as without the option),
+ * "sampler" (0 = FromClassifiedDepthAdaptive, the threshold / top-K sampler and sigmoid(a) * zp composite [default];
+ *   1 = FromClassifiedDepth, the DONeRF sampler (src/nerf_raymarch_common.py:606-660): every render -- rays, aux, camera,
+ *   rgba8, surface, *_host, chunked or not -- places exactly K samples per ray by the inverse CDF of
+ *   pdf_transform(raw0) (nerf_sample_pdf, det = True, :160-192) and composites them with nerf_raw2outputs (:19-68):
+ *   alpha = 1 - exp(-relu(a) dist), dist = (z[k+1] - z[k], last 1e10) * |rays_d|.  `thr` is ignored; 1 <= K <= 128;
+ *   d_nsamples receives K for every ray; z_vals is never NaN; "sample_budget" > 0 and NDC scenes fail with
+ *   ADN_ERR_INVALID; "sampling_view" works as in the adaptive mode (it reads raw0 only)),
+ * "pdf_transform" (what sampler 1 applies to raw0 before the inverse CDF, chosen by losses[0] of the training config:
+ *   1 = sigmoid (BCEWithLogitsLoss) [default], 2 = softmax (CrossEntropyLoss, CrossEntropyLossWeighted).  0, the
+ *   reference's "no transform", fails with ADN_ERR_INVALID: raw0 then gives a non-monotone cdf, whose sample placement
+ *   would depend on the internals of ATen's binary search). */
 adn_status adn_set_option(adn_ctx* ctx, const char* name, int64_t value);
 
 /* Budget group: several contexts (one per row band, on one device or several) whose budgeted calls choose ONE threshold, the
@@ -271,6 +285,15 @@ adn_status adn_stage2_sample(adn_ctx* ctx, const float* d_raw0, int64_t n_rays, 
  * rank-2..K values. */
 adn_status adn_budget_threshold(adn_ctx* ctx, const float* d_raw0, int64_t n_rays, float thr_min, int K, int64_t max_samples,
                                 float* d_thr, void* stream);
+/* FromClassifiedDepth's sample placement (the stage 2 of option "sampler" = 1): nerf_sample_pdf(linspace(0, 1, 129),
+ * transform(raw0), K + 2, det = True) (src/nerf_raymarch_common.py:160-192, 606-660), samples 1 .. K, warped to world depth
+ * with the scene's LogTransform.  d_raw0 [N,128] fp32; transform 1 = sigmoid, 2 = softmax.  Outputs (d_count, d_offset,
+ * d_ray may be NULL): d_count [N] = K, d_offset [N] = r K, d_ray [N K] = r, d_z [N K] world depth, ascending per ray.
+ * N K < 2^31.  Like adn_sampling_view it is an inspection entry and takes no stream: it runs on the context's own stream,
+ * after the context's earlier calls, and returns once its outputs are written; d_raw0 must be complete when it is called
+ * (the stream-ordered path is option "sampler" on the render entries). */
+adn_status adn_pdf_sample(adn_ctx* ctx, const float* d_raw0, int64_t n_rays, int K, int transform, int32_t* d_count,
+                          int32_t* d_offset, int32_t* d_ray, float* d_z);
 /* The sampling network's view of raw0 alone (what option "sampling_view" draws after the sampling MLP), the viewer's
  * samplesToImage (adanerf_real_time_viewer/src/cuda/base_cuda_kernels.cu:487-528): d_raw0 [N,128] fp32, 16-byte aligned ->
  * d_rgb [N,3] fp32 (c0, c1, c2 as (c + 0.5) / 128) and d_rgba8 [N] uchar4 (each value * 255 truncated, alpha 255); either
@@ -300,6 +323,14 @@ adn_status adn_stage5_composite(adn_ctx* ctx, const float* d_raw1, const float* 
 adn_status adn_stage5_composite_aux(adn_ctx* ctx, const float* d_raw1, const float* d_zp, const float* d_z,
                                     const int32_t* d_offset, const int32_t* d_count, int64_t n_rays, int K, int dense,
                                     float* d_rgb, uint8_t* d_rgba8, const adn_aux_outputs* aux, void* stream);
+
+/* stage 5 of option "sampler" = 1: nerf_raw2outputs (src/nerf_raymarch_common.py:19-68) over K samples per ray,
+ * d_raw1 [N K, 4] and d_z [N K] in adn_pdf_sample's layout, d_ray_d [N,3] the ray directions of stage 0.  Outputs as
+ * adn_stage5_composite_aux (each may be NULL); z_vals is d_z unchanged, alpha the density alpha.  K = 1: the reference's
+ * dists are empty ([N, 0], :35-37), so every ray composites to nothing (rgb, weights, alpha, acc and depth 0; disp NaN).
+ * No stream: it runs and synchronises like adn_pdf_sample. */
+adn_status adn_stage5_density_composite(adn_ctx* ctx, const float* d_raw1, const float* d_z, const float* d_ray_d, int64_t n_rays,
+                                        int K, float* d_rgb, uint8_t* d_rgba8, const adn_aux_outputs* aux);
 
 /* ---- evaluation metric on the device ------------------------------------------------------ */
 /* calculate_mse / calculate_psnr (src/evaluate.py:49-54) of two device images of n_values floats each:
