@@ -9,6 +9,7 @@ import torch
 
 from conftest import load_golden
 from oracle import adanerf_oracle as orc
+from oracle import donerf_oracle as dno
 from oracle import stage_emulation as se
 
 F32 = np.float32
@@ -231,23 +232,36 @@ def test_ndc_depth_tables_are_the_cell_centres():
     np.testing.assert_array_equal(se.zlut_dense(orc.SCENE_PAVILLON_NDC, 128).view(np.uint32), dense.view(np.uint32))
 
 
-def test_linspace_is_atens_rule():
-    """linspace01 is ATen's per-element linspace rule (k * step below the half-way index, 1 - (K - k) * step from it).
-    torch's vectorised CPU kernel continues a lane chunk that starts below the half-way index with k * step past it, so
-    where 1 / K is inexact it can differ by 1 ulp; where 1 / K is a power of two every term is exact and the two agree bit
-    for bit -- K = 128 among them, the only K dense mode takes."""
-    for K in range(1, 257):
+def test_linspace_is_torch_linspace():
+    """linspace01 is torch.linspace(0, 1, K + 1) on the CPU bit for bit at every length 2 ... 259 (the sampler's u takes
+    lengths K + 2 <= 130, its cell edges and the dense table 129): k * step below the half-way index, fma(-step, K - k, 1)
+    from it.  The two-rounding form 1 - (K - k) * step differs at most lengths, though not at 129."""
+    n_two = 0
+    for K in range(1, 259):
         ours = se.linspace01(K)
         ref = torch.linspace(0, 1, K + 1).numpy()
-        diff = np.abs(ours.view(np.int32).astype(np.int64) - ref.view(np.int32))
-        assert diff.max() <= 1, K
-        if K & (K - 1) == 0:
-            np.testing.assert_array_equal(ours.view(np.uint32), ref.view(np.uint32), err_msg=f"K={K}")
+        np.testing.assert_array_equal(ours.view(np.uint32), ref.view(np.uint32), err_msg=f"length {K + 1}")
         assert ours[0] == 0 and ours[-1] == 1 and (np.diff(ours) > 0).all(), K
-    K = 9                                       # the rule itself, written out once: ATen's symmetric evaluation
+        step, k = F32(1) / F32(K), np.arange(K + 1)
+        two = np.where(k < (K + 1) // 2, k.astype(F32) * step, F32(1) - (K - k).astype(F32) * step).astype(F32)
+        n_two += not np.array_equal(two, ref)
+        if K == 128:
+            np.testing.assert_array_equal(two, ref)
+    assert n_two > 200, n_two
+    K = 9                                       # the rule itself, written out once
     step = F32(1) / F32(K)
-    want = [F32(k) * step if k < 5 else F32(1) - F32(K - k) * step for k in range(K + 1)]
+    want = [F32(k) * step if k < 5 else se.fma32(-step, F32(K - k), F32(1)) for k in range(K + 1)]
     np.testing.assert_array_equal(se.linspace01(K), np.array(want, F32))
+    assert any(not np.array_equal(se.linspace01(k, symmetric=False), se.linspace01(k)) for k in range(2, 130))
+
+
+@pytest.mark.parametrize("name", sorted(LOG_SCENES))
+def test_dense_table_keeps_its_bits(name):
+    """zlut_dense(scene, 128) is the table of the two-rounding linspace: 1 / 128 is a power of two, so both forms are exact."""
+    scene = LOG_SCENES[name]
+    t = (np.arange(128, dtype=F32) * F32(1.0 / 128)).astype(F32) + F32(0.5 / 128)
+    z = F32(0.001) * (F32(1) - t) + F32(1.0) * t
+    np.testing.assert_array_equal(se.zlut_dense(scene, 128).view(np.uint32), se._to_world(z, scene).view(np.uint32))
 
 
 def test_teeth_powf_depth_table():
@@ -466,3 +480,228 @@ def test_rgba8_is_the_viewers_compiled_clamp():
     np.testing.assert_array_equal(got, want)
     assert got[0, 0] == 0 and got[0, 1] == 0 and got[0, 2] == 255 and got[1, 0] == 0         # NaN, NaN, inf, -inf
     assert set(np.unique(se.rgba8(ks.reshape(-1, 1).repeat(3, 1))[:, 0])) == set(range(256))
+
+
+# ------------------------------------------------------------------------------------------------- fixed-K sampler
+DONERF_CASES = [("rand", t, K) for t in ("sigmoid", "softmax") for K in (1, 4, 8, 16)] + \
+               [("pav", t, K) for t in ("sigmoid", "softmax") for K in (4, 16)]
+TRANSFORM = {"sigmoid": 1, "softmax": 2}
+
+
+def _expf64(x):
+    """Correctly rounded expf through float64."""
+    with np.errstate(over="ignore"):
+        return np.exp(np.asarray(x, F32).astype(np.float64)).astype(F32)
+
+
+def _pow64(base, x):
+    return np.power(base, np.asarray(x, F32).astype(np.float64))
+
+
+def _powf(base, x):
+    return np.power(F32(base), np.asarray(x, F32), dtype=F32)
+
+
+def _donerf_fixture(nets, tname, K):
+    from adanerf_b200.synthetic import load_npz
+    import os
+    g = load_npz(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", f"donerf_{nets}_{tname}_k{K}.npz"))
+    return g, orc.SCENE_PAVILLON if nets == "pav" else orc.SCENE_BARBERSHOP
+
+
+def _pdf_edge_rows():
+    """raw0 rows [R,128] at the sampler's edges: constant rows (exact ties), one-hot rows (+-200), two spikes with long
+    clamped runs between them (cells 0 and 127 among them), all -200, softmax rows with x - m in [-104, -87] (subnormal
+    exp) and below -104 (exp = 0), +-1e30 and -0.0, rows holding +-inf or NaN, and plain random rows."""
+    R = [np.full(128, v) for v in (0.0, 3.5, -200.0, 200.0, 1e30, -1e30, -0.0)]
+    for c in (0, 1, 63, 64, 127):
+        for hi, lo in ((200.0, -200.0), (-200.0, 200.0)):
+            r = np.full(128, lo)
+            r[c] = hi
+            R.append(r)
+    for a, b in ((0, 127), (0, 64), (5, 90), (126, 127), (0, 1), (31, 96)):
+        r = np.full(128, -200.0)
+        r[[a, b]] = 200.0
+        R.append(r)
+        r = np.full(128, -200.0)
+        r[a], r[b] = 200.0, 0.0
+        R.append(r)
+    rng = np.random.default_rng(11)
+    for lo, hi in ((-104.0, -87.0), (-150.0, -104.0), (-110.0, -80.0)):
+        r = rng.uniform(lo, hi, 128)
+        r[rng.integers(128)] = 0.0
+        R.append(r)
+    R.extend(rng.choice([1e30, -1e30, -0.0, 0.0], (4, 128)))
+    for v in (np.inf, -np.inf, np.nan):
+        for c in (0, 77, 127):
+            r = rng.standard_normal(128) * 3
+            r[c] = v
+            R.append(r)
+        R.append(np.full(128, v))
+    r = rng.standard_normal(128)
+    r[3], r[90] = np.inf, -np.inf
+    R.append(r)
+    r = np.full(128, -200.0)
+    r[[10, 20]] = np.inf
+    R.append(r)
+    for s in (0.01, 1, 10, 50):
+        R.extend(rng.standard_normal((8, 128)) * s)
+    with np.errstate(over="ignore"):
+        return np.asarray(R, F32)
+
+
+@pytest.mark.parametrize("case", DONERF_CASES, ids=[f"{n}-{t}-k{k}" for n, t, k in DONERF_CASES])
+def test_pdf_sample_emulation_matches_the_oracle(case):
+    """With correctly rounded transcendentals the emulation is the reference's z (the fixtures, which
+    donerf_oracle.pdf_sample reproduces bit for bit) up to the documented deviations: within 10 ulp of the power w on the
+    Pavillon net's peaked distributions; on the random nets' flat ones, where t = (u - c0) / denom amplifies a last-bit
+    cdf difference, within 256 ulp of w and 1e-5 of the warped range.  z ascends per ray."""
+    g, scene = _donerf_fixture(*case)
+    K = case[2]
+    z = se.pdf_sample(g["raw0"], K, TRANSFORM[case[1]], scene, _expf64, _pow64)
+    assert z.shape == g["z"].shape and (np.diff(z, axis=1) >= 0).all()
+    dr0, dr1 = (float(F32(v)) for v in scene["depth_range"])
+    w = g["z"].astype(np.float64) - dr0 + 1.0
+    ulps = np.abs(z.astype(np.float64) - g["z"]) / se.ulp32(w)
+    du = np.abs(np.log(z.astype(np.float64) - dr0 + 1.0) - np.log(w)) / np.log(dr1 - dr0 + 1.0)
+    print(f"{case}: {100 * (ulps > 0).mean():.1f} % of z differ, at most {ulps.max():.0f} ulp of w, {du.max():.2g} of the warped range")
+    assert ulps.max() <= (10 if case[0] == "pav" else 256) and du.max() <= 1e-5
+
+
+def test_pdf_search_shortcut_is_the_binary_search():
+    """_search's counting shortcut (non-decreasing, NaN-free rows) equals the kernel's binary search and np.searchsorted
+    per row, for right=True and False; rows with NaN or a decreasing step take the search itself."""
+    rng = np.random.default_rng(3)
+    raw = np.concatenate([_pdf_edge_rows(), (rng.standard_normal((400, 128)) * rng.choice([0.1, 1, 5, 30], (400, 1)))])
+    for tr in (1, 2):
+        cdf = se.pdf_cdf(se.pdf_transform(raw.astype(F32), tr, _expf64))
+        mono = ~np.isnan(cdf).any(1) & (np.diff(cdf, axis=1) >= 0).all(1)
+        assert (~mono).sum() >= 4 and mono.sum() > 400
+        for K in (1, 7, 33, 128):
+            u = se.linspace01(K + 1)[1:K + 1]
+            for right in (True, False):
+                got, lit = se._search(cdf, u, right), se.binary_search(cdf, u, right)
+                np.testing.assert_array_equal(got, lit)
+                ref = np.stack([np.searchsorted(c, u, side="right" if right else "left") for c in cdf[mono]])
+                np.testing.assert_array_equal(got[mono], ref)
+
+
+def test_pdf_edge_rows_keep_nan_in_their_ray():
+    """Rows holding +-inf or NaN: the emulation's NaN samples are the oracle's, sample for sample, and no finite row has one."""
+    raw = _pdf_edge_rows()
+    finite = np.isfinite(raw).all(1)
+    for tr in (1, 2):
+        for K in (1, 7, 33, 128):
+            z = se.pdf_sample(raw, K, tr, orc.SCENE_PAVILLON, _expf64, _pow64)
+            ref = dno.pdf_sample(torch.from_numpy(raw), K, tr, orc.SCENE_PAVILLON["depth_range"]).numpy()
+            np.testing.assert_array_equal(np.isnan(z), np.isnan(ref))
+            assert not np.isnan(z[finite]).any() and np.isnan(z).any()
+
+
+SAMPLER_TEETH = {"fp32 cdf": dict(scan="fp32"), "fp32 sequential wsum": dict(wsum="fp32"), "right=False": dict(right=False),
+                 "no clamp": dict(clamp=False), "j step linspace": dict(symmetric=False), "fp32 pow": dict(pow64=_powf)}
+
+
+def test_teeth_sampler():
+    """Each mutation of the sampler's emulation moves at least one z of the edge rows and the fixtures' raw0."""
+    raw = np.concatenate([_pdf_edge_rows()] + [_donerf_fixture(*c)[0]["raw0"] for c in (("pav", "sigmoid", 16), ("rand", "softmax", 16))])
+    moved = {k: 0 for k in SAMPLER_TEETH}
+    for tr in (1, 2):
+        for K in (7, 33, 128):
+            good = se.pdf_sample(raw, K, tr, orc.SCENE_PAVILLON, _expf64, _pow64)
+            for name, kw in SAMPLER_TEETH.items():
+                kw = dict(dict(expf=_expf64, pow64=_pow64), **kw)
+                bad = se.pdf_sample(raw, K, tr, orc.SCENE_PAVILLON, **kw)
+                moved[name] += int((~((bad.view(np.int32) == good.view(np.int32)) | (np.isnan(bad) & np.isnan(good)))).sum())
+    print("samples moved:", moved)
+    assert all(v > 0 for v in moved.values()), moved
+
+
+def test_teeth_density_composite():
+    """tree=False and butterfly=False change the warp composite's outputs on the density path."""
+    rng = np.random.default_rng(8)
+    n, K = 300, 100
+    raw1 = (rng.standard_normal((n * K, 4)) * 2).astype(F32)
+    z = np.sort(rng.uniform(0.2, 8, (n, K)), axis=1).astype(F32).reshape(-1)
+    rd = rng.standard_normal((n, 3)).astype(F32)
+    alpha = se.density_alpha(raw1[:, 3], z, rd, K, _expf64)
+    sig = _sig32(raw1[:, :3])
+    args = (sig, None, z, np.arange(n) * K, np.full(n, K), K)
+    good = se.stage5_warp(*args, alpha=alpha)
+    for kw in (dict(tree=False), dict(butterfly=False)):
+        bad = se.stage5_warp(*args, alpha=alpha, **kw)
+        assert not np.array_equal(good["rgb"], bad["rgb"]), kw
+
+
+@pytest.mark.parametrize("case", DONERF_CASES, ids=[f"{n}-{t}-k{k}" for n, t, k in DONERF_CASES])
+def test_density_composite_emulation_matches_the_reference(case):
+    """density_alpha + stage5_density on the fixtures' raw1 / z / rays_d against the reference's tensors (at
+    test_donerf_gpu's tolerances: ATen's vectorised exp is not expf), z_vals = z, and K = 1 composites to nothing.  The
+    thread and warp chains agree with each other to the same tolerance."""
+    g, _ = _donerf_fixture(*case)
+    K = case[2]
+    n = g["ray_d"].shape[0]
+    raw1, z = g["raw1"].reshape(n * K, 4), g["z"].reshape(-1)
+    alpha = se.density_alpha(raw1[:, 3], z, g["ray_d"], K, _expf64)
+    for fn in (se.stage5_thread, se.stage5_warp):
+        out = fn(_sig32(raw1[:, :3]), None, z, np.arange(n) * K, np.full(n, K), K, alpha=alpha)
+        np.testing.assert_array_equal(out["z_vals"], g["z"])
+        if K == 1:
+            assert (out["alpha"] == 0).all() and (out["rgb"] == 0).all() and (out["acc_map"] == 0).all()
+            continue
+        np.testing.assert_allclose(out["alpha"], g["alpha"], rtol=1e-5, atol=2e-6)
+        np.testing.assert_allclose(out["weights"], g["weights"], rtol=1e-5, atol=2e-6)
+        np.testing.assert_allclose(out["rgb"], g["rgb"], rtol=1e-5, atol=2e-6)
+    assert se.stage5_density(_sig32(raw1[:, :3]), alpha, z, K)["z_vals"].shape == (n, K)
+
+
+def test_density_alpha_rules():
+    """relu keeps NaN, the last sample's distance is 1e10 |d|, repeated z with an inf density is 0 * inf = NaN, decreasing z
+    gives alpha < 0, |d| = 0 gives alpha 0, K = 1 gives alpha 0."""
+    a = np.array([np.nan, -1.0, 2.0, np.inf, 1.0, 1.0], F32)
+    z = np.array([0.0, 1.0, 2.0, 4.0, 4.0, 3.5], F32)
+    al = se.density_alpha(a, z, np.array([[0.0, 3.0, 4.0]], F32), 6, _expf64)
+    assert np.isnan(al[0]) and al[1] == 0 and al[2] == F32(1) - _expf64(F32(-20.0)) and np.isnan(al[3])
+    assert al[4] < 0 and al[5] == 1
+    assert (se.density_alpha(a, z, np.zeros((1, 3), F32), 6, _expf64)[1:3] == 0).all()
+    assert (se.density_alpha(a, z, np.ones((6, 3), F32), 1, _expf64) == 0).all()
+
+
+def test_fixture_z_attribution():
+    """Which documented deviation moves which fixture z bits.  Starting from torch's CPU sigmoid / softmax values, the
+    kernel's placement is switched to the reference's one deviation at a time: torch.sum for the double warp sum, one
+    sequential double cumsum for the warp scan, torch's fp32 pow for the double pow -- evaluated, as the reference does,
+    on the [:, 1:-1] slice of the K + 2 samples (ATen's fp32 pow gives other bits on a contiguous tensor).  With the sum
+    and the pow both switched every fixture bit is the reference's; the scan association moves none."""
+    tsum = lambda w: torch.sum(torch.from_numpy(w), -1).numpy()
+    counts, total = {}, 0
+
+    def pow_ref(scene):
+        dr = scene["depth_range"]
+
+        def f(base, x):
+            t = torch.zeros(x.shape[0], x.shape[1] + 2)
+            t[:, 1:-1] = torch.from_numpy(np.asarray(x, F32))
+            return ((dr[1] - dr[0] + 1) ** t[:, 1:-1]).numpy()
+        return f
+
+    for case in DONERF_CASES:
+        g, scene = _donerf_fixture(*case)
+        K = case[2]
+        x = torch.from_numpy(g["raw0"])
+        w = (torch.sigmoid(x) if case[1] == "sigmoid" else torch.softmax(x, -1)).numpy()
+        total += g["z"].size
+        for s in ("double", "torch.sum"):
+            for c in ("warp", "seq"):
+                cdf = se.pdf_cdf(w, wsum=tsum if s == "torch.sum" else "warp", scan=c)
+                for p in ("double", "fp32"):
+                    z = se.pdf_place(cdf, K, scene, pow_ref(scene) if p == "fp32" else _pow64)
+                    key = (s, c, p)
+                    counts[key] = counts.get(key, 0) + int((z.view(np.int32) != g["z"].view(np.int32)).sum())
+    for k, v in counts.items():
+        print(f"sum {k[0]:9s} scan {k[1]:4s} pow {k[2]:6s}: {v:5d} of {total} fixture z differ ({100 * v / total:.1f} %)")
+    assert counts[("torch.sum", "warp", "fp32")] == 0 and counts[("torch.sum", "seq", "fp32")] == 0
+    for s in ("double", "torch.sum"):
+        for p in ("double", "fp32"):
+            assert counts[(s, "warp", p)] == counts[(s, "seq", p)]
+    assert counts[("double", "warp", "fp32")] > 0 and counts[("torch.sum", "warp", "double")] > 0
