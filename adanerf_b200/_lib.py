@@ -49,7 +49,8 @@ SYMBOLS = [
     "adn_render_camera_rgba8", "adn_render_rays_host", "adn_render_camera_host", "adn_stage0_features",
     "adn_generate_ray_directions", "adn_mlp0_forward", "adn_stage2_sample", "adn_budget_threshold", "adn_stage3_encode",
     "adn_mlp1_forward", "adn_stage5_composite", "adn_stage5_composite_aux", "adn_image_metrics", "adn_sampling_view",
-    "adn_image_flip", "adn_image_iwssim", "adn_pdf_sample", "adn_stage5_density_composite",
+    "adn_image_flip", "adn_image_iwssim", "adn_pdf_sample", "adn_stage5_density_composite", "adn_camera_rays",
+    "adn_linear_depths",
 ]
 
 _lib = None
@@ -100,6 +101,8 @@ def load_library():
     lib.adn_sampling_view.argtypes = [vp, f32p, i64, f32p, vp]
     lib.adn_pdf_sample.argtypes = [vp, f32p, i64, C.c_int, C.c_int, i32p, i32p, i32p, f32p]
     lib.adn_stage5_density_composite.argtypes = [vp, f32p, f32p, f32p, i64, C.c_int, f32p, vp, C.POINTER(AuxOutputs)]
+    lib.adn_camera_rays.argtypes = [vp, fp, fp, f32p, i64, f32p, f32p, f32p]
+    lib.adn_linear_depths.argtypes = [vp, C.c_int, f32p]
     lib.adn_stage3_encode.argtypes = [vp, f32p, f32p, i32p, f32p, i64, f32p, vp]
     lib.adn_mlp1_forward.argtypes = [vp, f32p, i64, f32p, vp]
     lib.adn_stage5_composite.argtypes = [vp, f32p, f32p, f32p, i32p, i32p, i64, C.c_int, f32p, f32p, f32p, vp]

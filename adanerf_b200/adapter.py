@@ -12,6 +12,8 @@ existing TrainConfig).  Only the entries those callers read are produced:
 With rayMarchSampler FromClassifiedDepth (sampler=1, the DONeRF baseline) the reference's shading-net dict has neither
 AdaptiveSamplePositions (the feature set is not adaptive, features.py:561-563) nor OracleWeights (its losses[0] is the
 sampler's transform loss, not NeRFWeightMultiplicationLoss, features.py:503-504), and neither has this one's.
+A one-network run (rayMarchSampler LinearlySpacedZNearZFar, sampler=2, plain NeRF) returns `([rgb], [dict])`: one network,
+one dict, as TrainConfig.inference of a one-model run does.
     dicts[i]["PostProcessedNetworkOutput"]   = outs[i]                           (util/helper.py:79-130)
 
 The batch keys are the reference's DatasetKeyConstants (src/datasets.py:24-38)."""
@@ -19,6 +21,9 @@ import torch
 
 from .onnx_weights import PDF_TRANSFORMS
 from .renderer import Renderer
+
+# the rayMarchSampler of a one-network (plain NeRF) run, on world and on NDC scenes (src/nerf_raymarch_common.py:261-326)
+LINEAR_SAMPLERS = ("LinearlySpacedZNearZFar", "LinearlySpacedZNearZFarNoDepthRange")
 
 # src/datasets.py:29-35 and src/features.py:20-40
 KEY_POSE, KEY_ROT, KEY_DIRS = "ImagePose", "ImageRotation", "RayDirectionsSamples"
@@ -35,13 +40,15 @@ class B200Inference:
     def __init__(self, scene, sampling_net, shading_net, threshold, num_samples, device=0, want_oracle_weights=None,
                  want_aux=False, sampler=0, pdf_transform=1):
         """sampler / pdf_transform: the renderer options of the same names (0 = the adaptive sampler; 1 = FromClassifiedDepth
-        with transform 1 = sigmoid or 2 = softmax; threshold is then not used)."""
+        with transform 1 = sigmoid or 2 = softmax; 2 = LinearlySpacedZNearZFar, plain NeRF: sampling_net is None and
+        inference returns one network's outputs; threshold is not used by 1 and 2)."""
         self.renderer = Renderer(scene, device=device, sampling_net=sampling_net, shading_net=shading_net)
         self.threshold = float(threshold)
         self.K = int(num_samples)
         self.sampler = int(sampler)
         if self.sampler:
             self.renderer.set_option("sampler", self.sampler)
+        if self.sampler == 1:
             self.renderer.set_option("pdf_transform", int(pdf_transform))
         default_ow = self.threshold == 0.0 and not self.sampler
         self.want_oracle_weights = default_ow if want_oracle_weights is None else bool(want_oracle_weights)
@@ -51,8 +58,10 @@ class B200Inference:
     @staticmethod
     def args_from_train_config(train_config):
         """(scene, [sampling_net, shading_net], threshold, K) read from an initialised reference TrainConfig -- no device
-        needed (tests/test_adapter_config.py runs this against the live reference)."""
-        f1 = train_config.f_in[1]
+        needed (tests/test_adapter_config.py runs this against the live reference).  A one-network run (plain NeRF,
+        inFeatures = [RayMarchFromPoses]) gives [None, its net], and its depth_range is f_in[0]'s: without SpherePosDir the
+        reference places and reports depth with the dataset's unwarped range (datasets.py:154-159)."""
+        f1 = train_config.f_in[-1]
         info = train_config.dataset_info
         scene = dict(view_cell_center=list(info.view.view_cell_center), view_cell_size=list(info.view.view_cell_size),
                      depth_range=list(f1.depth_range), max_depth=float(f1.max_depth), fov=float(info.view.fov),
@@ -66,15 +75,21 @@ class B200Inference:
             if hasattr(f, "enc_type"):
                 p, d = (-1, -1) if f.enc_type == "none" else (int(f.n_freq_pos), int(f.n_freq_dir))
                 scene.update({kp: p if p > 0 else min(p, zero), kd: d if d > 0 else min(d, zero)})
-        thr = float(getattr(f1.z_sampler, "threshold", 0.0))   # FromClassifiedDepth has none
-        return scene, [train_config.models[0], train_config.models[1]], thr, int(f1.n_ray_samples)
+        thr = float(getattr(f1.z_sampler, "threshold", 0.0))   # FromClassifiedDepth and the linear samplers have none
+        models = [train_config.models[0], train_config.models[1]] if len(train_config.models) > 1 else [None, train_config.models[0]]
+        return scene, models, thr, int(f1.n_ray_samples)
 
     @staticmethod
     def sampler_from_train_config(train_config):
         """(sampler, pdf_transform) of the shading net's rayMarchSampler and losses[0] (src/nerf_raymarch_common.py:625-637):
         (1, 1 or 2) for FromClassifiedDepth, else (0, 1): the adaptive path.  Raises ValueError for a FromClassifiedDepth run
-        whose losses[0] selects no transform."""
-        if type(train_config.f_in[1].z_sampler).__name__ != "FromClassifiedDepth":
+        whose losses[0] selects no transform.  A one-network run with LinearlySpacedZNearZFar (NoDepthRange) gives (2, 1)."""
+        name = type(train_config.f_in[-1].z_sampler).__name__
+        if len(train_config.f_in) == 1:
+            if name not in LINEAR_SAMPLERS:
+                raise ValueError(f"one-network runs need rayMarchSampler {' or '.join(LINEAR_SAMPLERS)}, not {name}")
+            return 2, 1
+        if name != "FromClassifiedDepth":
             return 0, 1
         loss0 = train_config.config_file.losses[0]
         if loss0 not in PDF_TRANSFORMS:
@@ -99,6 +114,12 @@ class B200Inference:
                                         want_nsamples=True, want_oracle_weights=self.want_oracle_weights,
                                         want_aux=("weights", "alpha", "z_vals", "depth_est") if self.want_aux else False)
         rgb = out["rgb"]
+        if self.sampler == 2:   # one network: its dict only (TrainConfig.inference of a one-model run)
+            d = {KEY_POST: rgb}
+            if self.want_aux:
+                d[KEY_WEIGHTS], d[KEY_ALPHA], d[KEY_ZVALS] = out["weights"], out["alpha"], out["z_vals"]
+                d[KEY_DEPTH] = out["depth_est"].reshape(-1, 1)
+            return [rgb], [d]
         raw0 = out["oracle_weights"]
         d0 = {KEY_POST: raw0, KEY_NET_OUT: raw0}
         d1 = {KEY_POST: rgb}

@@ -11,6 +11,10 @@ without instantiating the reference's classes, so trained checkpoints run throug
         --dataset-info dataset_info.txt --threshold 0.2 --samples 8 --out export_dir \
         [--pos-enc nerf,nerf --pos-enc-args 10-4,10-4] [--sampler FromClassifiedDepth --sampling-loss BCEWithLogitsLoss]
 
+A plain NeRF run has one network: `--sampler LinearlySpacedZNearZFar --weights0 Net0_opt.weights` (no --weights1,
+--threshold or sampling net) writes {config.ini, dataset_info.txt, model0.onnx} with one-item lists; --pos-enc /
+--pos-enc-args then name that one net's encoding.
+
 The run's posEnc / posEncArgs (sampling net, shading net) go on the command line: the sampling net's split into position
 and direction bands cannot be read from the width of layers.0.
 """
@@ -20,7 +24,7 @@ from collections import OrderedDict
 
 import torch
 
-from .onnx_weights import PDF_TRANSFORMS, net_shapes, write_export_dir
+from .onnx_weights import PDF_TRANSFORMS, net_shapes, write_export_dir, write_nerf_export_dir
 from .renderer import enc_columns
 
 SAMPLING_KEYS = ("layers.0.weight", "layers.0.bias")
@@ -160,23 +164,54 @@ def weights_to_export_dir(weights0, weights1, out_dir, scene, threshold, num_sam
     return sd0, sd1
 
 
+def nerf_weights_to_export_dir(weights, out_dir, scene, num_samples, allow_pickle=False, encoding=None):
+    """One NeRF `.weights` file -> a one-network export directory (onnx_weights.write_nerf_export_dir).  encoding: (P, D)
+    band counts of the net, None keeps the scene's."""
+    sd = load_weights_file(weights, allow_pickle)
+    for k in SHADING_KEYS:
+        if k not in sd:
+            raise ValueError(f"NeRF net: missing {k} (expected NeRF with use_viewdirs, src/models.py:214-250)")
+    if encoding is not None:
+        scene = dict(scene, n_freq_pos=encoding[0], n_freq_dir=encoding[1])
+    n_p = enc_columns(scene.get("n_freq_pos", 10))
+    if sd["pts_linears.0.weight"].shape[1] != n_p:
+        raise ValueError(f"NeRF net: pts_linears.0.weight reads {sd['pts_linears.0.weight'].shape[1]} columns, expected {n_p}")
+    write_nerf_export_dir(out_dir, scene, sd, int(num_samples))
+    return sd
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
-    ap.add_argument("--weights0", required=True, help="sampling net checkpoint (.weights)")
-    ap.add_argument("--weights1", required=True, help="shading net checkpoint (.weights)")
+    ap.add_argument("--weights0", required=True, help="sampling net checkpoint (.weights); the NeRF net of a one-network run")
+    ap.add_argument("--weights1", default=None, help="shading net checkpoint (.weights); required unless --sampler LinearlySpacedZNearZFar")
     ap.add_argument("--dataset-info", required=True, help="dataset_info.txt of the run (scene constants)")
-    ap.add_argument("--threshold", type=float, required=True, help="adaptiveSamplingThreshold")
+    ap.add_argument("--threshold", type=float, default=None, help="adaptiveSamplingThreshold (two-network runs)")
     ap.add_argument("--samples", type=int, required=True, help="numRaymarchSamples of the shading net (K)")
     ap.add_argument("--out", required=True)
     ap.add_argument("--allow-pickle", action="store_true",
                     help="also read checkpoints that hold a pickled nn.Module (executes code from the file: trusted files only)")
     ap.add_argument("--pos-enc", default=None, help="posEnc of the run, sampling net then shading net: nerf,nerf (default) or none")
     ap.add_argument("--pos-enc-args", default=None, help="posEncArgs of the run, e.g. 10-4,10-4 (default) or 16-4,6-2")
-    ap.add_argument("--sampler", default="FromClassifiedDepthAdaptive", choices=("FromClassifiedDepthAdaptive", "FromClassifiedDepth"),
-                    help="rayMarchSampler of the shading net: the adaptive sampler (default) or DONeRF's fixed-K FromClassifiedDepth")
+    ap.add_argument("--sampler", default="FromClassifiedDepthAdaptive",
+                    choices=("FromClassifiedDepthAdaptive", "FromClassifiedDepth", "LinearlySpacedZNearZFar"),
+                    help="rayMarchSampler of the shading net: the adaptive sampler (default), DONeRF's fixed-K FromClassifiedDepth, "
+                         "or LinearlySpacedZNearZFar for a one-network NeRF run (--weights0 only)")
+    ap.add_argument("--ndc", action="store_true", help="a one-network run on an NDC scene (LinearlySpacedZNearZFarNoDepthRange)")
+    ap.add_argument("--z-near", type=float, default=0.001, help="zNear of a one-network run")
+    ap.add_argument("--z-far", type=float, default=1.0, help="zFar of a one-network run")
     ap.add_argument("--sampling-loss", default="BCEWithLogitsLoss", choices=tuple(PDF_TRANSFORMS),
                     help="losses[0] of a FromClassifiedDepth run: sigmoid (BCEWithLogitsLoss) or softmax (the CrossEntropy losses)")
     a = ap.parse_args(argv)
+    if a.sampler == "LinearlySpacedZNearZFar":
+        enc = None
+        if a.pos_enc is not None or a.pos_enc_args is not None:
+            enc = parse_encoding(("nerf", a.pos_enc or "nerf"), ("10-4", a.pos_enc_args or "10-4"))[1]
+        scene = dict(read_dataset_info(a.dataset_info), use_ndc=a.ndc, z_near=a.z_near, z_far=a.z_far)
+        nerf_weights_to_export_dir(a.weights0, a.out, scene, a.samples, a.allow_pickle, enc)
+        print(f"wrote {a.out}")
+        return
+    if a.weights1 is None or a.threshold is None:
+        ap.error("--weights1 and --threshold are required for two-network runs")
     encoding = None
     if a.pos_enc is not None or a.pos_enc_args is not None:
         split = lambda v, d: tuple(x.strip() for x in (v or d).strip("[]").split(","))

@@ -66,6 +66,7 @@ struct adn_ctx {
   Buf zlut;                       // [128] world depth of the cell centres (log warp)
   Buf zlut_dense;                 // [dense_K]
   int dense_K = 0;
+  Buf zlin;                       // linear_depths(K) of every K = 1..128, the table of K at K (K - 1) / 2 (sampler 2)
   Net net[2];
   int mlp0_terms = 3;
   int n_feat0 = 90;               // sampling-net input features: 6 + 6 (n_freq_pos0 + n_freq_dir0)
@@ -79,10 +80,12 @@ struct adn_ctx {
   bool sampling_view = false;     // adn_set_option "sampling_view": renders draw the sampling net's view (stages 0-1 + view)
   bool last_view = false;         // the last render drew the view (it counts no samples)
   bool prof_view = false;         // the profiled render drew the view (slots 2-4 unused, the view kernel in slot 5)
-  int sampler = 0;                // adn_set_option "sampler": 0 = FromClassifiedDepthAdaptive, 1 = FromClassifiedDepth (fixed K)
+  int sampler = 0;                // adn_set_option "sampler": 0 = FromClassifiedDepthAdaptive, 1 = FromClassifiedDepth (fixed K),
+                                  // 2 = LinearlySpacedZNearZFar (no sampling net)
+  bool prof_linear = false;       // the profiled render ran sampler 2 (rays in slot 0, slot 1 unused)
   int pdf_transform = kPdfSigmoid;   // adn_set_option "pdf_transform": what FromClassifiedDepth applies to raw0 first
   // scratch
-  Buf tiles0, raw0, ray_o, ray_d, count, offset, rayidx, zbuf, zpbuf, tiles1, raw1, s2scratch, rgba, metric, flip, iwssim;
+  Buf tiles0, raw0, ray_o, ray_d, ray_dirs, count, offset, rayidx, zbuf, zpbuf, tiles1, raw1, s2scratch, rgba, metric, flip, iwssim;
   Buf dirs, rgb, nsamples;        // device side of the *_host entry points
   Buf budget_keys, budget_work, budget_thr;   // sample budget: candidate keys, histograms + select state, t*
   BudgetGroup group;              // adn_set_budget_group: the reducer that sums the selection's histograms across members
@@ -495,20 +498,28 @@ void set_ndc_projection(adn_ctx* ctx, int W, int H, float focal_in) {
   ctx->sc.ndc_ch = float(-1.0 / (double(H) / (2.0 * focal)));
 }
 
+// The K depths of LinearlySpacedZNearZFar.generate with det = True (nerf_raymarch_common.py:310-326), which the thr == 0
+// branch of FromClassifiedDepthAdaptive.generate (:708-720) shares, in torch's fp32 steps: t = linspace(0, 1, K + 1)[k] +
+// 0.5 / K, with ATen's CPU linspace (k step below the half-way index, fma(-step, K - k, 1) from it on), z = z_near (1 - t) +
+// z_far t, then LogTransform.to_world with the pow in double.  NDC scenes (the NoDepthRange samplers, :276-289 / :797-805)
+// keep z.
+std::vector<float> linear_depths(const adn_scene& sc, int K) {
+  std::vector<float> lut(K);
+  const double max_v = double(sc.depth_range[1]) - double(sc.depth_range[0]);
+  const float step = 1.0f / float(K);
+  for (int k = 0; k < K; ++k) {
+    const float lin = (k < (K + 1) / 2) ? float(k) * step : std::fma(-step, float(K - k), 1.0f);
+    const float t = lin + float(0.5 / K);
+    const float z = sc.z_near * (1.0f - t) + sc.z_far * t;
+    const float w = float(std::pow(max_v + 1.0, double(z)));
+    lut[k] = sc.use_ndc ? z : (w - 1.0f) + sc.depth_range[0];
+  }
+  return lut;
+}
+
 adn_status ensure_dense_lut(adn_ctx* ctx, int K) {
   if (ctx->dense_K == K) return ADN_OK;
-  // thr == 0 branch of FromClassifiedDepthAdaptive.generate (nerf_raymarch_common.py:708-720), fp32 steps
-  std::vector<float> lut(K);
-  const double max_v = double(ctx->scene.depth_range[1]) - double(ctx->scene.depth_range[0]);
-  for (int k = 0; k < K; ++k) {
-    // torch.linspace(0,1,K+1)[k] + 0.5/K in fp32
-    const float step = 1.0f / float(K);
-    const float lin = (k < (K + 1) / 2) ? float(k) * step : 1.0f - float(K - k) * step;  // ATen linspace is symmetric
-    const float t = lin + float(0.5 / K);
-    const float z = ctx->scene.z_near * (1.0f - t) + ctx->scene.z_far * t;
-    const float w = float(std::pow(max_v + 1.0, double(z)));
-    lut[k] = ctx->scene.use_ndc ? z : (w - 1.0f) + ctx->scene.depth_range[0];   // NoDepthRange: :797-805
-  }
+  const std::vector<float> lut = linear_depths(ctx->scene, K);
   adn_status s = ensure(ctx, ctx->zlut_dense, sizeof(float) * K);
   if (s != ADN_OK) return s;
   ADN_CUDA(ctx, cudaMemcpy(ctx->zlut_dense.p, lut.data(), sizeof(float) * K, cudaMemcpyHostToDevice));
@@ -622,12 +633,31 @@ adn_status run_stages_0_1(adn_ctx* ctx, const RenderCall& c, int64_t w, bool tim
   return ADN_OK;
 }
 
-// Stages 2-5 of one chunk, stream ordered: read what run_stages_0_1 wrote for the same chunk and w.  d_thr: stage 2's
+// Sampler 2's rays of one chunk, in place of stages 0-1: ray_o / ray_d for stage 3 and, on NDC scenes, the composite's NDC
+// directions (ray_dirs).  timing: record ev[0..2] (stage 1's slot stays empty).
+adn_status run_rays(adn_ctx* ctx, const RenderCall& c, bool timing) {
+  if (timing) cudaEventRecord(ctx->ev[0], c.st);
+  ADN_CUDA(ctx, launch_camera_rays(ctx->sc, make_pose(c.pose, c.rot), c.d_dirs, c.cam ? &*c.cam : nullptr, c.n_rays,
+                                   ctx->ray_o.as<float>(), ctx->ray_d.as<float>(),
+                                   ctx->scene.use_ndc ? ctx->ray_dirs.as<float>() : nullptr, c.st));
+  ctx->stats.kernel_launches++;
+  if (timing) {
+    cudaEventRecord(ctx->ev[1], c.st);
+    cudaEventRecord(ctx->ev[2], c.st);
+  }
+  return ADN_OK;
+}
+
+// Sampler 2's depth table for K (1-128) in ctx->zlin.
+const float* zlin_table(const adn_ctx* ctx, int K) { return ctx->zlin.as<float>() + K * (K - 1) / 2; }
+
+// Stages 2-5 of one chunk, stream ordered: read what run_stages_0_1 (run_rays) wrote for the same chunk and w.  d_thr: stage 2's
 // threshold as a device float (sample budget), null = c.thr.  timing: record ev[3..6].
 adn_status run_stages_2_5(adn_ctx* ctx, const RenderCall& c, int64_t w, const float* d_thr, bool timing) {
   const int64_t n = c.n_rays;
   const int K = c.K;
-  const bool fixed_k = ctx->sampler == 1;   // FromClassifiedDepth: the inverse-CDF sampler and the density composite
+  const bool fixed_k = ctx->sampler != 0;   // K samples on every ray and the density composite
+  const bool linear = ctx->sampler == 2;    // LinearlySpacedZNearZFar: the depth table, no sampling net
   const bool dense = !fixed_k && c.thr == 0.0f;
   const int64_t cap = n * K;
   adn_status s;
@@ -647,7 +677,7 @@ adn_status run_stages_2_5(adn_ctx* ctx, const RenderCall& c, int64_t w, const fl
   if (!fused_enc && (s = ensure(ctx, ctx->tiles1, size_t(pad128(cap) / 128) * ctx->net[1].prog.in.tile_bytes())) != ADN_OK) return s;
   if ((s = ensure(ctx, ctx->raw1, size_t(pad128(cap)) * 16)) != ADN_OK) return s;
 
-  float* raw0 = c.d_oracle_w ? c.d_oracle_w : ctx->raw0.as<float>() + 128 * w;
+  float* raw0 = linear ? nullptr : c.d_oracle_w ? c.d_oracle_w : ctx->raw0.as<float>() + 128 * w;
   const float* ray_o = ctx->ray_o.as<float>() + 3 * w;
   const float* ray_d = ctx->ray_d.as<float>() + 3 * w;
   int32_t* count = c.d_nsamples ? c.d_nsamples : ctx->count.as<int32_t>();
@@ -659,7 +689,9 @@ adn_status run_stages_2_5(adn_ctx* ctx, const RenderCall& c, int64_t w, const fl
   long long* total = ctx->total.as<long long>();
 
   // stage 2
-  if (fixed_k) {
+  if (linear) {
+    ADN_CUDA(ctx, launch_linear_sample(n, K, zlin_table(ctx, K), count, offset, rayidx, z, total, c.st));
+  } else if (fixed_k) {
     ADN_CUDA(ctx, launch_pdf_sample(raw0, n, K, ctx->pdf_transform, depth_base(ctx), ctx->scene.depth_range[0], count, offset,
                                     rayidx, z, total, c.st));
   } else if (dense) {
@@ -683,7 +715,8 @@ adn_status run_stages_2_5(adn_ctx* ctx, const RenderCall& c, int64_t w, const fl
   if (timing) cudaEventRecord(ctx->ev[5], c.st);
   // stage 5
   ADN_CUDA(ctx, launch_stage5(raw1, dense ? raw0 : ctx->zpbuf.as<float>(), z, ctx->zlut_dense.as<float>(), offset, count, n, K,
-                              dense ? 1 : 0, c.d_rgb, c.d_rgba8, stage5_aux(ctx, c.aux), c.st, fixed_k ? ray_d : nullptr));
+                              dense ? 1 : 0, c.d_rgb, c.d_rgba8, stage5_aux(ctx, c.aux), c.st,
+                              !fixed_k ? nullptr : linear && ctx->scene.use_ndc ? ctx->ray_dirs.as<float>() : ray_d));
   ctx->stats.kernel_launches++;
   if (timing) cudaEventRecord(ctx->ev[6], c.st);
   return ADN_OK;
@@ -711,10 +744,18 @@ adn_status render(adn_ctx* ctx, const RenderCall& call) {
   const bool joins = joins_group(ctx);   // an empty call still joins the selection's reductions
   if (!ctx || !call.pose || !call.rot || n_rays < 0 || (!call.d_rgb && !call.d_rgba8 && !(joins && n_rays == 0)))
     return fail(ctx, ADN_ERR_INVALID, "render: bad arguments");
-  if (!ctx->net[0].ready || !ctx->net[1].ready) return fail(ctx, ADN_ERR_NO_WEIGHTS, "render: set both networks first");
-  if (ctx->net[0].n_in != ctx->n_feat0 || ctx->net[0].n_out != 128)
+  const bool linear = ctx->sampler == 2;   // LinearlySpacedZNearZFar: one network, in the shading slot
+  if (linear && !ctx->net[1].ready) return fail(ctx, ADN_ERR_NO_WEIGHTS, "render: set the shading network (slot 1) first");
+  if (!linear && (!ctx->net[0].ready || !ctx->net[1].ready)) return fail(ctx, ADN_ERR_NO_WEIGHTS, "render: set both networks first");
+  if (!linear && (ctx->net[0].n_in != ctx->n_feat0 || ctx->net[0].n_out != 128))
     return fail(ctx, ADN_ERR_INVALID, "render: sampling net must be " + std::to_string(ctx->n_feat0) + " -> 128 for this scene's encoding");
-  const bool fixed_k = ctx->sampler == 1;   // FromClassifiedDepth ignores thr
+  if (linear && ctx->sampling_view)
+    return fail(ctx, ADN_ERR_INVALID, "render: sampler 2 (LinearlySpacedZNearZFar) runs no sampling net, so option sampling_view has nothing to draw");
+  if (linear && call.d_oracle_w)
+    return fail(ctx, ADN_ERR_INVALID, "render: sampler 2 (LinearlySpacedZNearZFar) runs no sampling net; pass d_oracle_weights = NULL");
+  if (linear && ctx->sample_budget > 0)
+    return fail(ctx, ADN_ERR_INVALID, "render: sampler 2 (LinearlySpacedZNearZFar) places K samples on every ray; it takes no sample_budget");
+  const bool fixed_k = ctx->sampler != 0;   // FromClassifiedDepth and LinearlySpacedZNearZFar ignore thr
   if (K < 1 || K > 128 || (!fixed_k && thr < 0.0f)) return fail(ctx, ADN_ERR_INVALID, "render: need 1 <= K <= 128 and thr >= 0");
   if (!fixed_k && thr == 0.0f && K != 128)
     return fail(ctx, ADN_ERR_INVALID, "render: dense mode (thr == 0) needs K == 128 (one sample per depth cell)");
@@ -729,7 +770,7 @@ adn_status render(adn_ctx* ctx, const RenderCall& call) {
   const int64_t budget = view ? 0 : ctx->sample_budget;   // the view selects no samples
   if (fixed_k && budget > 0)
     return fail(ctx, ADN_ERR_INVALID, "render: sampler 1 (FromClassifiedDepth) places K samples on every ray; it takes no sample_budget");
-  if (fixed_k && ctx->scene.use_ndc)
+  if (ctx->sampler == 1 && ctx->scene.use_ndc)
     return fail(ctx, ADN_ERR_INVALID, "render: sampler 1 (FromClassifiedDepth) is not supported on NDC scenes");
   if (budget > 0 && thr == 0.0f)
     return fail(ctx, ADN_ERR_INVALID, "render: sample_budget needs the adaptive path (thr > 0 is the floor threshold), not dense mode");
@@ -757,23 +798,27 @@ adn_status render(adn_ctx* ctx, const RenderCall& call) {
   }
   chunk = pad128(chunk);
   if (call.cam && chunk % call.cam->W) chunk = (chunk / call.cam->W + 1) * call.cam->W;  // whole rows per chunk
+  if (linear && std::min(chunk, n_rays) * K > INT32_MAX)
+    return fail(ctx, ADN_ERR_INVALID, "render: sampler 2 needs N * K < 2^31 per chunk (int32 offsets); lower option chunk_rays");
   ctx->stats.n_rays = n_rays;
   ctx->last_budget = budget > 0;
   ctx->last_thr = thr;
   ctx->last_view = view;
   if (ctx->profile) ctx->prof_budget = budget > 0;
   if (ctx->profile) ctx->prof_view = view;
+  if (ctx->profile) ctx->prof_linear = linear;
   // raw0 / ray_o / ray_d: one chunk's worth, or with a sample budget the whole call's (the threshold is chosen over all of
   // raw0 before any chunk runs stage 2)
   const int64_t span = budget > 0 ? n_rays : std::min(chunk, n_rays);
-  if (!call.d_oracle_w && (s = ensure(ctx, ctx->raw0, size_t(span) * 128 * 4)) != ADN_OK) return s;
+  if (!linear && !call.d_oracle_w && (s = ensure(ctx, ctx->raw0, size_t(span) * 128 * 4)) != ADN_OK) return s;
+  if (linear && ctx->scene.use_ndc && (s = ensure(ctx, ctx->ray_dirs, size_t(span) * 12)) != ADN_OK) return s;
   if ((s = ensure(ctx, ctx->ray_o, size_t(span) * 12)) != ADN_OK) return s;
   if ((s = ensure(ctx, ctx->ray_d, size_t(span) * 12)) != ADN_OK) return s;
   if (budget == 0) {
     for (int64_t r0 = 0; r0 < n_rays; r0 += chunk) {
       const RenderCall c = chunk_of(call, r0, chunk);
       const bool timing = ctx->profile && r0 == 0;
-      if ((s = run_stages_0_1(ctx, c, 0, timing)) != ADN_OK) return s;
+      if ((s = linear ? run_rays(ctx, c, timing) : run_stages_0_1(ctx, c, 0, timing)) != ADN_OK) return s;
       if ((s = view ? run_view(ctx, c, timing) : run_stages_2_5(ctx, c, 0, nullptr, timing)) != ADN_OK) return s;
     }
     return ADN_OK;
@@ -916,8 +961,16 @@ adn_status adn_create(adn_ctx** out, const adn_scene* scene, int device) {
     // FromClassifiedDepthAdaptiveNoDepthRange (NDC configs): the cell centre itself (nerf_raymarch_common.py:826-833)
     lut[i] = scene->use_ndc ? z : (w - 1.0f) + scene->depth_range[0];
   }
+  // sampler 2's depth tables, one per K, so that no render uploads one
+  std::vector<float> zlin;
+  for (int K = 1; K <= 128; ++K) {
+    const std::vector<float> t = linear_depths(*scene, K);
+    zlin.insert(zlin.end(), t.begin(), t.end());
+  }
   bool ok = ensure(ctx, ctx->zlut, sizeof(lut)) == ADN_OK &&
             cudaMemcpy(ctx->zlut.p, lut, sizeof(lut), cudaMemcpyHostToDevice) == cudaSuccess &&
+            ensure(ctx, ctx->zlin, zlin.size() * 4) == ADN_OK &&
+            cudaMemcpy(ctx->zlin.p, zlin.data(), zlin.size() * 4, cudaMemcpyHostToDevice) == cudaSuccess &&
             ensure(ctx, ctx->total, sizeof(long long)) == ADN_OK &&
             cudaMemset(ctx->total.p, 0, sizeof(long long)) == cudaSuccess &&
             cudaHostAlloc(&ctx->watchdog.p, sizeof(int), cudaHostAllocMapped) == cudaSuccess &&
@@ -948,6 +1001,9 @@ void adn_destroy(adn_ctx* ctx) {
 
 adn_status adn_set_weights(adn_ctx* ctx, int net_id, const adn_tensor_desc* tensors, int n_tensors) {
   if (!ctx || (net_id != 0 && net_id != 1) || !tensors || n_tensors < 1) return fail(ctx, ADN_ERR_INVALID, "set_weights: bad arguments");
+  if (net_id == 0 && ctx->sampler == 2)
+    return fail(ctx, ADN_ERR_INVALID, "set_weights: option sampler 2 (LinearlySpacedZNearZFar) runs no sampling network; "
+                                      "set sampler 0 or 1 first");
   ADN_CUDA(ctx, cudaSetDevice(ctx->device));
   ADN_CUDA(ctx, cudaDeviceSynchronize());
   Net& net = ctx->net[net_id];
@@ -989,8 +1045,15 @@ adn_status adn_set_option(adn_ctx* ctx, const char* name, int64_t value) {
     ctx->sampling_view = value != 0;
     return ADN_OK;
   }
-  if (n == "sampler") {   // 0 (default): FromClassifiedDepthAdaptive; 1: FromClassifiedDepth (DONeRF's fixed K samples per ray)
-    if (value != 0 && value != 1) return fail(ctx, ADN_ERR_INVALID, "sampler must be 0 (adaptive) or 1 (FromClassifiedDepth)");
+  if (n == "sampler") {   // 0 (default): FromClassifiedDepthAdaptive; 1: FromClassifiedDepth (DONeRF's fixed K samples per ray);
+                          // 2: LinearlySpacedZNearZFar (NeRF's K evenly spaced samples, no sampling net)
+    if (value < 0 || value > 2)
+      return fail(ctx, ADN_ERR_INVALID, "sampler must be 0 (adaptive), 1 (FromClassifiedDepth) or 2 (LinearlySpacedZNearZFar)");
+    // a context holding a sampling net belongs to a two-network run, whose shading net was trained on that net's samples:
+    // rendering it alone as a NeRF would ignore the sampling net and give a picture of nothing the run trained
+    if (value == 2 && ctx->net[0].ready)
+      return fail(ctx, ADN_ERR_INVALID, "sampler 2 (LinearlySpacedZNearZFar) renders one network from the shading slot, but this "
+                                        "context holds a sampling network (a two-network run); use a context without one");
     ctx->sampler = int(value);
     return ADN_OK;
   }
@@ -1036,7 +1099,7 @@ adn_status adn_get_stats(adn_ctx* ctx, adn_stats* out) {
   if (ctx->profile) {
     for (int i = 0; i < 6; ++i) {
       float ms = 0;
-      if (ctx->prof_view && i >= 2 && i <= 4) {   // the view runs no stages 2-4
+      if ((ctx->prof_view && i >= 2 && i <= 4) || (ctx->prof_linear && i == 1)) {   // the view runs no stages 2-4, sampler 2 no stage 1
         ctx->stats.ms_stage[i] = 0.0f;
         continue;
       }
@@ -1244,6 +1307,41 @@ adn_status adn_pdf_sample(adn_ctx* ctx, const float* d_raw0, int64_t n_rays, int
     ADN_CUDA(ctx, launch_pdf_sample(d_raw0, n_rays, K, transform, depth_base(ctx), ctx->scene.depth_range[0], d_count, d_offset,
                                     d_ray, d_z, nullptr, st));
     ctx->stats.kernel_launches++;
+  }
+  ADN_CUDA(ctx, cudaStreamSynchronize(st));
+  return ADN_OK;
+}
+
+adn_status adn_camera_rays(adn_ctx* ctx, const float* pose, const float* rot, const float* d_dirs, int64_t n_rays, float* d_ray_o,
+                           float* d_ray_d, float* d_ray_dirs) {
+  if (!ctx || !pose || !rot || n_rays < 0 || (n_rays > 0 && (!d_dirs || !d_ray_o || !d_ray_d)))
+    return fail(ctx, ADN_ERR_INVALID, "camera_rays: bad arguments (need pose, rot, d_dirs, d_ray_o and d_ray_d)");
+  if (ctx->scene.use_ndc && d_ray_dirs) {
+    if (ctx->scene.ndc_w <= 0 || ctx->scene.ndc_h <= 0)
+      return fail(ctx, ADN_ERR_INVALID, "camera_rays: the NDC directions need the scene's ndc_w / ndc_h");
+    set_ndc_projection(ctx, ctx->scene.ndc_w, ctx->scene.ndc_h, ctx->scene.ndc_focal);
+  }
+  if (n_rays == 0) return ADN_OK;
+  ADN_CUDA(ctx, cudaSetDevice(ctx->device));
+  const cudaStream_t st = ctx->own_stream;
+  {
+    CallOrder order(ctx, st);
+    if (adn_status s = order.begin("camera_rays"); s != ADN_OK) return s;
+    ADN_CUDA(ctx, launch_camera_rays(ctx->sc, make_pose(pose, rot), d_dirs, nullptr, n_rays, d_ray_o, d_ray_d, d_ray_dirs, st));
+    ctx->stats.kernel_launches++;
+  }
+  ADN_CUDA(ctx, cudaStreamSynchronize(st));
+  return ADN_OK;
+}
+
+adn_status adn_linear_depths(adn_ctx* ctx, int K, float* d_z) {
+  if (!ctx || K < 1 || K > 128 || !d_z) return fail(ctx, ADN_ERR_INVALID, "linear_depths: bad arguments (need 1 <= K <= 128 and d_z)");
+  ADN_CUDA(ctx, cudaSetDevice(ctx->device));
+  const cudaStream_t st = ctx->own_stream;
+  {
+    CallOrder order(ctx, st);
+    if (adn_status s = order.begin("linear_depths"); s != ADN_OK) return s;
+    ADN_CUDA(ctx, cudaMemcpyAsync(d_z, zlin_table(ctx, K), size_t(K) * 4, cudaMemcpyDeviceToDevice, st));
   }
   ADN_CUDA(ctx, cudaStreamSynchronize(st));
   return ADN_OK;
@@ -1463,6 +1561,7 @@ adn_status adn_create_from_export_dir(adn_ctx** out, const char* dir, int device
   adn_status s = adn_create(&ctx, &ex.scene, device);
   if (s != ADN_OK) return s;
   for (int id = 0; id < 2; ++id) {
+    if (ex.sampler == 2 && id == 0) continue;   // a one-network export: its net is in slot 1
     std::vector<adn_tensor_desc> descs;
     for (auto& t : ex.nets[id]) descs.push_back({t.name.c_str(), t.data.data(), t.rows, t.cols});
     s = adn_set_weights(ctx, id, descs.data(), int(descs.size()));
@@ -1472,8 +1571,9 @@ adn_status adn_create_from_export_dir(adn_ctx** out, const char* dir, int device
       return s;
     }
   }
-  if (ex.sampler == 1 && ((s = adn_set_option(ctx, "sampler", 1)) != ADN_OK ||
-                          (s = adn_set_option(ctx, "pdf_transform", ex.pdf_transform)) != ADN_OK)) {
+  if ((ex.sampler == 2 && (s = adn_set_option(ctx, "sampler", 2)) != ADN_OK) ||
+      (ex.sampler == 1 && ((s = adn_set_option(ctx, "sampler", 1)) != ADN_OK ||
+                           (s = adn_set_option(ctx, "pdf_transform", ex.pdf_transform)) != ADN_OK))) {
     std::fprintf(stderr, "adanerf_b200: %s\n", ctx->last_error.c_str());
     adn_destroy(ctx);
     return s;

@@ -185,11 +185,17 @@ bool load_export_dir(const std::string& dir_in, ExportDir& out, std::string& err
   }
   s.fov = fov;
   s.max_depth = md;
+  // A one-network export (plain NeRF: inFeatures = [RayMarchFromPoses], rayMarchSampler = [LinearlySpacedZNearZFar]) has
+  // one-item lists; its network is model0.onnx and goes to the shading slot
+  auto sm = cfg.find("rayMarchSampler");
+  const auto sitems = sm == cfg.end() ? std::vector<std::string>{} : list_items(sm->second);
+  const bool one_net = sitems.size() == 1;
+  const size_t n_nets = one_net ? 1 : 2;
   float zn[2] = {0.001f, 0.001f}, zf[2] = {1.0f, 1.0f};
-  floats_of(cfg, "zNear", zn, 2);
-  floats_of(cfg, "zFar", zf, 2);
-  s.z_near = zn[1];
-  s.z_far = zf[1];
+  floats_of(cfg, "zNear", zn, n_nets);
+  floats_of(cfg, "zFar", zf, n_nets);
+  s.z_near = zn[n_nets - 1];
+  s.z_far = zf[n_nets - 1];
   s.n_freq_pos = 10;
   s.n_freq_dir = 4;
   auto pe = cfg.find("posEncArgs");
@@ -258,9 +264,36 @@ bool load_export_dir(const std::string& dir_in, ExportDir& out, std::string& err
     const auto items = list_items(it->second);
     return items.empty() || items.back() == want;
   };
-  auto sm = cfg.find("rayMarchSampler");
-  const auto sitems = sm == cfg.end() ? std::vector<std::string>{} : list_items(sm->second);
-  if (!sitems.empty() && sitems.back() == "FromClassifiedDepth") {
+  auto value_of = [&](const char* key) {
+    auto it = cfg.find(key);
+    return it == cfg.end() ? std::string("(missing)") : strip(it->second);
+  };
+  if (one_net) {
+    // LinearlySpacedZNearZFar (src/nerf_raymarch_common.py:293-326; NoDepthRange on NDC scenes, :261-289): K evenly spaced
+    // samples from the camera, one NeRF net, the density composite (features.py:564-577).  The depths are warped with
+    // dataset_info.txt's depth_range, as the viewer does: src/export.py:50 writes the warped range there, while a Python run
+    // without SpherePosDir places them with the dataset's unwarped range (datasets.py:154-159); see INTEGRATION.md.
+    auto inf = cfg.find("inFeatures");
+    const auto fitems = inf == cfg.end() ? std::vector<std::string>{} : list_items(inf->second);
+    if (fitems.size() != 1 || fitems[0] != "RayMarchFromPoses") {
+      err = "config.ini: a one-network export needs inFeatures = [RayMarchFromPoses], not " + value_of("inFeatures");
+      return false;
+    }
+    if (s.use_ndc) {
+      if (sitems[0] != "LinearlySpacedZNearZFarNoDepthRange" || !check("rayMarchNormalization", "None")) {
+        err = "config.ini: a one-network NDC export must use rayMarchSampler = [LinearlySpacedZNearZFarNoDepthRange] and "
+              "rayMarchNormalization = [None], not " + value_of("rayMarchSampler") + " / " + value_of("rayMarchNormalization");
+        return false;
+      }
+    } else if (sitems[0] != "LinearlySpacedZNearZFar" || !check("rayMarchNormalization", "InverseSqrtDistCentered") ||
+               !check("depthTransform", "log")) {
+      err = "config.ini: a one-network export must use rayMarchSampler = [LinearlySpacedZNearZFar], rayMarchNormalization = "
+            "[InverseSqrtDistCentered] and depthTransform = log (or LinearlySpacedZNearZFarNoDepthRange / None with useNDC), not " +
+            value_of("rayMarchSampler") + " / " + value_of("rayMarchNormalization") + " / " + value_of("depthTransform");
+      return false;
+    }
+    out.sampler = 2;
+  } else if (!sitems.empty() && sitems.back() == "FromClassifiedDepth") {
     // FromClassifiedDepth (the DONeRF sampler, src/nerf_raymarch_common.py:606-660) returns z only, so the composite is
     // nerf_raw2outputs without OracleWeights and accumulationMult does not apply; its transform of raw0 is chosen by
     // losses[0] (:625-637)
@@ -293,12 +326,16 @@ bool load_export_dir(const std::string& dir_in, ExportDir& out, std::string& err
     err = "config.ini: only FromClassifiedDepthAdaptive / InverseSqrtDistCentered / log / alpha exports are supported";
     return false;
   }
-  for (int i = 0; i < 2; ++i)
-    if (!read_onnx_initializers(dir + "model" + std::to_string(i) + ".onnx", out.nets[i], err)) return false;
+  if (one_net) {
+    if (!read_onnx_initializers(dir + "model0.onnx", out.nets[1], err)) return false;
+  } else {
+    for (int i = 0; i < 2; ++i)
+      if (!read_onnx_initializers(dir + "model" + std::to_string(i) + ".onnx", out.nets[i], err)) return false;
+  }
   // The networks' shapes come from the initialisers.  config.ini's layers / layerWidth (src/util/config.py:55-56), when
   // present, must describe the same networks: depth = the number of layers.{i} / pts_linears.{i} weights, width = the
   // input columns of layers.1 (the rows of layers.0 of a one-layer net) / of alpha_linear.
-  for (int i = 0; i < 2; ++i) {
+  for (int i = one_net ? 1 : 0; i < 2; ++i) {
     const std::string prefix = i == 0 ? "layers." : "pts_linears.";
     int depth = 0, width = 0, width0 = 0;
     for (const NamedTensor& t : out.nets[i]) {
@@ -311,13 +348,13 @@ bool load_export_dir(const std::string& dir_in, ExportDir& out, std::string& err
       if (i == 0 && idx == 1) width = int(t.cols);
     }
     if (i == 0 && depth == 1) width = width0;
-    const std::string onnx = "model" + std::to_string(i) + ".onnx";
+    const std::string onnx = one_net ? "model0.onnx" : "model" + std::to_string(i) + ".onnx";
     for (const auto& [key, have] : {std::pair<const char*, int>{"layers", depth}, {"layerWidth", width}}) {
       auto it = cfg.find(key);
       if (it == cfg.end()) continue;
       const auto items = list_items(it->second);
-      if (items.size() != 2) continue;
-      const int want = std::atoi(items[size_t(i)].c_str());
+      if (items.size() != n_nets) continue;
+      const int want = std::atoi(items[one_net ? 0 : size_t(i)].c_str());
       if (want != have) {
         err = "config.ini: " + std::string(key) + " = " + strip(it->second) + " but " + onnx + " holds a network with " + key + " " +
               std::to_string(have);

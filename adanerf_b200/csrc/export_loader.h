@@ -21,9 +21,10 @@ struct ExportDir {
   adn_scene scene{};
   float threshold = 0.0f;  // adaptiveSamplingThreshold
   int num_samples = 0;     // numRaymarchSamples[1]
-  int sampler = 0;         // rayMarchSampler[1]: 0 = FromClassifiedDepthAdaptive(NoDepthRange), 1 = FromClassifiedDepth
+  int sampler = 0;         // rayMarchSampler[1]: 0 = FromClassifiedDepthAdaptive(NoDepthRange), 1 = FromClassifiedDepth;
+                           // 2 = a one-network export, rayMarchSampler = [LinearlySpacedZNearZFar(NoDepthRange)]
   int pdf_transform = 0;   // sampler 1: 1 = sigmoid, 2 = softmax (from losses[0])
-  std::vector<NamedTensor> nets[2];
+  std::vector<NamedTensor> nets[2];   // sampler 2: nets[0] empty, model0.onnx in nets[1]
 };
 
 bool read_onnx_initializers(const std::string& path, std::vector<NamedTensor>& out, std::string& err);

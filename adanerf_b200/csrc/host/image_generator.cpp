@@ -7,8 +7,11 @@ namespace adn_host {
 bool Config::load(const std::string& dir) {
   model_dir = dir;
   int n[2] = {0, 0};
-  return adn_probe_export_dir(dir.c_str(), &scene, &adaptiveSamplingThreshold, &numRaymarchSamples, n) == ADN_OK && n[0] > 0 &&
-         n[1] > 0;
+  // a one-network export (LinearlySpacedZNearZFar) has its net in the shading slot and none in the sampling slot
+  if (adn_probe_export_dir(dir.c_str(), &scene, &adaptiveSamplingThreshold, &numRaymarchSamples, n) != ADN_OK || n[1] <= 0)
+    return false;
+  one_network = n[0] == 0;
+  return true;
 }
 
 void Camera::rotation(float rot[9]) const {

@@ -26,6 +26,7 @@ struct Config {
   float adaptiveSamplingThreshold = 0.f;
   int numRaymarchSamples = 0;
   std::string model_dir;
+  bool one_network = false;            // a NeRF export with no sampling net (rayMarchSampler = [LinearlySpacedZNearZFar])
   bool load(const std::string& dir);   // parses config.ini + dataset_info.txt + model{0,1}.onnx headers
 };
 

@@ -41,6 +41,11 @@ int main(int argc, char** argv) {
   adn_host::Config config;
   if (!config.load(model)) { std::fprintf(stderr, "couldn't read export directory %s\n", model.c_str()); return 1; }
   std::printf("model %s: K = %d, adaptiveSamplingThreshold = %g\n", model.c_str(), config.numRaymarchSamples, config.adaptiveSamplingThreshold);
+  if (config.one_network && (oracle || budget > 0)) {
+    std::fprintf(stderr, "%s is a one-network export (LinearlySpacedZNearZFar): it has no sampling network to view (--oracle) "
+                 "and places K samples on every ray (--budget)\n", model.c_str());
+    return 2;
+  }
   // -w: the last frame as a binary PPM in the model directory, saturate(x) * 255 truncated (the viewer's pixels)
   auto write_ppm = [&](const std::vector<float>& rgb) {
     const std::string out = model + "/adn_frame.ppm";

@@ -119,6 +119,7 @@ adn_status adn_multi_create_from_export_dir(adn_multi** out, const char* dir, co
   adn_status s = adn_multi_create(out, &ex.scene, devices, n_devices);
   if (s != ADN_OK) return s;
   for (int id = 0; id < 2; ++id) {
+    if (ex.sampler == 2 && id == 0) continue;   // a one-network export: its net is in slot 1
     std::vector<adn_tensor_desc> descs;
     for (auto& t : ex.nets[id]) descs.push_back({t.name.c_str(), t.data.data(), t.rows, t.cols});
     s = adn_multi_set_weights(*out, id, descs.data(), int(descs.size()));
@@ -130,8 +131,10 @@ adn_status adn_multi_create_from_export_dir(adn_multi** out, const char* dir, co
     }
   }
   // a FromClassifiedDepth export: every band renders with the fixed-K sampler and the export's transform
-  if (ex.sampler == 1 && ((s = adn_multi_set_option(*out, "sampler", 1)) != ADN_OK ||
-                          (s = adn_multi_set_option(*out, "pdf_transform", ex.pdf_transform)) != ADN_OK)) {
+  // a LinearlySpacedZNearZFar export: every band renders K evenly spaced samples with the one network
+  if ((ex.sampler == 2 && (s = adn_multi_set_option(*out, "sampler", 2)) != ADN_OK) ||
+      (ex.sampler == 1 && ((s = adn_multi_set_option(*out, "sampler", 1)) != ADN_OK ||
+                           (s = adn_multi_set_option(*out, "pdf_transform", ex.pdf_transform)) != ADN_OK))) {
     std::fprintf(stderr, "adanerf_b200: %s\n", (*out)->err.c_str());
     adn_multi_destroy(*out);
     *out = nullptr;

@@ -64,6 +64,28 @@ __device__ __forceinline__ void posenc3_rt(const float (&v)[3], int L, Emit emit
   }
 }
 
+// ndc_rays(H, W, focal, near = 1) (src/nerf_raymarch_common.py:71-88) of one ray in the reference's operation order:
+// origin o and direction d -> the NDC origin oo and the un-normalised NDC direction dd.
+__device__ __forceinline__ void ndc_ray(const SceneDev& sc, const float (&o)[3], const float (&d)[3], float (&oo)[3],
+                                        float (&dd)[3]) {
+  const float t = __fdiv_rn(-__fadd_rn(1.0f, o[2]), d[2]);
+  float on[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) on[a] = __fadd_rn(o[a], __fmul_rn(t, d[a]));
+  const float q0 = __fdiv_rn(on[0], on[2]), q1 = __fdiv_rn(on[1], on[2]);
+  oo[0] = __fdiv_rn(__fmul_rn(sc.ndc_cw, on[0]), on[2]);
+  oo[1] = __fdiv_rn(__fmul_rn(sc.ndc_ch, on[1]), on[2]);
+  oo[2] = __fadd_rn(1.0f, __fdiv_rn(2.0f, on[2]));
+  dd[0] = __fmul_rn(sc.ndc_cw, __fsub_rn(__fdiv_rn(d[0], d[2]), q0));
+  dd[1] = __fmul_rn(sc.ndc_ch, __fsub_rn(__fdiv_rn(d[1], d[2]), q1));
+  dd[2] = __fdiv_rn(-2.0f, on[2]);
+}
+
+// torch.norm(v, dim=-1) of a 3-vector in fp32: sqrt((x x + y y) + z z).
+__device__ __forceinline__ float norm3(const float (&v)[3]) {
+  return __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(v[0], v[0]), __fmul_rn(v[1], v[1])), __fmul_rn(v[2], v[2])));
+}
+
 // The shading net's inputs of one sample at world depth zw on ray r (RayMarchFromPoses.batch, src/features.py:458-479), in
 // the reference's operation order: the position into pos and the direction to encode into dir.  Stage 3 and the fused
 // encoder both call this, so their features are the same bits.
@@ -77,26 +99,15 @@ __device__ __forceinline__ void sample_inputs(const SceneDev& sc, bool ndc, cons
     dir[a] = __ldg(ray_d + 3 * r + a);   // un-normalised nds, as SpherePosDir hands it on
   }
   if (ndc) {
-    // ndc_rays(H, W, focal, near = 1) (src/nerf_raymarch_common.py:71-88) in the reference's operation order, then
-    // pos = o' + d' z with the un-normalised NDC direction, no position normalisation, view encoding of d' / |d'|
-    const float t = __fdiv_rn(-__fadd_rn(1.0f, o[2]), dir[2]);
-    float on[3];
+    // ndc_rays, then pos = o' + d' z with the un-normalised NDC direction, no position normalisation, view encoding of
+    // d' / |d'|
+    float oo[3], dd[3];
+    ndc_ray(sc, o, dir, oo, dd);
 #pragma unroll
-    for (int a = 0; a < 3; ++a) on[a] = __fadd_rn(o[a], __fmul_rn(t, dir[a]));
-    const float q0 = __fdiv_rn(on[0], on[2]), q1 = __fdiv_rn(on[1], on[2]);
-    const float o0 = __fdiv_rn(__fmul_rn(sc.ndc_cw, on[0]), on[2]);
-    const float o1 = __fdiv_rn(__fmul_rn(sc.ndc_ch, on[1]), on[2]);
-    const float o2 = __fadd_rn(1.0f, __fdiv_rn(2.0f, on[2]));
-    const float d0 = __fmul_rn(sc.ndc_cw, __fsub_rn(__fdiv_rn(dir[0], dir[2]), q0));
-    const float d1 = __fmul_rn(sc.ndc_ch, __fsub_rn(__fdiv_rn(dir[1], dir[2]), q1));
-    const float d2 = __fdiv_rn(-2.0f, on[2]);
-    pos[0] = __fadd_rn(o0, __fmul_rn(d0, zw));                                                    // :458
-    pos[1] = __fadd_rn(o1, __fmul_rn(d1, zw));
-    pos[2] = __fadd_rn(o2, __fmul_rn(d2, zw));
-    const float dn = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(d0, d0), __fmul_rn(d1, d1)), __fmul_rn(d2, d2)));
-    dir[0] = __fdiv_rn(d0, dn);                                                                   // :431
-    dir[1] = __fdiv_rn(d1, dn);
-    dir[2] = __fdiv_rn(d2, dn);
+    for (int a = 0; a < 3; ++a) pos[a] = __fadd_rn(oo[a], __fmul_rn(dd[a], zw));                 // :458
+    const float dn = norm3(dd);
+#pragma unroll
+    for (int a = 0; a < 3; ++a) dir[a] = __fdiv_rn(dd[a], dn);                                    // :431
   } else {
 #pragma unroll
     for (int a = 0; a < 3; ++a) pos[a] = __fsub_rn(__fadd_rn(o[a], __fmul_rn(dir[a], zw)), sc.c[a]);   // :458, loc = pos - c

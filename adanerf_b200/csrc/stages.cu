@@ -49,6 +49,14 @@ cudaError_t launch_gen_dirs(const CameraRays& cam, long long n_rays, float* d_di
 }
 
 // ------------------------------------------------------------------------------------ stage 0b
+// nds = R * d : ATen bmm with K = 3 accumulates as an FMA chain over k = 0,1,2 (src/features.py:858-859, and
+// nerf_get_ray_dirs, src/nerf_raymarch_common.py:147-152)
+__device__ __forceinline__ void rotate_dir(const PoseDev& pd, const float (&d)[3], float (&nds)[3]) {
+#pragma unroll
+  for (int r = 0; r < 3; ++r)
+    nds[r] = __fmaf_rn(pd.rot[3 * r + 2], d[2], __fmaf_rn(pd.rot[3 * r + 1], d[1], __fmul_rn(pd.rot[3 * r + 0], d[0])));
+}
+
 // SpherePosDir.batch (src/features.py:845-899) up to the encodings: the pixel direction d of ray i, the ray origin p on the
 // view-cell sphere, the rotated direction nds and its unit copy dn.
 template <bool FROM_CAMERA>
@@ -62,10 +70,7 @@ __device__ __forceinline__ void sphere_pos_dir(const SceneDev& sc, const PoseDev
     d[1] = dirs[3 * i + 1];
     d[2] = dirs[3 * i + 2];
   }
-  // nds = R * d : ATen bmm with K = 3 accumulates as an FMA chain over k = 0,1,2 (:858-859)
-#pragma unroll
-  for (int r = 0; r < 3; ++r)
-    nds[r] = __fmaf_rn(pd.rot[3 * r + 2], d[2], __fmaf_rn(pd.rot[3 * r + 1], d[1], __fmul_rn(pd.rot[3 * r + 0], d[0])));
+  rotate_dir(pd, d, nds);
   // compute_ray_offset (:769-791)
   float omc[3];
 #pragma unroll
@@ -176,6 +181,52 @@ cudaError_t launch_stage0(const SceneDev& sc, const PoseDev& pd, const float* d_
   if (sc.n_freq_pos0 == kNFreqPos && sc.n_freq_dir0 == kNFreqDir) return run(stage0_kernel<true>, stage0_kernel<false>, attr104);
   if (sc.n_freq_pos0 == 2 && sc.n_freq_dir0 == 2) return run(stage0_kernel<true, 2, 2>, stage0_kernel<false, 2, 2>, attr22);
   return run(stage0_rt_kernel<true>, stage0_rt_kernel<false>, attr_rt);
+}
+
+// ------------------------------------------------------------------------------------ camera rays (sampler 2)
+// RayMarchFromPoses.batch's rays when no sampling net runs (src/features.py:417-431): rays_d = R d as nerf_get_ray_dirs'
+// bmm forms it (not renormalised) and rays_o = pose.  ray_dirs (may be null) gets the directions whose norm
+// nerf_raw2outputs scales its distances by: rays_d itself, or on NDC scenes ndc_rays' un-normalised direction (what
+// RayMarchFromPoses.postprocess hands it, not the unit copy that is encoded).  12 B in (or the pixel's direction from cam),
+// 24 B out per ray, 36 B with ray_dirs.
+template <bool FROM_CAMERA>
+__global__ void __launch_bounds__(256)
+camera_rays_kernel(const __grid_constant__ SceneDev sc, const __grid_constant__ PoseDev pd, const float* __restrict__ dirs,
+                   const __grid_constant__ CameraRays cam, long long n_rays, float* __restrict__ ray_o, float* __restrict__ ray_d,
+                   float* __restrict__ ray_dirs) {
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i >= n_rays) return;
+  float d[3], nds[3];
+  if (FROM_CAMERA) {
+    pixel_dir(cam, i, d);
+  } else {
+#pragma unroll
+    for (int a = 0; a < 3; ++a) d[a] = __ldg(dirs + 3 * i + a);
+  }
+  rotate_dir(pd, d, nds);
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    ray_o[3 * i + a] = pd.pose[a];
+    ray_d[3 * i + a] = nds[a];
+  }
+  if (ray_dirs) {
+    float v[3] = {nds[0], nds[1], nds[2]};
+    if (sc.ndc) {   // :430
+      float oo[3];
+      ndc_ray(sc, pd.pose, nds, oo, v);
+    }
+#pragma unroll
+    for (int a = 0; a < 3; ++a) ray_dirs[3 * i + a] = v[a];
+  }
+}
+
+cudaError_t launch_camera_rays(const SceneDev& sc, const PoseDev& pd, const float* d_dirs, const CameraRays* cam,
+                               long long n_rays, float* d_ray_o, float* d_ray_d, float* d_ray_dirs, cudaStream_t s) {
+  if (n_rays <= 0) return cudaSuccess;
+  const unsigned grid = unsigned((n_rays + 255) / 256);
+  if (cam) camera_rays_kernel<true><<<grid, 256, 0, s>>>(sc, pd, d_dirs, *cam, n_rays, d_ray_o, d_ray_d, d_ray_dirs);
+  else camera_rays_kernel<false><<<grid, 256, 0, s>>>(sc, pd, d_dirs, CameraRays{}, n_rays, d_ray_o, d_ray_d, d_ray_dirs);
+  return cudaGetLastError();
 }
 
 // ------------------------------------------------------------------------------------- stage 2
@@ -938,6 +989,30 @@ cudaError_t launch_stage2_dense(long long n_rays, int K, int32_t* d_count, int32
                                 cudaStream_t s) {
   const long long n = n_rays > 0 ? n_rays : 1;
   stage2_dense_kernel<<<unsigned((n + 255) / 256), 256, 0, s>>>(n_rays, K, d_count, d_offset, d_total);
+  return cudaGetLastError();
+}
+
+// LinearlySpacedZNearZFar(NoDepthRange).generate with det = True (src/nerf_raymarch_common.py:276-326): every ray takes
+// the same K depths zt [K].  One thread per sample (N K < 2^31), in pdf_sample_kernel's packed layout.
+__global__ void __launch_bounds__(256)
+linear_sample_kernel(int n_rays, int K, const float* __restrict__ zt, int32_t* __restrict__ count, int32_t* __restrict__ offset,
+                     int32_t* __restrict__ ray, float* __restrict__ z, long long* __restrict__ total) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i == 0 && total) *total = (long long)n_rays * K;
+  if (i >= n_rays * K) return;
+  const int r = i / K, k = i - r * K;
+  z[i] = __ldg(zt + k);
+  if (ray) ray[i] = r;
+  if (k == 0) {
+    if (count) count[r] = K;
+    if (offset) offset[r] = i;
+  }
+}
+
+cudaError_t launch_linear_sample(long long n_rays, int K, const float* d_zt, int32_t* d_count, int32_t* d_offset, int32_t* d_ray,
+                                 float* d_z, long long* d_total, cudaStream_t s) {
+  const long long n = n_rays * K > 0 ? n_rays * K : 1;   // an empty call still writes *d_total = 0
+  linear_sample_kernel<<<unsigned((n + 255) / 256), 256, 0, s>>>(int(n_rays), K, d_zt, d_count, d_offset, d_ray, d_z, d_total);
   return cudaGetLastError();
 }
 

@@ -33,6 +33,11 @@ cudaError_t launch_gen_dirs(const CameraRays& cam, long long n_rays, float* d_di
 cudaError_t launch_stage0(const SceneDev& sc, const PoseDev& pd, const float* d_dirs, const CameraRays* cam,
                           long long n_rays, float* d_x0, float* d_ray_o, float* d_ray_d, uint8_t* d_tiles0, int tile_terms,
                           cudaStream_t s);
+// The rays of a render without a sampling net (option "sampler" 2): d_ray_o [N,3] = pose, d_ray_d [N,3] = R d (the FMA
+// chain of stage 0), from d_dirs or, when cam is given, the pixels' directions.  d_ray_dirs (may be null): the directions
+// whose norm nerf_raw2outputs scales its distances by, R d or on NDC scenes (sc.ndc) ndc_rays' un-normalised direction.
+cudaError_t launch_camera_rays(const SceneDev& sc, const PoseDev& pd, const float* d_dirs, const CameraRays* cam,
+                               long long n_rays, float* d_ray_o, float* d_ray_d, float* d_ray_dirs, cudaStream_t s);
 
 // Stage 2.  tile_state: [n_ctas + 2] uint64 scratch zeroed by the launcher (memsetAsync).
 size_t stage2_scratch_bytes(long long n_rays);
@@ -71,6 +76,11 @@ cudaError_t launch_budget_threshold(const float* d_raw0, long long n_rays, float
 // Dense (thr == 0): count = K, offset = ray*K, total = N*K; no index arrays are materialised.
 cudaError_t launch_stage2_dense(long long n_rays, int K, int32_t* d_count, int32_t* d_offset, long long* d_total,
                                 cudaStream_t s);
+// Linear placement (option "sampler" 2, LinearlySpacedZNearZFar): every ray takes the K depths d_zt [K].  Writes the layout
+// of launch_pdf_sample: count = K, offset = r K, ray [N K] = r, z [N K] and *d_total = N K; d_count, d_offset, d_ray and
+// d_total may be null (not written).  N K < 2^31.
+cudaError_t launch_linear_sample(long long n_rays, int K, const float* d_zt, int32_t* d_count, int32_t* d_offset, int32_t* d_ray,
+                                 float* d_z, long long* d_total, cudaStream_t s);
 
 // Fixed-K sampler (rayMarchSampler FromClassifiedDepth, the DONeRF baseline): per ray the inverse CDF of the transformed
 // raw0 [n_rays, 128] at K + 2 evenly spaced u, the first and last dropped, warped to world depth.  transform: 1 = sigmoid,

@@ -148,11 +148,17 @@ def net_shapes(sd0, sd1):
         while f"{prefix}{d}.weight" in sd:
             d += 1
         return d
-    d0, d1 = depth(sd0, "layers."), depth(sd1, "pts_linears.")
-    w0, w1 = int(sd0["layers.0.weight"].shape[0]), int(sd1["pts_linears.0.weight"].shape[0])
-    p = int(sd1["pts_linears.0.weight"].shape[1])
+    return (depth(sd0, "layers."), int(sd0["layers.0.weight"].shape[0]), -1), shading_shape(sd1)
+
+
+def shading_shape(sd1):
+    """(D, W, skip) of a NeRF net, as net_shapes reads the shading net."""
+    d1 = 0
+    while f"pts_linears.{d1}.weight" in sd1:
+        d1 += 1
+    w1, p = int(sd1["pts_linears.0.weight"].shape[0]), int(sd1["pts_linears.0.weight"].shape[1])
     skips = [i - 1 for i in range(1, d1) if int(sd1[f"pts_linears.{i}.weight"].shape[1]) == w1 + p]
-    return (d0, w0, -1), (d1, w1, skips[0] if skips else -1)
+    return d1, w1, skips[0] if skips else -1
 
 
 def _skips_entry(depth, skip):
@@ -185,8 +191,8 @@ PDF_TRANSFORMS = {"BCEWithLogitsLoss": 1, "CrossEntropyLoss": 2, "CrossEntropyLo
 
 def export_sampler(path):
     """(sampler, pdf_transform) of an export directory's config.ini, as adn_create_from_export_dir sets options "sampler" and
-    "pdf_transform": (0, None) for the adaptive samplers, (1, 1 or 2) for FromClassifiedDepth.  Raises ValueError for a
-    FromClassifiedDepth run whose losses[0] selects no transform."""
+    "pdf_transform": (0, None) for the adaptive samplers, (1, 1 or 2) for FromClassifiedDepth, (2, None) for a one-network
+    LinearlySpacedZNearZFar export.  Raises ValueError for a FromClassifiedDepth run whose losses[0] selects no transform."""
     import os
     cfg = {}
     with open(os.path.join(path, "config.ini")) as f:
@@ -194,6 +200,8 @@ def export_sampler(path):
             if "=" in line and not line.lstrip().startswith(("#", ";")):
                 k, v = line.split("=", 1)
                 cfg[k.strip()] = [x.strip() for x in v.strip().strip("[]").split(",")]
+    if len(cfg.get("rayMarchSampler", [])) == 1:
+        return 2, None
     if cfg.get("rayMarchSampler", [""])[-1] != "FromClassifiedDepth":
         return 0, None
     loss0 = cfg.get("losses", [""])[0]
@@ -244,3 +252,36 @@ def write_export_dir(path, scene, sd0, sd1, thr, K, sampler="FromClassifiedDepth
             if sampler == "FromClassifiedDepth":
                 f.write(f"losses = [{sampling_loss}, MSE]\n")
         f.write(f"activation = [relu, nerf]\nlayers = [{d0}, {d1}]\nlayerWidth = [{w0}, {w1}]\nskips = [, {_skips_entry(d1, skip)}]\n")
+
+
+def write_nerf_export_dir(path, scene, sd, K):
+    """Writes {config.ini, dataset_info.txt, model0.onnx} of a one-network run (plain NeRF: inFeatures =
+    [RayMarchFromPoses], rayMarchSampler = [LinearlySpacedZNearZFar], or on NDC scenes [LinearlySpacedZNearZFarNoDepthRange]
+    with rayMarchNormalization [None]), config.ini with one-item lists.  sd: the NeRF net (pts_linears.*).  The scene's
+    depth_range goes to dataset_info.txt as it is: the renderer warps the depths with it (see INTEGRATION.md on which range
+    a run uses)."""
+    import os
+    os.makedirs(path, exist_ok=True)
+    d1, w1, skip = shading_shape(sd)
+    write_onnx_initializers(os.path.join(path, "model0.onnx"),
+                            {k: (v.detach().cpu().numpy() if hasattr(v, "detach") else np.asarray(v)) for k, v in sd.items()})
+    ndc = bool(scene.get("use_ndc"))
+    with open(os.path.join(path, "dataset_info.txt"), "w") as f:
+        f.write(f"view_cell_center = {list(scene['view_cell_center'])}\n")
+        f.write(f"view_cell_size = {list(scene['view_cell_size'])}\n")
+        f.write(f"depth_range = {list(scene['depth_range'])}\n")
+        f.write(f"fov = {scene['fov']}\nfocal = 0.0\ncamera_scale = 1.0\nmax_depth = {scene['max_depth']}\n")
+        if ndc and scene.get("w") and scene.get("h"):
+            f.write(f"w = {int(scene['w'])}\nh = {int(scene['h'])}\n")
+    pos_enc, pos_enc_args = (e.strip("[]").split(", ")[-1] for e in _enc_entries(scene))
+    zn, zf = float(scene.get("z_near", 0.001)), float(scene.get("z_far", 1.0))
+    with open(os.path.join(path, "config.ini"), "w") as f:
+        f.write(f"posEnc = [{pos_enc}]\nposEncArgs = [{pos_enc_args}]\ninFeatures = [RayMarchFromPoses]\noutFeatures = [RGBARayMarch]\n")
+        if ndc:
+            f.write("rayMarchSampler = [LinearlySpacedZNearZFarNoDepthRange]\nrayMarchNormalization = [None]\nuseNDC = True\n"
+                    "depthTransform = linear\n")
+        else:
+            f.write("rayMarchSampler = [LinearlySpacedZNearZFar]\nrayMarchNormalization = [InverseSqrtDistCentered]\n"
+                    "depthTransform = log\n")
+        f.write(f"numRaymarchSamples = [{K}]\nzNear = [{zn}]\nzFar = [{zf}]\nactivation = [nerf]\nlosses = [MSE]\n"
+                f"layers = [{d1}]\nlayerWidth = [{w1}]\nskips = [{_skips_entry(d1, skip)}]\n")

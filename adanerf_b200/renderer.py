@@ -64,7 +64,8 @@ def _state_dict_of(net):
 
 class Renderer:
     """One context per device.  `sampling_net` / `shading_net`: nn.Module or state_dict with the
-    reference's parameter names (src/models.py:71-76, :226-244)."""
+    reference's parameter names (src/models.py:71-76, :226-244).  A plain NeRF (rayMarchSampler LinearlySpacedZNearZFar) has
+    no sampling net: pass its network as shading_net and set option "sampler" to 2."""
 
     def __init__(self, scene, device=0, sampling_net=None, shading_net=None, _handle=None):
         self.lib = _lib.load_library()
@@ -90,7 +91,8 @@ class Renderer:
     def from_export_dir(cls, path, device=0):
         """Loads the reference's export directory (src/export.py:28-93). Returns (renderer, thr, K).  A FromClassifiedDepth
         export comes back with options "sampler" = 1 and its "pdf_transform" set (export_sampler reads them from
-        config.ini); its thr is not used."""
+        config.ini); its thr is not used.  A one-network LinearlySpacedZNearZFar export comes back with its net in the
+        shading slot and option "sampler" = 2."""
         lib = _lib.load_library()
         h, thr, k = C.c_void_p(), C.c_float(), C.c_int()
         st = lib.adn_create_from_export_dir(C.byref(h), str(path).encode(), int(device), C.byref(thr), C.byref(k))
@@ -457,6 +459,30 @@ class Renderer:
                                                               out["rgb"].data_ptr(), out["rgba8"].data_ptr() if rgba8 else None,
                                                               C.byref(a)))
         return out
+
+    def camera_rays(self, pose, rot, dirs, want_ray_dirs=True):
+        """The rays of option "sampler" = 2 (adn_camera_rays): dirs [N,3] -> dict(ray_o [N,3] = pose, ray_d [N,3] = R d,
+        which stage3 reads, and ray_dirs [N,3], the directions whose norm stage5_density scales its distances by: ray_d, or
+        on NDC scenes ndc_rays' un-normalised direction).  Waits for the current stream first, like pdf_sample."""
+        p, r = self._pose_rot(pose, rot)
+        d = self._f32(dirs).reshape(-1, 3)
+        n, dev = d.shape[0], self._dev()
+        out = {k: torch.empty((n, 3), dtype=torch.float32, device=dev) for k in ("ray_o", "ray_d")}
+        out["ray_dirs"] = torch.empty((n, 3), dtype=torch.float32, device=dev) if want_ray_dirs else None
+        with torch.cuda.device(self.device):
+            torch.cuda.current_stream().synchronize()
+            self._check(self.lib.adn_camera_rays(self.handle, _fptr(p), _fptr(r), d.data_ptr(), n, out["ray_o"].data_ptr(),
+                                                 out["ray_d"].data_ptr(), out["ray_dirs"].data_ptr() if want_ray_dirs else None))
+        return out
+
+    def linear_depths(self, K):
+        """The K depths option "sampler" = 2 places on every ray (adn_linear_depths) -> [K] float32 on the device.  Waits for
+        the current stream first, like pdf_sample."""
+        z = torch.empty((int(K),), dtype=torch.float32, device=self._dev())
+        with torch.cuda.device(self.device):
+            torch.cuda.current_stream().synchronize()
+            self._check(self.lib.adn_linear_depths(self.handle, int(K), z.data_ptr()))
+        return z
 
     def budget_threshold(self, raw0, thr_min, K, max_samples, out=None):
         """raw0 [N,128] -> [1] float32 device tensor: the smallest threshold >= thr_min at which stage 2 with K samples per

@@ -161,7 +161,19 @@ adn_status adn_probe_export_dir(const char* dir, adn_scene* scene_out, float* th
  *   pdf_transform(raw0) (nerf_sample_pdf, det = True, :160-192) and composites them with nerf_raw2outputs (:19-68):
  *   alpha = 1 - exp(-relu(a) dist), dist = (z[k+1] - z[k], last 1e10) * |rays_d|.  `thr` is ignored; 1 <= K <= 128;
  *   d_nsamples receives K for every ray; z_vals is never NaN; "sample_budget" > 0 and NDC scenes fail with
- *   ADN_ERR_INVALID; "sampling_view" works as in the adaptive mode (it reads raw0 only)),
+ *   ADN_ERR_INVALID; "sampling_view" works as in the adaptive mode (it reads raw0 only);
+ *   2 = LinearlySpacedZNearZFar, NeRF with no sampling network (src/features.py:417-479,564-577): only the shading slot
+ *   (adn_set_weights net 1, pts_linears.*) is used.  It is a one-network context: setting sampler 2 fails with
+ *   ADN_ERR_INVALID while the sampling slot holds a network (the shading net of a two-network run is not a NeRF of its
+ *   own), and adn_set_weights(ctx, 0, ...) fails while sampler is 2.  Every render entry -- rays, aux, camera, rgba8, surface, *_host,
+ *   chunked or not -- starts the rays at the camera, rays_o = pose and rays_d = R dir (not renormalised; on NDC scenes
+ *   ndc_rays follows), places the same K depths on every ray, z = z_near (1 - t) + z_far t with t = linspace(0, 1, K + 1)[k] +
+ *   0.5 / K, warped by LogTransform.to_world with the scene's depth_range (NDC scenes: not warped; adn_linear_depths), and
+ *   composites them with nerf_raw2outputs as sampler 1 does (on NDC scenes |rays_d| is that of ndc_rays' direction).
+ *   `thr` is ignored; 1 <= K <= 128 and N K < 2^31 per chunk; d_nsamples receives K for every ray; z_vals is never NaN;
+ *   d_oracle_weights must be NULL; "sample_budget" > 0 and "sampling_view" fail with ADN_ERR_INVALID.  Profiled,
+ *   adn_get_stats reports the rays in ms_stage[0], 0 in ms_stage[1], the placement in ms_stage[2], the encoding (when not
+ *   fused) in ms_stage[3], the shading MLP in ms_stage[4] and the composite in ms_stage[5]),
  * "pdf_transform" (what sampler 1 applies to raw0 before the inverse CDF, chosen by losses[0] of the training config:
  *   1 = sigmoid (BCEWithLogitsLoss) [default], 2 = softmax (CrossEntropyLoss, CrossEntropyLossWeighted).  0, the
  *   reference's "no transform", fails with ADN_ERR_INVALID: raw0 then gives a non-monotone cdf, whose sample placement
@@ -292,6 +304,21 @@ adn_status adn_budget_threshold(adn_ctx* ctx, const float* d_raw0, int64_t n_ray
  * N K < 2^31.  Like adn_sampling_view it is an inspection entry and takes no stream: it runs on the context's own stream,
  * after the context's earlier calls, and returns once its outputs are written; d_raw0 must be complete when it is called
  * (the stream-ordered path is option "sampler" on the render entries). */
+/* The rays of option "sampler" = 2 (RayMarchFromPoses.batch without a sampling net, src/features.py:417-431): d_dirs [N,3]
+ * camera-space directions -> d_ray_o [N,3] = pose and d_ray_d [N,3] = R d, as nerf_get_ray_dirs' bmm forms it (the FMA chain
+ * of stage 0), which adn_stage3_encode reads (it applies ndc_rays itself on NDC scenes).  d_ray_dirs [N,3] (may be NULL):
+ * the directions whose norm nerf_raw2outputs scales its distances by, which adn_stage5_density_composite reads: R d, or on
+ * NDC scenes ndc_rays' un-normalised direction (:430, as RayMarchFromPoses.postprocess passes it; needs the scene's ndc_w /
+ * ndc_h).  Like adn_pdf_sample it is an inspection entry and takes no stream: it runs on the context's own stream, after
+ * the context's earlier calls, and returns once its outputs are written (the stream-ordered path is option "sampler" = 2
+ * on the render entries). */
+adn_status adn_camera_rays(adn_ctx* ctx, const float* pose, const float* rot, const float* d_dirs, int64_t n_rays, float* d_ray_o,
+                           float* d_ray_d, float* d_ray_dirs);
+/* The K depths (1 <= K <= 128) option "sampler" = 2 places on every ray: LinearlySpacedZNearZFar.generate with det = True
+ * (src/nerf_raymarch_common.py:310-326) in torch's fp32 steps, the to_world pow in double; on NDC scenes
+ * LinearlySpacedZNearZFarNoDepthRange (:276-289), no warp.  d_z [K] fp32.  Like adn_pdf_sample it runs on the context's
+ * own stream and returns once d_z is written. */
+adn_status adn_linear_depths(adn_ctx* ctx, int K, float* d_z);
 adn_status adn_pdf_sample(adn_ctx* ctx, const float* d_raw0, int64_t n_rays, int K, int transform, int32_t* d_count,
                           int32_t* d_offset, int32_t* d_ray, float* d_z);
 /* The sampling network's view of raw0 alone (what option "sampling_view" draws after the sampling MLP), the viewer's
