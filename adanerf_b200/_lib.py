@@ -52,6 +52,8 @@ SYMBOLS = [
     "adn_image_flip", "adn_image_iwssim", "adn_pdf_sample", "adn_stage5_density_composite", "adn_camera_rays",
     "adn_linear_depths",
 ]
+# every symbol include/adanerf_b200_views.h declares (several cameras in one call; tests/test_views_abi.py checks them)
+VIEWS_SYMBOLS = ["adn_render_views_rays", "adn_render_views_camera", "adn_render_views_camera_rgba8"]
 
 _lib = None
 
@@ -91,6 +93,10 @@ def load_library():
     lib.adn_render_camera.argtypes = [vp, fp, fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, f32p, i32p, vp]
     lib.adn_render_camera_rgba8.argtypes = [vp, fp, fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, vp, vp]
     lib.adn_render_camera_surface.argtypes = [vp, fp, fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, C.c_ulonglong, vp]
+    lib.adn_render_views_rays.argtypes = [vp, C.c_int, fp, fp, f32p, i64, C.c_float, C.c_int, f32p, i32p, f32p,
+                                          C.POINTER(AuxOutputs), vp]
+    lib.adn_render_views_camera.argtypes = [vp, C.c_int, fp, fp, C.c_int, C.c_int, C.c_float, C.c_int, f32p, i32p, vp]
+    lib.adn_render_views_camera_rgba8.argtypes = [vp, C.c_int, fp, fp, C.c_int, C.c_int, C.c_float, C.c_int, vp, vp]
     lib.adn_render_rays_host.argtypes = [vp, fp, fp, f32p, i64, C.c_float, C.c_int, f32p, i32p]
     lib.adn_render_camera_host.argtypes = [vp, fp, fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, f32p, i32p]
     lib.adn_stage0_features.argtypes = [vp, fp, fp, f32p, i64, f32p, f32p, f32p, vp]
@@ -111,7 +117,7 @@ def load_library():
     lib.adn_image_metrics.argtypes = [vp, f32p, f32p, i64, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double), vp]
     lib.adn_image_flip.argtypes = [vp, f32p, f32p, C.c_int, C.c_int, C.c_double, f32p, C.POINTER(C.c_double)]
     lib.adn_image_iwssim.argtypes = [vp, f32p, f32p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double)]
-    for name in SYMBOLS:
+    for name in SYMBOLS + VIEWS_SYMBOLS:
         fn = getattr(lib, name)
         if fn.restype is C.c_int and name not in ("adn_destroy", "adn_strerror", "adn_last_error", "adn_version"):
             fn.restype = C.c_int

@@ -16,6 +16,9 @@ A one-network run (rayMarchSampler LinearlySpacedZNearZFar, sampler=2, plain NeR
 one dict, as TrainConfig.inference of a one-model run does.
     dicts[i]["PostProcessedNetworkOutput"]   = outs[i]                           (util/helper.py:79-130)
 
+A batch of several images (ImagePose [n_images, 3], RayDirectionsSamples [n_images, n_samples, 3]) is rendered in one
+views call; every output is then [n_images * n_samples, ...], image-major, as the reference's flattened outputs are.
+
 The batch keys are the reference's DatasetKeyConstants (src/datasets.py:24-38)."""
 import torch
 
@@ -108,11 +111,15 @@ class B200Inference:
             raise NotImplementedError("adanerf_b200 is an inference renderer (src/train.py is out of scope)")
         b = batch_idx.get_batch_input(1) if hasattr(batch_idx, "get_batch_input") else batch_idx
         pose, rot, dirs = b[KEY_POSE], b[KEY_ROT], b[KEY_DIRS]
-        if pose.shape[0] != 1:
-            raise ValueError("one image per inference call (evaluate.py / plots.py batch a single image)")
-        out = self.renderer.render_rays(pose[0], rot[0], dirs.reshape(-1, 3), self.threshold, self.K,
-                                        want_nsamples=True, want_oracle_weights=self.want_oracle_weights,
-                                        want_aux=("weights", "alpha", "z_vals", "depth_est") if self.want_aux else False)
+        # [n_images, n_samples] batches (SpherePosDir.batch / RayMarchFromPoses.batch, features.py:392-427,845-864): one views
+        # call, outputs view-major [n_images * n_samples, ...] like the reference's flattened ones
+        kw = dict(want_nsamples=True, want_oracle_weights=self.want_oracle_weights,
+                  want_aux=("weights", "alpha", "z_vals", "depth_est") if self.want_aux else False)
+        if pose.shape[0] == 1:
+            out = self.renderer.render_rays(pose[0], rot[0], dirs.reshape(-1, 3), self.threshold, self.K, **kw)
+        else:
+            out = self.renderer.render_views(pose.reshape(-1, 3), rot.reshape(-1, 3, 3), dirs.reshape(pose.shape[0], -1, 3),
+                                             self.threshold, self.K, **kw)
         rgb = out["rgb"]
         if self.sampler == 2:   # one network: its dict only (TrainConfig.inference of a one-model run)
             d = {KEY_POST: rgb}

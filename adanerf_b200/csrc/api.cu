@@ -12,6 +12,7 @@
 #include <vector>
 
 #include "../../include/adanerf_b200.h"
+#include "../../include/adanerf_b200_views.h"
 #include "export_loader.h"
 #include "flip.cuh"
 #include "iwssim.cuh"
@@ -568,8 +569,11 @@ adn_status run_mlp(adn_ctx* ctx, int id, const uint8_t* tiles, float* out, const
 // One render call: the camera pose, where the rays come from and where each output goes.  A chunk of a call is a call of
 // its own (chunk_of).
 struct RenderCall {
-  const float* pose;                // [3], host
-  const float* rot;                 // [9] row-major, host
+  const float* pose;                // [3], host ([n_views, 3] for several views)
+  const float* rot;                 // [9] row-major, host ([n_views, 9])
+  int n_views = 1;                  // > 1: the rays are view-major, n_per_view of each view, and stage 0 / the ray kernels
+  int64_t n_per_view = 0;           // take each ray's camera from a ViewTable (views_of)
+  int64_t ray0 = 0;                 // the chunk's first ray in the call (several views)
   const float* d_dirs = nullptr;    // the rays [n_rays, 3], or
   std::optional<CameraRays> cam;    // image rows whose pinhole rays are generated on the device
   int64_t n_rays;
@@ -590,7 +594,8 @@ RenderCall chunk_of(const RenderCall& call, int64_t r0, int64_t chunk) {
   RenderCall c = call;
   c.n_rays = std::min(chunk, call.n_rays - r0);
   if (c.d_dirs) c.d_dirs += 3 * r0;
-  if (c.cam) c.cam->row0 += int(r0 / c.cam->W);
+  if (c.n_views > 1) c.ray0 = r0;   // the pixel is the ray's index inside its view; cam->row0 stays 0
+  else if (c.cam) c.cam->row0 += int(r0 / c.cam->W);
   if (c.d_rgb) c.d_rgb += 3 * r0;
   if (c.d_rgba8) c.d_rgba8 += 4 * r0;
   if (c.d_nsamples) c.d_nsamples += r0;
@@ -612,6 +617,16 @@ Stage5Aux stage5_aux(const adn_ctx* ctx, const adn_aux_outputs& a) {
 // depth_range[1] - depth_range[0] + 1 in double: the base of LogTransform.to_world (the z tables and the fixed-K sampler).
 double depth_base(const adn_ctx* ctx) { return double(ctx->scene.depth_range[1]) - double(ctx->scene.depth_range[0]) + 1.0; }
 
+// The camera table of a chunk of a call over several views (null for one view): a kernel parameter of the stage-0 and ray
+// kernels, so each launch carries its own copy.
+const ViewTable* views_of(const RenderCall& c, ViewTable& t) {
+  if (c.n_views <= 1) return nullptr;
+  t.ray0 = c.ray0;
+  t.n_per_view = c.n_per_view;
+  for (int v = 0; v < c.n_views; ++v) t.v[v] = make_pose(c.pose + 3 * v, c.rot + 9 * v);
+  return &t;
+}
+
 // Stage 0 + the sampling MLP of one chunk, stream ordered.  Writes the chunk's raw0 [n, 128] (the caller's
 // d_oracle_weights when given, else the context's scratch from ray w on) and its ray origins / directions (scratch from ray
 // w on).  w is 0 unless a sample budget keeps the whole call's rows.  timing: record ev[0..2].
@@ -621,10 +636,12 @@ adn_status run_stages_0_1(adn_ctx* ctx, const RenderCall& c, int64_t w, bool tim
   if (s != ADN_OK) return s;
   float* raw0 = c.d_oracle_w ? c.d_oracle_w : ctx->raw0.as<float>() + 128 * w;
   uint8_t* tiles0 = ctx->tiles0.as<uint8_t>();
+  ViewTable vt{};
   if (timing) cudaEventRecord(ctx->ev[0], c.st);
   // stage 0 (writes the sampling net's packed input tiles)
   ADN_CUDA(ctx, launch_stage0(ctx->sc, make_pose(c.pose, c.rot), c.d_dirs, c.cam ? &*c.cam : nullptr, c.n_rays, nullptr,
-                              ctx->ray_o.as<float>() + 3 * w, ctx->ray_d.as<float>() + 3 * w, tiles0, n0.prog.in.n_terms, c.st));
+                              ctx->ray_o.as<float>() + 3 * w, ctx->ray_d.as<float>() + 3 * w, tiles0, n0.prog.in.n_terms, c.st,
+                              views_of(c, vt)));
   ctx->stats.kernel_launches++;
   if (timing) cudaEventRecord(ctx->ev[1], c.st);
   // stage 1
@@ -636,10 +653,11 @@ adn_status run_stages_0_1(adn_ctx* ctx, const RenderCall& c, int64_t w, bool tim
 // Sampler 2's rays of one chunk, in place of stages 0-1: ray_o / ray_d for stage 3 and, on NDC scenes, the composite's NDC
 // directions (ray_dirs).  timing: record ev[0..2] (stage 1's slot stays empty).
 adn_status run_rays(adn_ctx* ctx, const RenderCall& c, bool timing) {
+  ViewTable vt{};
   if (timing) cudaEventRecord(ctx->ev[0], c.st);
   ADN_CUDA(ctx, launch_camera_rays(ctx->sc, make_pose(c.pose, c.rot), c.d_dirs, c.cam ? &*c.cam : nullptr, c.n_rays,
                                    ctx->ray_o.as<float>(), ctx->ray_d.as<float>(),
-                                   ctx->scene.use_ndc ? ctx->ray_dirs.as<float>() : nullptr, c.st));
+                                   ctx->scene.use_ndc ? ctx->ray_dirs.as<float>() : nullptr, c.st, views_of(c, vt)));
   ctx->stats.kernel_launches++;
   if (timing) {
     cudaEventRecord(ctx->ev[1], c.st);
@@ -898,6 +916,37 @@ adn_status render_host(adn_ctx* ctx, RenderCall c, const float* h_dirs, float* h
   if (rgb_staged) std::memcpy(h_rgb, ctx->h_out.p, n * 12);
   if (ns_staged) std::memcpy(h_nsamples, ctx->h_ns.p, n * 4);
   return check_device_error(ctx);
+}
+
+// The checks every views entry makes before anything is enqueued: the camera tables and V (at most kMaxViews, the
+// ViewTable a kernel parameter holds), N >= 1 rays per view and V N within int64.
+adn_status check_views(adn_ctx* ctx, const char* who, int n_views, const float* poses, const float* rots, int64_t n_per_view) {
+  const std::string w(who);
+  if (!ctx) return ADN_ERR_INVALID;
+  if (n_views < 1 || n_views > kMaxViews)
+    return fail(ctx, ADN_ERR_INVALID, w + ": n_views must be 1-" + std::to_string(kMaxViews) + ", not " + std::to_string(n_views));
+  if (!poses || !rots) return fail(ctx, ADN_ERR_INVALID, w + ": poses and rots must not be null");
+  if (n_per_view < 1) return fail(ctx, ADN_ERR_INVALID, w + ": every view needs at least one ray");
+  if (n_per_view > INT64_MAX / n_views)
+    return fail(ctx, ADN_ERR_INVALID, w + ": n_views * rays per view overflows a 64-bit ray count");
+  return ADN_OK;
+}
+
+// A views call over the camera entries: V frames of W x H, every pixel of every view.
+adn_status render_views_camera(adn_ctx* ctx, const char* who, int n_views, const float* poses, const float* rots, int W, int H,
+                               float thr, int K, float* d_rgb, int32_t* d_nsamples, uint8_t* d_rgba8, void* stream) {
+  const std::optional<CameraRays> cam = camera_rays(ctx, W, H, 0, H);
+  if (ctx && !cam) return fail(ctx, ADN_ERR_INVALID, std::string(who) + ": bad image size");
+  adn_status s = check_views(ctx, who, n_views, poses, rots, int64_t(std::max(W, 0)) * std::max(H, 0));
+  if (s != ADN_OK) return s;
+  RenderCall c(poses, rots, int64_t(W) * H * n_views, thr, K, stream);
+  c.cam = cam;
+  c.n_views = n_views;
+  c.n_per_view = int64_t(W) * H;
+  c.d_rgb = d_rgb;
+  c.d_nsamples = d_nsamples;
+  c.d_rgba8 = d_rgba8;
+  return render_ordered(ctx, c, who);
 }
 
 }  // namespace
@@ -1176,6 +1225,34 @@ adn_status adn_render_camera_surface(adn_ctx* ctx, const float* pose, const floa
   ADN_CUDA(ctx, launch_rgba_to_surface(c.d_rgba8, W, row0, rows, surface, c.st));
   ctx->stats.kernel_launches++;
   return ADN_OK;
+}
+
+adn_status adn_render_views_rays(adn_ctx* ctx, int n_views, const float* poses, const float* rots, const float* d_dirs,
+                                 int64_t n_per_view, float thr, int K, float* d_rgb, int32_t* d_nsamples,
+                                 float* d_oracle_weights, const adn_aux_outputs* aux, void* stream) {
+  adn_status s = check_views(ctx, "render_views_rays", n_views, poses, rots, n_per_view);
+  if (s != ADN_OK) return s;
+  if (!d_dirs) return fail(ctx, ADN_ERR_INVALID, "render_views_rays: d_dirs is null");
+  RenderCall c(poses, rots, n_per_view * n_views, thr, K, stream);
+  c.n_views = n_views;
+  c.n_per_view = n_per_view;
+  c.d_dirs = d_dirs;
+  c.d_rgb = d_rgb;
+  c.d_nsamples = d_nsamples;
+  c.d_oracle_w = d_oracle_weights;
+  if (aux) c.aux = *aux;
+  return render_ordered(ctx, c, "render_views_rays");
+}
+
+adn_status adn_render_views_camera(adn_ctx* ctx, int n_views, const float* poses, const float* rots, int W, int H, float thr,
+                                   int K, float* d_rgb, int32_t* d_nsamples, void* stream) {
+  return render_views_camera(ctx, "render_views_camera", n_views, poses, rots, W, H, thr, K, d_rgb, d_nsamples, nullptr, stream);
+}
+
+adn_status adn_render_views_camera_rgba8(adn_ctx* ctx, int n_views, const float* poses, const float* rots, int W, int H,
+                                         float thr, int K, uint8_t* d_rgba8, void* stream) {
+  return render_views_camera(ctx, "render_views_camera_rgba8", n_views, poses, rots, W, H, thr, K, nullptr, nullptr, d_rgba8,
+                             stream);
 }
 
 adn_status adn_register_host_buffer(adn_ctx* ctx, const void* p, size_t bytes) {

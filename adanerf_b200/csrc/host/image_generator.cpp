@@ -89,6 +89,30 @@ bool ImageGenerator::inference_host(const Camera& camera, float* h_rgb, int batc
   return s == ADN_OK;
 }
 
+bool ImageGenerator::inference_views(const Camera* cameras, int n_views, float* d_rgb, int batch_size, int num_samples,
+                                     int32_t* d_nsamples, void* stream) {
+  if (!ctx_) return false;
+  if (!cameras || n_views < 1) {
+    err_ = "inference_views: need at least one camera";
+    return false;
+  }
+  std::vector<float> poses(size_t(n_views) * 3), rots(size_t(n_views) * 9);
+  for (int v = 0; v < n_views; ++v) {
+    const Camera& c = cameras[v];
+    if (c.width != cameras[0].width || c.height != cameras[0].height) {
+      err_ = "inference_views: every camera must have the same size";
+      return false;
+    }
+    for (int a = 0; a < 3; ++a) poses[size_t(v) * 3 + a] = c.pos[a];
+    c.rotation(rots.data() + size_t(v) * 9);
+  }
+  if (!apply_options(batch_size)) return false;
+  const adn_status s = adn_render_views_camera(ctx_, n_views, poses.data(), rots.data(), cameras[0].width, cameras[0].height, thr_,
+                                               num_samples, d_rgb, d_nsamples, stream);
+  if (s != ADN_OK) err_ = adn_last_error(ctx_);
+  return s == ADN_OK;
+}
+
 bool ImageGenerator::set_sample_budget(int64_t max_samples) {
   if (!ctx_) return false;
   const adn_status s = adn_set_option(ctx_, "sample_budget", max_samples);

@@ -10,6 +10,7 @@
 #include <vector>
 
 #include "../../../include/adanerf_b200.h"
+#include "../../../include/adanerf_b200_views.h"
 
 // The viewer's own types that appear in ImageGenerator::inference's parameter list (include/featureset.h:25,
 // include/encoding.h:10).  The replacement never looks inside them -- the features and encodings of the hot path live in
@@ -60,6 +61,11 @@ class ImageGenerator {
                  std::vector<::FeatureSet*>& feature_sets, std::vector<::Encoding>& encodings);
   // Same into a host fp32 buffer [W*H*3] (copies inside).
   bool inference_host(const Camera& camera, float* h_rgb, int batch_size, int num_samples, int32_t* h_nsamples = nullptr);
+  // Several cameras in one call (adn_render_views_camera): n_views frames of the cameras' common size (1-64 views, e.g. the
+  // two eyes of a head-mounted display) under one sample budget.  d_rgb: device buffer [n_views*H*W*3] fp32, view-major;
+  // d_nsamples (may be null): [n_views*H*W].
+  bool inference_views(const Camera* cameras, int n_views, float* d_rgb, int batch_size, int num_samples,
+                       int32_t* d_nsamples = nullptr, void* stream = nullptr);
 
   // Frame-cost control (adn_set_option "sample_budget"): at most `max_samples` samples per inference call, the config's
   // adaptiveSamplingThreshold being the floor; 0 = off.  last_threshold(): the threshold the last frame used (synchronises).

@@ -57,14 +57,35 @@ __device__ __forceinline__ void rotate_dir(const PoseDev& pd, const float (&d)[3
     nds[r] = __fmaf_rn(pd.rot[3 * r + 2], d[2], __fmaf_rn(pd.rot[3 * r + 1], d[1], __fmul_rn(pd.rot[3 * r + 0], d[0])));
 }
 
-// SpherePosDir.batch (src/features.py:845-899) up to the encodings: the pixel direction d of ray i, the ray origin p on the
-// view-cell sphere, the rotated direction nds and its unit copy dn.
+// Where ray i of a launch takes its camera from, and its index inside its view (pix: its pixel when the rays are generated
+// from a camera).  OnePose: one camera for the launch, pix = i.  PerView: the row of its view in a ViewTable (view-major
+// rays, the launch starting at ray t.ray0 of the call).
+struct OnePose {
+  const PoseDev& pd;
+  __device__ __forceinline__ const PoseDev& of(long long i, long long& pix) const {
+    pix = i;
+    return pd;
+  }
+};
+struct PerView {
+  const ViewTable& t;
+  __device__ __forceinline__ const PoseDev& of(long long i, long long& pix) const {
+    const long long g = t.ray0 + i;
+    const long long v = g / t.n_per_view;
+    pix = g - v * t.n_per_view;
+    return t.v[v];
+  }
+};
+
+// SpherePosDir.batch (src/features.py:845-899) up to the encodings: the pixel direction d of ray i (pixel pix), the ray
+// origin p on the view-cell sphere, the rotated direction nds and its unit copy dn.
 template <bool FROM_CAMERA>
 __device__ __forceinline__ void sphere_pos_dir(const SceneDev& sc, const PoseDev& pd, const float* __restrict__ dirs,
-                                               const CameraRays& cam, long long i, float (&p)[3], float (&nds)[3], float (&dn)[3]) {
+                                               const CameraRays& cam, long long i, long long pix, float (&p)[3], float (&nds)[3],
+                                               float (&dn)[3]) {
   float d[3];
   if (FROM_CAMERA) {
-    pixel_dir(cam, i, d);
+    pixel_dir(cam, pix, d);
   } else {
     d[0] = dirs[3 * i + 0];
     d[1] = dirs[3 * i + 1];
@@ -87,11 +108,11 @@ __device__ __forceinline__ void sphere_pos_dir(const SceneDev& sc, const PoseDev
 }
 
 // One thread per ray, the encodings "10-4" or "2-2" at compile time.
-template <bool FROM_CAMERA, int NFD = kNFreqDir, int NFP = kNFreqPos>
-__global__ void __launch_bounds__(128)
-stage0_kernel(const __grid_constant__ SceneDev sc, const __grid_constant__ PoseDev pd, const float* __restrict__ dirs,
-              const __grid_constant__ CameraRays cam, long long n_rays, float* __restrict__ x0, float* __restrict__ ray_o,
-              float* __restrict__ ray_d, uint8_t* __restrict__ tiles0, int tile_terms) {
+template <bool FROM_CAMERA, int NFD, int NFP, class Poses>
+__device__ __forceinline__ void stage0_body(const SceneDev& sc, const Poses& poses, const float* __restrict__ dirs,
+                                            const CameraRays& cam, long long n_rays, float* __restrict__ x0,
+                                            float* __restrict__ ray_o, float* __restrict__ ray_d, uint8_t* __restrict__ tiles0,
+                                            int tile_terms, uint8_t* s_tile) {
   constexpr int F0 = 6 + 6 * (NFD + NFP);       // 90 ("10-4") or 30 ("2-2")
   const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;   // grid covers whole 128-ray tiles
   float f[F0];
@@ -99,7 +120,9 @@ stage0_kernel(const __grid_constant__ SceneDev sc, const __grid_constant__ PoseD
   for (int j = 0; j < F0; ++j) f[j] = 0.0f;
   if (i < n_rays) {
     float p[3], nds[3], dn[3];
-    sphere_pos_dir<FROM_CAMERA>(sc, pd, dirs, cam, i, p, nds, dn);
+    long long pix;
+    const PoseDev& pd = poses.of(i, pix);
+    sphere_pos_dir<FROM_CAMERA>(sc, pd, dirs, cam, i, pix, p, nds, dn);
     posenc3<NFD>(dn, f);                           // 27 / 15: direction block FIRST (:868)
     posenc3<NFP>(p, f + 3 + 6 * NFD);              // 63 / 15
     if (ray_o) {
@@ -115,29 +138,48 @@ stage0_kernel(const __grid_constant__ SceneDev sc, const __grid_constant__ PoseD
     }
   }
   if (tiles0) {   // the CTA's 128 rays are one tile of the sampling net's input
-    extern __shared__ __align__(1024) uint8_t s_tile[];
     const TileFormat fmt = sampling_tiles(F0, tile_terms);
     store_tile(fmt, f, s_tile, tiles0 + size_t(i >> 7) * fmt.tile_bytes());
     store_tiles_drain();
   }
 }
 
+template <bool FROM_CAMERA, int NFD = kNFreqDir, int NFP = kNFreqPos>
+__global__ void __launch_bounds__(128)
+stage0_kernel(const __grid_constant__ SceneDev sc, const __grid_constant__ PoseDev pd, const float* __restrict__ dirs,
+              const __grid_constant__ CameraRays cam, long long n_rays, float* __restrict__ x0, float* __restrict__ ray_o,
+              float* __restrict__ ray_d, uint8_t* __restrict__ tiles0, int tile_terms) {
+  extern __shared__ __align__(1024) uint8_t s_tile[];
+  stage0_body<FROM_CAMERA, NFD, NFP>(sc, OnePose{pd}, dirs, cam, n_rays, x0, ray_o, ray_d, tiles0, tile_terms, s_tile);
+}
+
+// The same over the views of a multi-view call: each ray takes its view's camera.
+template <bool FROM_CAMERA, int NFD = kNFreqDir, int NFP = kNFreqPos>
+__global__ void __launch_bounds__(128)
+stage0_views_kernel(const __grid_constant__ SceneDev sc, const __grid_constant__ ViewTable views, const float* __restrict__ dirs,
+                    const __grid_constant__ CameraRays cam, long long n_rays, float* __restrict__ x0, float* __restrict__ ray_o,
+                    float* __restrict__ ray_d, uint8_t* __restrict__ tiles0, int tile_terms) {
+  extern __shared__ __align__(1024) uint8_t s_tile[];
+  stage0_body<FROM_CAMERA, NFD, NFP>(sc, PerView{views}, dirs, cam, n_rays, x0, ray_o, ray_d, tiles0, tile_terms, s_tile);
+}
+
 // Any other encoding (sc.n_freq_dir0 + sc.n_freq_pos0 <= 20 bands, 0 = posEnc none): the same features, written one at a
 // time into x0 and the tile image, so no thread holds its up to 126 features at once.
-template <bool FROM_CAMERA>
-__global__ void __launch_bounds__(128)
-stage0_rt_kernel(const __grid_constant__ SceneDev sc, const __grid_constant__ PoseDev pd, const float* __restrict__ dirs,
-                 const __grid_constant__ CameraRays cam, long long n_rays, float* __restrict__ x0, float* __restrict__ ray_o,
-                 float* __restrict__ ray_d, uint8_t* __restrict__ tiles0, int tile_terms) {
+template <bool FROM_CAMERA, class Poses>
+__device__ __forceinline__ void stage0_rt_body(const SceneDev& sc, const Poses& poses, const float* __restrict__ dirs,
+                                               const CameraRays& cam, long long n_rays, float* __restrict__ x0,
+                                               float* __restrict__ ray_o, float* __restrict__ ray_d,
+                                               uint8_t* __restrict__ tiles0, int tile_terms, uint8_t* s_tile) {
   const int nfd = sc.n_freq_dir0, nfp = sc.n_freq_pos0;
   const int F0 = 6 + 6 * (nfd + nfp);
   const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;   // grid covers whole 128-ray tiles
-  extern __shared__ __align__(1024) uint8_t s_tile[];
   const TileFormat fmt = sampling_tiles(F0, tile_terms);
   if (tiles0) zero_row(fmt, s_tile, threadIdx.x, 0, fmt.n_blk);
   if (i < n_rays) {
     float p[3], nds[3], dn[3];
-    sphere_pos_dir<FROM_CAMERA>(sc, pd, dirs, cam, i, p, nds, dn);
+    long long pix;
+    const PoseDev& pd = poses.of(i, pix);
+    sphere_pos_dir<FROM_CAMERA>(sc, pd, dirs, cam, i, pix, p, nds, dn);
     auto put = [&](int c, float v) {
       if (x0) x0[i * F0 + c] = v;
       if (tiles0) put_feature(fmt, s_tile, c >> 6, threadIdx.x, c & 63, v);
@@ -158,9 +200,27 @@ stage0_rt_kernel(const __grid_constant__ SceneDev sc, const __grid_constant__ Po
   }
 }
 
+template <bool FROM_CAMERA>
+__global__ void __launch_bounds__(128)
+stage0_rt_kernel(const __grid_constant__ SceneDev sc, const __grid_constant__ PoseDev pd, const float* __restrict__ dirs,
+                 const __grid_constant__ CameraRays cam, long long n_rays, float* __restrict__ x0, float* __restrict__ ray_o,
+                 float* __restrict__ ray_d, uint8_t* __restrict__ tiles0, int tile_terms) {
+  extern __shared__ __align__(1024) uint8_t s_tile[];
+  stage0_rt_body<FROM_CAMERA>(sc, OnePose{pd}, dirs, cam, n_rays, x0, ray_o, ray_d, tiles0, tile_terms, s_tile);
+}
+
+template <bool FROM_CAMERA>
+__global__ void __launch_bounds__(128)
+stage0_rt_views_kernel(const __grid_constant__ SceneDev sc, const __grid_constant__ ViewTable views, const float* __restrict__ dirs,
+                       const __grid_constant__ CameraRays cam, long long n_rays, float* __restrict__ x0, float* __restrict__ ray_o,
+                       float* __restrict__ ray_d, uint8_t* __restrict__ tiles0, int tile_terms) {
+  extern __shared__ __align__(1024) uint8_t s_tile[];
+  stage0_rt_body<FROM_CAMERA>(sc, PerView{views}, dirs, cam, n_rays, x0, ray_o, ray_d, tiles0, tile_terms, s_tile);
+}
+
 cudaError_t launch_stage0(const SceneDev& sc, const PoseDev& pd, const float* d_dirs, const CameraRays* cam,
                           long long n_rays, float* d_x0, float* d_ray_o, float* d_ray_d, uint8_t* d_tiles0, int tile_terms,
-                          cudaStream_t s) {
+                          cudaStream_t s, const ViewTable* views) {
   if (n_rays <= 0) return cudaSuccess;
   const long long n_pad = ((n_rays + kTileM - 1) / kTileM) * kTileM;
   const unsigned grid = unsigned((n_pad + 127) / 128);
@@ -177,9 +237,24 @@ cudaError_t launch_stage0(const SceneDev& sc, const PoseDev& pd, const float* d_
     else k_rays<<<grid, 128, smem, s>>>(sc, pd, d_dirs, c, n_rays, d_x0, d_ray_o, d_ray_d, d_tiles0, tile_terms);
     return cudaGetLastError();
   };
+  auto run_views = [&](auto k_cam, auto k_rays, unsigned long long* attr) -> cudaError_t {
+    if (set_max_dyn_smem_once(reinterpret_cast<const void*>(k_cam), tile_bytes, &attr[0]) != cudaSuccess ||
+        set_max_dyn_smem_once(reinterpret_cast<const void*>(k_rays), tile_bytes, &attr[1]) != cudaSuccess)
+      return cudaGetLastError();
+    if (cam) k_cam<<<grid, 128, smem, s>>>(sc, *views, d_dirs, c, n_rays, d_x0, d_ray_o, d_ray_d, d_tiles0, tile_terms);
+    else k_rays<<<grid, 128, smem, s>>>(sc, *views, d_dirs, c, n_rays, d_x0, d_ray_o, d_ray_d, d_tiles0, tile_terms);
+    return cudaGetLastError();
+  };
   static unsigned long long attr104[2] = {0, 0}, attr22[2] = {0, 0}, attr_rt[2] = {0, 0};   // per device
-  if (sc.n_freq_pos0 == kNFreqPos && sc.n_freq_dir0 == kNFreqDir) return run(stage0_kernel<true>, stage0_kernel<false>, attr104);
-  if (sc.n_freq_pos0 == 2 && sc.n_freq_dir0 == 2) return run(stage0_kernel<true, 2, 2>, stage0_kernel<false, 2, 2>, attr22);
+  static unsigned long long vattr104[2] = {0, 0}, vattr22[2] = {0, 0}, vattr_rt[2] = {0, 0};
+  const bool e104 = sc.n_freq_pos0 == kNFreqPos && sc.n_freq_dir0 == kNFreqDir, e22 = sc.n_freq_pos0 == 2 && sc.n_freq_dir0 == 2;
+  if (views) {
+    if (e104) return run_views(stage0_views_kernel<true>, stage0_views_kernel<false>, vattr104);
+    if (e22) return run_views(stage0_views_kernel<true, 2, 2>, stage0_views_kernel<false, 2, 2>, vattr22);
+    return run_views(stage0_rt_views_kernel<true>, stage0_rt_views_kernel<false>, vattr_rt);
+  }
+  if (e104) return run(stage0_kernel<true>, stage0_kernel<false>, attr104);
+  if (e22) return run(stage0_kernel<true, 2, 2>, stage0_kernel<false, 2, 2>, attr22);
   return run(stage0_rt_kernel<true>, stage0_rt_kernel<false>, attr_rt);
 }
 
@@ -189,16 +264,17 @@ cudaError_t launch_stage0(const SceneDev& sc, const PoseDev& pd, const float* d_
 // nerf_raw2outputs scales its distances by: rays_d itself, or on NDC scenes ndc_rays' un-normalised direction (what
 // RayMarchFromPoses.postprocess hands it, not the unit copy that is encoded).  12 B in (or the pixel's direction from cam),
 // 24 B out per ray, 36 B with ray_dirs.
-template <bool FROM_CAMERA>
-__global__ void __launch_bounds__(256)
-camera_rays_kernel(const __grid_constant__ SceneDev sc, const __grid_constant__ PoseDev pd, const float* __restrict__ dirs,
-                   const __grid_constant__ CameraRays cam, long long n_rays, float* __restrict__ ray_o, float* __restrict__ ray_d,
-                   float* __restrict__ ray_dirs) {
+template <bool FROM_CAMERA, class Poses>
+__device__ __forceinline__ void camera_rays_body(const SceneDev& sc, const Poses& poses, const float* __restrict__ dirs,
+                                                 const CameraRays& cam, long long n_rays, float* __restrict__ ray_o,
+                                                 float* __restrict__ ray_d, float* __restrict__ ray_dirs) {
   const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (i >= n_rays) return;
+  long long pix;
+  const PoseDev& pd = poses.of(i, pix);
   float d[3], nds[3];
   if (FROM_CAMERA) {
-    pixel_dir(cam, i, d);
+    pixel_dir(cam, pix, d);
   } else {
 #pragma unroll
     for (int a = 0; a < 3; ++a) d[a] = __ldg(dirs + 3 * i + a);
@@ -220,12 +296,33 @@ camera_rays_kernel(const __grid_constant__ SceneDev sc, const __grid_constant__ 
   }
 }
 
+template <bool FROM_CAMERA>
+__global__ void __launch_bounds__(256)
+camera_rays_kernel(const __grid_constant__ SceneDev sc, const __grid_constant__ PoseDev pd, const float* __restrict__ dirs,
+                   const __grid_constant__ CameraRays cam, long long n_rays, float* __restrict__ ray_o, float* __restrict__ ray_d,
+                   float* __restrict__ ray_dirs) {
+  camera_rays_body<FROM_CAMERA>(sc, OnePose{pd}, dirs, cam, n_rays, ray_o, ray_d, ray_dirs);
+}
+
+// The same over the views of a multi-view call: each ray takes its view's camera.
+template <bool FROM_CAMERA>
+__global__ void __launch_bounds__(256)
+camera_rays_views_kernel(const __grid_constant__ SceneDev sc, const __grid_constant__ ViewTable views, const float* __restrict__ dirs,
+                         const __grid_constant__ CameraRays cam, long long n_rays, float* __restrict__ ray_o,
+                         float* __restrict__ ray_d, float* __restrict__ ray_dirs) {
+  camera_rays_body<FROM_CAMERA>(sc, PerView{views}, dirs, cam, n_rays, ray_o, ray_d, ray_dirs);
+}
+
 cudaError_t launch_camera_rays(const SceneDev& sc, const PoseDev& pd, const float* d_dirs, const CameraRays* cam,
-                               long long n_rays, float* d_ray_o, float* d_ray_d, float* d_ray_dirs, cudaStream_t s) {
+                               long long n_rays, float* d_ray_o, float* d_ray_d, float* d_ray_dirs, cudaStream_t s,
+                               const ViewTable* views) {
   if (n_rays <= 0) return cudaSuccess;
   const unsigned grid = unsigned((n_rays + 255) / 256);
-  if (cam) camera_rays_kernel<true><<<grid, 256, 0, s>>>(sc, pd, d_dirs, *cam, n_rays, d_ray_o, d_ray_d, d_ray_dirs);
-  else camera_rays_kernel<false><<<grid, 256, 0, s>>>(sc, pd, d_dirs, CameraRays{}, n_rays, d_ray_o, d_ray_d, d_ray_dirs);
+  const CameraRays c = cam ? *cam : CameraRays{};
+  if (views && cam) camera_rays_views_kernel<true><<<grid, 256, 0, s>>>(sc, *views, d_dirs, c, n_rays, d_ray_o, d_ray_d, d_ray_dirs);
+  else if (views) camera_rays_views_kernel<false><<<grid, 256, 0, s>>>(sc, *views, d_dirs, c, n_rays, d_ray_o, d_ray_d, d_ray_dirs);
+  else if (cam) camera_rays_kernel<true><<<grid, 256, 0, s>>>(sc, pd, d_dirs, c, n_rays, d_ray_o, d_ray_d, d_ray_dirs);
+  else camera_rays_kernel<false><<<grid, 256, 0, s>>>(sc, pd, d_dirs, c, n_rays, d_ray_o, d_ray_d, d_ray_dirs);
   return cudaGetLastError();
 }
 

@@ -27,17 +27,32 @@ struct PoseDev {
   float rot[9];
 };
 
+// The cameras of a call over several views, passed to the kernels as a kernel parameter: every launch carries its own copy,
+// so nothing is uploaded that a later call could overwrite before the kernel reads it, and no host synchronisation is
+// needed.  Rays are view-major: ray g of the call is ray g - v N of view v = g / N.  kMaxViews x 48 B = 3 KB keeps every
+// launch's parameters under the 4 KB of the classic kernel-parameter limit.
+constexpr int kMaxViews = 64;
+struct ViewTable {
+  long long ray0;         // the launch's first ray in the call's view-major order (a chunk's offset)
+  long long n_per_view;   // N
+  PoseDev v[kMaxViews];
+};
+
 cudaError_t launch_gen_dirs(const CameraRays& cam, long long n_rays, float* d_dirs, cudaStream_t s);
 // Stage 0.  Any of d_x0 (fp32 features), d_ray_o / d_ray_d and d_tiles0 may be null (not written).  d_tiles0: the sampling
 // net's packed input tiles (sampling_tiles in tiles.cuh) with tile_terms terms (1 or 2).
+// views (may be null): ray i of the launch takes the camera of its view instead of pd; with cam its pixel is its index inside
+// the view (cam.row0 must then be 0).
 cudaError_t launch_stage0(const SceneDev& sc, const PoseDev& pd, const float* d_dirs, const CameraRays* cam,
                           long long n_rays, float* d_x0, float* d_ray_o, float* d_ray_d, uint8_t* d_tiles0, int tile_terms,
-                          cudaStream_t s);
+                          cudaStream_t s, const ViewTable* views = nullptr);
 // The rays of a render without a sampling net (option "sampler" 2): d_ray_o [N,3] = pose, d_ray_d [N,3] = R d (the FMA
 // chain of stage 0), from d_dirs or, when cam is given, the pixels' directions.  d_ray_dirs (may be null): the directions
 // whose norm nerf_raw2outputs scales its distances by, R d or on NDC scenes (sc.ndc) ndc_rays' un-normalised direction.
+// views: as for launch_stage0.
 cudaError_t launch_camera_rays(const SceneDev& sc, const PoseDev& pd, const float* d_dirs, const CameraRays* cam,
-                               long long n_rays, float* d_ray_o, float* d_ray_d, float* d_ray_dirs, cudaStream_t s);
+                               long long n_rays, float* d_ray_o, float* d_ray_d, float* d_ray_dirs, cudaStream_t s,
+                               const ViewTable* views = nullptr);
 
 // Stage 2.  tile_state: [n_ctas + 2] uint64 scratch zeroed by the launcher (memsetAsync).
 size_t stage2_scratch_bytes(long long n_rays);

@@ -236,8 +236,19 @@ class Renderer:
         p, r = self._pose_rot(pose, rot)
         d = self._f32(dirs).reshape(-1, 3)
         n = d.shape[0]
+        out, aux = self._ray_outputs("render_rays", n, K, want_nsamples, want_oracle_weights, want_aux, out, aux_out)
+        ptr = lambda t: t.data_ptr() if t is not None else None
+        with torch.cuda.device(self.device):
+            self._check(self.lib.adn_render_rays_aux(self.handle, _fptr(p), _fptr(r), d.data_ptr(), n, float(thr), int(K),
+                                                     out["rgb"].data_ptr(), ptr(out["n_samples"]), ptr(out["oracle_weights"]),
+                                                     C.byref(aux) if aux is not None else None, self._stream()))
+        return out
+
+    def _ray_outputs(self, who, n, K, want_nsamples, want_oracle_weights, want_aux, out, aux_out):
+        """The output tensors of a render over n rays (render_rays, render_views) and the adn_aux_outputs that point at the
+        requested aux ones (None when none is)."""
         if out is not None and (out.dtype != torch.float32 or out.numel() != 3 * n or not out.is_contiguous() or out.device != self._dev()):
-            raise ValueError("render_rays: out must be a contiguous float32 [N,3] tensor on the renderer's device")
+            raise ValueError(f"{who}: out must be a contiguous float32 [N,3] tensor on the renderer's device")
         rgb = out if out is not None else torch.empty((n, 3), dtype=torch.float32, device=self._dev())
         ns = torch.empty((n,), dtype=torch.int32, device=self._dev()) if want_nsamples else None
         ow = torch.empty((n, 128), dtype=torch.float32, device=self._dev()) if want_oracle_weights else None
@@ -253,15 +264,56 @@ class Renderer:
                 if t is None:
                     t = torch.empty(shape, dtype=torch.float32, device=self._dev())
                 elif t.dtype != torch.float32 or tuple(t.shape) != shape or not t.is_contiguous() or t.device != self._dev():
-                    raise ValueError(f"render_rays: aux_out[{k!r}] must be a contiguous float32 {list(shape)} tensor on the renderer's device")
+                    raise ValueError(f"{who}: aux_out[{k!r}] must be a contiguous float32 {list(shape)} tensor on the renderer's device")
                 out[k] = t
                 setattr(aux, "d_" + k, t.data_ptr())
+        return out, aux
+
+    @staticmethod
+    def _view_tables(poses, rots):
+        """poses [V,3] and rots [V,3,3] (tensors or arrays) -> contiguous float32 host arrays [V,3], [V,9] and V."""
+        host = lambda x: np.asarray(x.detach().cpu() if isinstance(x, torch.Tensor) else x, dtype=np.float32)
+        p, r = host(poses), host(rots)
+        v = p.reshape(-1, 3).shape[0] if p.size % 3 == 0 else -1
+        if p.size != 3 * v or r.size != 9 * v or v < 1:
+            raise ValueError(f"views: poses must be [V,3] and rots [V,3,3] for the same V >= 1, got {p.shape} and {r.shape}")
+        return np.ascontiguousarray(p.reshape(v, 3)), np.ascontiguousarray(r.reshape(v, 9)), v
+
+    def render_views(self, poses, rots, dirs, thr, K, want_nsamples=True, want_oracle_weights=False, want_aux=False, out=None,
+                     aux_out=None):
+        """V cameras in one call (adn_render_views_rays): poses [V,3], rots [V,3,3], dirs [V,N,3] (cuda tensor) -> the dict
+        of render_rays over the V N rays, view-major ([V N, ...]: ray v N + i is ray i of view v).  Without a sample budget
+        this is bit for bit the V render_rays calls concatenated; under one, one threshold covers all views."""
+        p, r, v = self._view_tables(poses, rots)
+        d = self._f32(dirs).reshape(-1, 3)
+        if d.shape[0] % v:
+            raise ValueError(f"render_views: dirs must be [V,N,3] with V = {v}, got {tuple(dirs.shape)}")
+        n = d.shape[0]
+        out, aux = self._ray_outputs("render_views", n, K, want_nsamples, want_oracle_weights, want_aux, out, aux_out)
+        ptr = lambda t: t.data_ptr() if t is not None else None
         with torch.cuda.device(self.device):
-            self._check(self.lib.adn_render_rays_aux(self.handle, _fptr(p), _fptr(r), d.data_ptr(), n, float(thr), int(K),
-                                                     rgb.data_ptr(), ns.data_ptr() if ns is not None else None,
-                                                     ow.data_ptr() if ow is not None else None,
-                                                     C.byref(aux) if aux is not None else None, self._stream()))
+            self._check(self.lib.adn_render_views_rays(self.handle, v, _fptr(p), _fptr(r), d.data_ptr(), n // v, float(thr), int(K),
+                                                       out["rgb"].data_ptr(), ptr(out["n_samples"]), ptr(out["oracle_weights"]),
+                                                       C.byref(aux) if aux is not None else None, self._stream()))
         return out
+
+    def render_views_camera(self, poses, rots, W, H, thr, K, rgba8=False, want_nsamples=False):
+        """V whole W x H frames in one call (adn_render_views_camera / _rgba8) -> dict(rgb [V*H*W, 3] float32, n_samples
+        [V*H*W] int32 or None), or with rgba8=True the viewer's pixels [V*H*W, 4] uint8."""
+        p, r, v = self._view_tables(poses, rots)
+        n = v * int(W) * int(H)
+        dev = self._dev()
+        with torch.cuda.device(self.device):
+            if rgba8:
+                px = torch.empty((n, 4), dtype=torch.uint8, device=dev)
+                self._check(self.lib.adn_render_views_camera_rgba8(self.handle, v, _fptr(p), _fptr(r), int(W), int(H), float(thr),
+                                                                   int(K), px.data_ptr(), self._stream()))
+                return px
+            rgb = torch.empty((n, 3), dtype=torch.float32, device=dev)
+            ns = torch.empty((n,), dtype=torch.int32, device=dev) if want_nsamples else None
+            self._check(self.lib.adn_render_views_camera(self.handle, v, _fptr(p), _fptr(r), int(W), int(H), float(thr), int(K),
+                                                         rgb.data_ptr(), ns.data_ptr() if ns is not None else None, self._stream()))
+        return dict(rgb=rgb, n_samples=ns)
 
     def render_camera(self, pose, rot, W, H, thr, K, row0=0, rows=None, out=None, want_nsamples=False):
         """Renders image rows [row0, row0+rows) of a WxH pinhole frame; rays generated on the device."""
