@@ -104,6 +104,13 @@ class B200Inference:
         """Builds the renderer from an initialised reference TrainConfig (models, feature sets, dataset_info)."""
         scene, models, thr, k = cls.args_from_train_config(train_config)
         sampler, transform = cls.sampler_from_train_config(train_config)
+        disc = getattr(train_config.f_in[-1].z_sampler, "disc", None)   # multiDepthFeatures[1] (nerf_raymarch_common.py:674-676)
+        if models[0] is not None and disc is not None:
+            sd = models[0].state_dict()
+            last = max(int(n.split(".")[1]) for n in sd if n.startswith("layers.") and n.endswith(".weight"))
+            width = int(sd[f"layers.{last}.weight"].shape[0])
+            if width != int(disc):
+                raise ValueError(f"the sampler places {disc} depth cells (multiDepthFeatures) but the sampling net has {width} outputs")
         return cls(scene, models[0], models[1], thr, k, device=device, sampler=sampler, pdf_transform=transform)
 
     def inference(self, batch_idx, gradient=False, **kwargs):

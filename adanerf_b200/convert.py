@@ -72,10 +72,13 @@ def parse_encoding(pos_enc=("nerf", "nerf"), pos_enc_args=("10-4", "10-4")):
     return tuple(out)
 
 
-def check_state_dicts(sd0, sd1, encoding=None):
+DEPTH_CELLS = (32, 64, 128, 256)   # multiDepthFeatures the renderer supports: the sampling net's output width D
+
+
+def check_state_dicts(sd0, sd1, encoding=None, depth_cells=128):
     """The architecture the hot path implements: BaseNet sampling net, NeRF shading net with a view branch, in the shapes
-    adn_set_weights accepts (include/adanerf_b200.h): sampling net 1-12 layers of hidden width 128 or 256, 128 outputs,
-    no skips; shading net 1-10 pts layers of width W = 128 or 256, at most one skip, view branch W/2.
+    adn_set_weights accepts (include/adanerf_b200.h): sampling net 1-12 layers of hidden width 128 or 256, D = depth_cells
+    outputs (multiDepthFeatures: 32, 64, 128 or 256), no skips; shading net 1-10 pts layers of width W = 128 or 256, at most one skip, view branch W/2.
     encoding: parse_encoding's ((P0, D0), (P, D)); the input columns must be those of that encoding.  None: posEncArgs
     [10-4, 10-4] or [2-2, 10-4].
     Returns net_shapes(sd0, sd1); raises ValueError naming the offending tensor."""
@@ -112,12 +115,14 @@ def check_state_dicts(sd0, sd1, encoding=None):
 
     if not 1 <= d0 <= 12:
         raise ValueError(f"sampling net: layers.0 .. layers.{d0 - 1}: {d0} layers, 1-12 are supported")
+    if depth_cells not in DEPTH_CELLS:
+        raise ValueError(f"depth cells (multiDepthFeatures) {depth_cells}: 32, 64, 128 or 256 are supported")
     for i in range(d0):
-        n_out = 128 if i == d0 - 1 else w0
-        if n_out not in (128, 256):
+        n_out = depth_cells if i == d0 - 1 else w0
+        if i != d0 - 1 and n_out not in (128, 256):
             raise ValueError(f"sampling net: layers.{i}.weight has {n_out} outputs; the hidden width must be 128 or 256")
         expect(sd0, f"layers.{i}.weight", n_out, sd0["layers.0.weight"].shape[1] if i == 0 else w0,
-               "sampling net (no skips; layer widths must chain, 128 outputs)")
+               f"sampling net (no skips; layer widths must chain, {depth_cells} outputs = the depth cells)")
     if w1 not in (128, 256):
         raise ValueError(f"shading net: pts_linears.0.weight has {w1} rows; the width W must be 128 or 256")
     if not 1 <= d1 <= 10:
@@ -151,15 +156,16 @@ def read_dataset_info(path):
 
 
 def weights_to_export_dir(weights0, weights1, out_dir, scene, threshold, num_samples, allow_pickle=False, encoding=None,
-                          sampler="FromClassifiedDepthAdaptive", sampling_loss="BCEWithLogitsLoss"):
+                          sampler="FromClassifiedDepthAdaptive", sampling_loss="BCEWithLogitsLoss", depth_cells=128):
     """encoding: parse_encoding's band counts; None keeps the scene's (posEncArgs [10-4, 10-4] unless it says otherwise).
-    sampler / sampling_loss: rayMarchSampler and losses[0] of the run (onnx_weights.write_export_dir)."""
+    sampler / sampling_loss: rayMarchSampler and losses[0] of the run (onnx_weights.write_export_dir).  depth_cells: the
+    run's multiDepthFeatures, the sampling net's output width."""
     sd0, sd1 = load_weights_file(weights0, allow_pickle), load_weights_file(weights1, allow_pickle)
     if encoding is not None:
         (p0, d0), (p, d) = encoding
         # the sampling net's 0 means "the shading net's count" in the scene: zero bands are -1 there
         scene = dict(scene, n_freq_pos=p, n_freq_dir=d, n_freq_pos0=p0 if p0 > 0 else -1, n_freq_dir0=d0 if d0 > 0 else -1)
-    check_state_dicts(sd0, sd1, encoding)
+    check_state_dicts(sd0, sd1, encoding, depth_cells)
     write_export_dir(out_dir, scene, sd0, sd1, float(threshold), int(num_samples), sampler=sampler, sampling_loss=sampling_loss)
     return sd0, sd1
 
@@ -201,6 +207,8 @@ def main(argv=None):
     ap.add_argument("--z-far", type=float, default=1.0, help="zFar of a one-network run")
     ap.add_argument("--sampling-loss", default="BCEWithLogitsLoss", choices=tuple(PDF_TRANSFORMS),
                     help="losses[0] of a FromClassifiedDepth run: sigmoid (BCEWithLogitsLoss) or softmax (the CrossEntropy losses)")
+    ap.add_argument("--depth-cells", type=int, default=128, choices=DEPTH_CELLS,
+                    help="multiDepthFeatures of the run: the depth cells D the sampling net classifies (its output width)")
     a = ap.parse_args(argv)
     if a.sampler == "LinearlySpacedZNearZFar":
         enc = None
@@ -217,7 +225,7 @@ def main(argv=None):
         split = lambda v, d: tuple(x.strip() for x in (v or d).strip("[]").split(","))
         encoding = parse_encoding(split(a.pos_enc, "nerf,nerf"), split(a.pos_enc_args, "10-4,10-4"))
     weights_to_export_dir(a.weights0, a.weights1, a.out, read_dataset_info(a.dataset_info), a.threshold, a.samples, a.allow_pickle,
-                          encoding, sampler=a.sampler, sampling_loss=a.sampling_loss)
+                          encoding, sampler=a.sampler, sampling_loss=a.sampling_loss, depth_cells=a.depth_cells)
     print(f"wrote {a.out}")
 
 

@@ -65,6 +65,7 @@ struct adn_ctx {
   adn_scene scene{};
   SceneDev sc{};
   Buf zlut;                       // [128] world depth of the cell centres (log warp)
+  Buf zlut_cells;                 // the same tables for D = 32, 64 and 256 depth cells, one after another (cell_table)
   Buf zlut_dense;                 // [dense_K]
   int dense_K = 0;
   Buf zlin;                       // linear_depths(K) of every K = 1..128, the table of K at K (K - 1) / 2 (sampler 2)
@@ -86,6 +87,7 @@ struct adn_ctx {
   bool prof_linear = false;       // the profiled render ran sampler 2 (rays in slot 0, slot 1 unused)
   int pdf_transform = kPdfSigmoid;   // adn_set_option "pdf_transform": what FromClassifiedDepth applies to raw0 first
   // scratch
+  Buf raw0_pad;                   // D < 128: the sampling MLP's rows at its 128-column stride, before the copy to raw0 [N, D]
   Buf tiles0, raw0, ray_o, ray_d, ray_dirs, count, offset, rayidx, zbuf, zpbuf, tiles1, raw1, s2scratch, rgba, metric, flip, iwssim;
   Buf dirs, rgb, nsamples;        // device side of the *_host entry points
   Buf budget_keys, budget_work, budget_thr;   // sample budget: candidate keys, histograms + select state, t*
@@ -283,9 +285,10 @@ adn_status upload(adn_ctx* ctx, Net& net, const std::vector<uint8_t>& wblob, con
 // The layer programs of the two networks are derived here, from the tensor shapes, and nowhere else in the library.
 //
 // Sampling net: BaseNet without skips (src/models.py:71-76,183-195): layers.{i}.weight/bias, D = 1-12 layers, n_in <= 128
-// inputs, every hidden layer W = 128 or 256 wide, 128 or 256 outputs.  Layer 0 reads the two input blocks, every other
-// layer the W/64 hidden blocks (split precision: in shared memory, overwritten in place by its epilogue; plain bf16: in
-// registers).
+// inputs, every hidden layer W = 128 or 256 wide, 32, 64, 128 or 256 outputs (the depth cells, multiDepthFeatures); 32 and
+// 64 outputs are padded to one 128-row N half with zero weights and biases, so the kernel writes rows of 128 columns.
+// Layer 0 reads the two input blocks, every other layer the W/64 hidden blocks (split precision: in shared memory,
+// overwritten in place by its epilogue; plain bf16: in registers).
 adn_status build_net0(adn_ctx* ctx) {
   Net& net = ctx->net[0];
   auto bad = [&](const std::string& msg) { return fail(ctx, ADN_ERR_INVALID, "sampling net: " + msg); };
@@ -318,8 +321,9 @@ adn_status build_net0(adn_ctx* ctx) {
                  std::to_string(width) + ")");
     if (!last && n_out != 128 && n_out != 256)
       return bad(name + ".weight has " + std::to_string(n_out) + " outputs; the hidden width must be 128 or 256");
-    if (last && n_out != 128 && n_out != 256)
-      return bad(name + ".weight has " + std::to_string(n_out) + " outputs; the output width must be 128 or 256");
+    if (last && n_out != 32 && n_out != 64 && n_out != 128 && n_out != 256)
+      return bad(name + ".weight has " + std::to_string(n_out) + " outputs; the output width (the depth cells D, "
+                 "multiDepthFeatures) must be 32, 64, 128 or 256");
     prev = n_out;
     MlpLayer& L = P.layers[l];
     std::vector<Seg> segs;
@@ -334,14 +338,16 @@ adn_status build_net0(adn_ctx* ctx) {
       // 16-wide K steps that hold data; block 0 keeps at least one (it initialises the accumulator)
       L.k_cnt[i] = uint8_t(std::max(i == 0 ? 1 : 0, (segs[i].valid + 15) / 16));
     }
-    L.n_half = uint8_t(n_out / 128);
+    L.n_half = uint8_t((n_out + 127) / 128);
     L.flags = last ? uint8_t(LF_FINAL_RAW) : uint8_t(LF_RELU | LF_OUT_ACT);
     L.w_off = uint32_t(wblob.size());
     pack_layer(W->data.data(), n_out, k_in, segs, nsplit, L, wblob);
-    L.bias_off = uint32_t(push_floats(fblob, B->data.data(), B->data.size()));
+    std::vector<float> bias(size_t(L.n_half) * 128, 0.0f);   // zero rows past D = 32 / 64 outputs
+    std::copy(B->data.begin(), B->data.end(), bias.begin());
+    L.bias_off = uint32_t(push_floats(fblob, bias.data(), bias.size()));
     if (last) {
       net.n_out = n_out;
-      P.out_cols = n_out;
+      P.out_cols = int(L.n_half) * 128;   // D < 128: rows padded to one 128-row half (zero weights and biases)
     }
   }
   P.in = sampling_tiles(net.n_in, nsplit);
@@ -557,12 +563,48 @@ std::optional<CameraRays> camera_rays(const adn_ctx* ctx, int W, int H, int row0
 
 int64_t pad128(int64_t n) { return (n + 127) / 128 * 128; }
 
+// D, the depth cells of raw0 (multiDepthFeatures): the sampling net's outputs, 128 while none is set.
+int depth_cells(const adn_ctx* ctx) { return ctx->net[0].ready ? ctx->net[0].n_out : 128; }
+
+// The adaptive depth table of D cells: zlut at D = 128, else its slice of zlut_cells (32, then 64, then 256 entries).
+const float* cell_table(const adn_ctx* ctx, int D) {
+  if (D == 128) return ctx->zlut.as<float>();
+  return ctx->zlut_cells.as<float>() + (D == 32 ? 0 : D == 64 ? 32 : 96);
+}
+
+// The adaptive depth table of D cells as adn_create uploads it: LogTransform.to_world((c + 0.5) / D)
+// (depth_transformations.py:37-48, nerf_raymarch_common.py:738-742), pow in double, the rest in fp32; on NDC scenes
+// (FromClassifiedDepthAdaptiveNoDepthRange, :826-833) the cell centre itself.  (c + 0.5) * (1 / D) is exact for D a power of 2.
+std::vector<float> cell_depths(const adn_scene& sc, int D) {
+  std::vector<float> lut(D);
+  const double max_v = double(sc.depth_range[1]) - double(sc.depth_range[0]);
+  for (int i = 0; i < D; ++i) {
+    const float z = (float(i) + 0.5f) * (1.0f / float(D));
+    const float w = float(std::pow(max_v + 1.0, double(z)));
+    lut[i] = sc.use_ndc ? z : (w - 1.0f) + sc.depth_range[0];
+  }
+  return lut;
+}
+
+// Runs the sampling MLP into raw0 [rows, D].  At D < 128 the kernel writes rows of 128 columns (the padded N half) into
+// ctx->raw0_pad, and a strided copy keeps the first D of each.
+adn_status run_mlp0(adn_ctx* ctx, const uint8_t* tiles, float* raw0, long long rows, cudaStream_t st);
+
 adn_status run_mlp(adn_ctx* ctx, int id, const uint8_t* tiles, float* out, const long long* rows_dev, long long rows,
                    cudaStream_t st, const EncodeParams* enc = nullptr) {
   Net& n = ctx->net[id];
   const cudaError_t e = launch_mlp(n.prog, n.wblob.as<uint8_t>(), tiles, out, rows_dev, rows, ctx->d_err, ctx->num_sms, st, enc);
   if (e != cudaSuccess) return cuda_fail(ctx, e, id == 0 ? "launch sampling MLP" : "launch shading MLP");
   ctx->stats.kernel_launches++;
+  return ADN_OK;
+}
+
+adn_status run_mlp0(adn_ctx* ctx, const uint8_t* tiles, float* raw0, long long rows, cudaStream_t st) {
+  const int D = ctx->net[0].n_out;
+  if (D >= 128) return run_mlp(ctx, 0, tiles, raw0, nullptr, rows, st);
+  adn_status s = ensure(ctx, ctx->raw0_pad, size_t(rows) * 128 * 4);
+  if (s != ADN_OK || (s = run_mlp(ctx, 0, tiles, ctx->raw0_pad.as<float>(), nullptr, rows, st)) != ADN_OK) return s;
+  ADN_CUDA(ctx, cudaMemcpy2DAsync(raw0, size_t(D) * 4, ctx->raw0_pad.p, 128 * 4, size_t(D) * 4, size_t(rows), cudaMemcpyDeviceToDevice, st));
   return ADN_OK;
 }
 
@@ -582,15 +624,15 @@ struct RenderCall {
   float* d_rgb = nullptr;           // [n_rays, 3]
   uint8_t* d_rgba8 = nullptr;       // [n_rays, 4]
   int32_t* d_nsamples = nullptr;    // [n_rays]
-  float* d_oracle_w = nullptr;      // [n_rays, 128]: the sampling net's output
+  float* d_oracle_w = nullptr;      // [n_rays, D]: the sampling net's output
   adn_aux_outputs aux{};            // all null: none
   cudaStream_t st;
   RenderCall(const float* pose_, const float* rot_, int64_t n_rays_, float thr_, int K_, void* stream)
       : pose(pose_), rot(rot_), n_rays(n_rays_), thr(thr_), K(K_), st(static_cast<cudaStream_t>(stream)) {}
 };
 
-// Rays [r0, r0 + chunk) of a call (fewer at its end): the ray source and every output start at ray r0.
-RenderCall chunk_of(const RenderCall& call, int64_t r0, int64_t chunk) {
+// Rays [r0, r0 + chunk) of a call (fewer at its end): the ray source and every output start at ray r0.  D: raw0's row width.
+RenderCall chunk_of(const RenderCall& call, int64_t r0, int64_t chunk, int D) {
   RenderCall c = call;
   c.n_rays = std::min(chunk, call.n_rays - r0);
   if (c.d_dirs) c.d_dirs += 3 * r0;
@@ -599,7 +641,7 @@ RenderCall chunk_of(const RenderCall& call, int64_t r0, int64_t chunk) {
   if (c.d_rgb) c.d_rgb += 3 * r0;
   if (c.d_rgba8) c.d_rgba8 += 4 * r0;
   if (c.d_nsamples) c.d_nsamples += r0;
-  if (c.d_oracle_w) c.d_oracle_w += 128 * r0;
+  if (c.d_oracle_w) c.d_oracle_w += D * r0;
   for (float** p : {&c.aux.d_weights, &c.aux.d_alpha, &c.aux.d_z_vals})
     if (*p) *p += r0 * c.K;
   for (float** p : {&c.aux.d_depth_map, &c.aux.d_acc_map, &c.aux.d_disp_map, &c.aux.d_depth_est})
@@ -627,14 +669,14 @@ const ViewTable* views_of(const RenderCall& c, ViewTable& t) {
   return &t;
 }
 
-// Stage 0 + the sampling MLP of one chunk, stream ordered.  Writes the chunk's raw0 [n, 128] (the caller's
+// Stage 0 + the sampling MLP of one chunk, stream ordered.  Writes the chunk's raw0 [n, D] (the caller's
 // d_oracle_weights when given, else the context's scratch from ray w on) and its ray origins / directions (scratch from ray
 // w on).  w is 0 unless a sample budget keeps the whole call's rows.  timing: record ev[0..2].
 adn_status run_stages_0_1(adn_ctx* ctx, const RenderCall& c, int64_t w, bool timing) {
   const Net& n0 = ctx->net[0];
   adn_status s = ensure(ctx, ctx->tiles0, size_t(pad128(c.n_rays) / 128) * n0.prog.in.tile_bytes());
   if (s != ADN_OK) return s;
-  float* raw0 = c.d_oracle_w ? c.d_oracle_w : ctx->raw0.as<float>() + 128 * w;
+  float* raw0 = c.d_oracle_w ? c.d_oracle_w : ctx->raw0.as<float>() + int64_t(depth_cells(ctx)) * w;
   uint8_t* tiles0 = ctx->tiles0.as<uint8_t>();
   ViewTable vt{};
   if (timing) cudaEventRecord(ctx->ev[0], c.st);
@@ -645,7 +687,7 @@ adn_status run_stages_0_1(adn_ctx* ctx, const RenderCall& c, int64_t w, bool tim
   ctx->stats.kernel_launches++;
   if (timing) cudaEventRecord(ctx->ev[1], c.st);
   // stage 1
-  if ((s = run_mlp(ctx, 0, tiles0, raw0, nullptr, c.n_rays, c.st)) != ADN_OK) return s;
+  if ((s = run_mlp0(ctx, tiles0, raw0, c.n_rays, c.st)) != ADN_OK) return s;
   if (timing) cudaEventRecord(ctx->ev[2], c.st);
   return ADN_OK;
 }
@@ -695,7 +737,8 @@ adn_status run_stages_2_5(adn_ctx* ctx, const RenderCall& c, int64_t w, const fl
   if (!fused_enc && (s = ensure(ctx, ctx->tiles1, size_t(pad128(cap) / 128) * ctx->net[1].prog.in.tile_bytes())) != ADN_OK) return s;
   if ((s = ensure(ctx, ctx->raw1, size_t(pad128(cap)) * 16)) != ADN_OK) return s;
 
-  float* raw0 = linear ? nullptr : c.d_oracle_w ? c.d_oracle_w : ctx->raw0.as<float>() + 128 * w;
+  const int D = depth_cells(ctx);
+  float* raw0 = linear ? nullptr : c.d_oracle_w ? c.d_oracle_w : ctx->raw0.as<float>() + int64_t(D) * w;
   const float* ray_o = ctx->ray_o.as<float>() + 3 * w;
   const float* ray_d = ctx->ray_d.as<float>() + 3 * w;
   int32_t* count = c.d_nsamples ? c.d_nsamples : ctx->count.as<int32_t>();
@@ -715,8 +758,8 @@ adn_status run_stages_2_5(adn_ctx* ctx, const RenderCall& c, int64_t w, const fl
   } else if (dense) {
     ADN_CUDA(ctx, launch_stage2_dense(n, K, count, offset, total, c.st));
   } else {
-    ADN_CUDA(ctx, launch_stage2(raw0, n, c.thr, K, ctx->zlut.as<float>(), count, offset, nullptr, rayidx, z,
-                                ctx->zpbuf.as<float>(), total, ctx->s2scratch.p, &ctx->s2sync, c.st, d_thr));
+    ADN_CUDA(ctx, launch_stage2(raw0, n, c.thr, K, cell_table(ctx, D), count, offset, nullptr, rayidx, z, ctx->zpbuf.as<float>(),
+                                total, ctx->s2scratch.p, &ctx->s2sync, c.st, d_thr, D));
   }
   ctx->stats.kernel_launches++;
   if (timing) cudaEventRecord(ctx->ev[3], c.st);
@@ -765,8 +808,15 @@ adn_status render(adn_ctx* ctx, const RenderCall& call) {
   const bool linear = ctx->sampler == 2;   // LinearlySpacedZNearZFar: one network, in the shading slot
   if (linear && !ctx->net[1].ready) return fail(ctx, ADN_ERR_NO_WEIGHTS, "render: set the shading network (slot 1) first");
   if (!linear && (!ctx->net[0].ready || !ctx->net[1].ready)) return fail(ctx, ADN_ERR_NO_WEIGHTS, "render: set both networks first");
-  if (!linear && (ctx->net[0].n_in != ctx->n_feat0 || ctx->net[0].n_out != 128))
-    return fail(ctx, ADN_ERR_INVALID, "render: sampling net must be " + std::to_string(ctx->n_feat0) + " -> 128 for this scene's encoding");
+  if (!linear && ctx->net[0].n_in != ctx->n_feat0)
+    return fail(ctx, ADN_ERR_INVALID, "render: sampling net must have " + std::to_string(ctx->n_feat0) + " inputs for this scene's encoding");
+  const int D = linear ? 128 : depth_cells(ctx);   // depth cells of raw0 (multiDepthFeatures)
+  if (D != 128 && ctx->sampler == 1)
+    return fail(ctx, ADN_ERR_INVALID, "render: sampler 1 (FromClassifiedDepth) supports 128 depth cells only; this sampling net has " +
+                                          std::to_string(D));
+  if (D != 128 && ctx->sampling_view)
+    return fail(ctx, ADN_ERR_INVALID, "render: option sampling_view supports 128 depth cells only; this sampling net has " +
+                                          std::to_string(D));
   if (linear && ctx->sampling_view)
     return fail(ctx, ADN_ERR_INVALID, "render: sampler 2 (LinearlySpacedZNearZFar) runs no sampling net, so option sampling_view has nothing to draw");
   if (linear && call.d_oracle_w)
@@ -774,9 +824,12 @@ adn_status render(adn_ctx* ctx, const RenderCall& call) {
   if (linear && ctx->sample_budget > 0)
     return fail(ctx, ADN_ERR_INVALID, "render: sampler 2 (LinearlySpacedZNearZFar) places K samples on every ray; it takes no sample_budget");
   const bool fixed_k = ctx->sampler != 0;   // FromClassifiedDepth and LinearlySpacedZNearZFar ignore thr
-  if (K < 1 || K > 128 || (!fixed_k && thr < 0.0f)) return fail(ctx, ADN_ERR_INVALID, "render: need 1 <= K <= 128 and thr >= 0");
-  if (!fixed_k && thr == 0.0f && K != 128)
-    return fail(ctx, ADN_ERR_INVALID, "render: dense mode (thr == 0) needs K == 128 (one sample per depth cell)");
+  if (K < 1 || K > std::min(D, 128) || (!fixed_k && thr < 0.0f))
+    return fail(ctx, ADN_ERR_INVALID, "render: need 1 <= K <= " + std::to_string(std::min(D, 128)) + " and thr >= 0" +
+                                          (D != 128 ? " (" + std::to_string(D) + " depth cells)" : std::string()));
+  if (!fixed_k && thr == 0.0f && K != D)
+    return fail(ctx, ADN_ERR_INVALID, "render: dense mode (thr == 0) needs K == " + std::to_string(D) + " (one sample per depth cell)" +
+                                          (D > 128 ? "; K is at most 128, so 256 depth cells have no dense mode" : ""));
   const bool view = ctx->sampling_view;
   if (view) {
     const adn_aux_outputs& a = call.aux;
@@ -797,7 +850,7 @@ adn_status render(adn_ctx* ctx, const RenderCall& call) {
                                           " rays of the call (every ray keeps at least one sample)");
   if (budget > 0 && n_rays * (K - 1) >= (int64_t(1) << 32))
     return fail(ctx, ADN_ERR_INVALID, "render: sample_budget supports at most 2^32 - 1 candidate samples (N * (K - 1)) per call");
-  if (budget > 0 && (reinterpret_cast<uintptr_t>(call.d_oracle_w) & 15u))
+  if (budget > 0 && D == 128 && (reinterpret_cast<uintptr_t>(call.d_oracle_w) & 15u))
     return fail(ctx, ADN_ERR_INVALID, "render: sample_budget needs 16-byte aligned d_oracle_weights rows");
   if (n_rays == 0 && !joins) return ADN_OK;
   if (ctx->scene.use_ndc && n_rays > 0) {
@@ -828,13 +881,14 @@ adn_status render(adn_ctx* ctx, const RenderCall& call) {
   // raw0 / ray_o / ray_d: one chunk's worth, or with a sample budget the whole call's (the threshold is chosen over all of
   // raw0 before any chunk runs stage 2)
   const int64_t span = budget > 0 ? n_rays : std::min(chunk, n_rays);
-  if (!linear && !call.d_oracle_w && (s = ensure(ctx, ctx->raw0, size_t(span) * 128 * 4)) != ADN_OK) return s;
+  if (!linear && !call.d_oracle_w && (s = ensure(ctx, ctx->raw0, size_t(span) * D * 4)) != ADN_OK) return s;
+  if (!linear && D < 128 && (s = ensure(ctx, ctx->raw0_pad, size_t(std::min(chunk, n_rays)) * 128 * 4)) != ADN_OK) return s;
   if (linear && ctx->scene.use_ndc && (s = ensure(ctx, ctx->ray_dirs, size_t(span) * 12)) != ADN_OK) return s;
   if ((s = ensure(ctx, ctx->ray_o, size_t(span) * 12)) != ADN_OK) return s;
   if ((s = ensure(ctx, ctx->ray_d, size_t(span) * 12)) != ADN_OK) return s;
   if (budget == 0) {
     for (int64_t r0 = 0; r0 < n_rays; r0 += chunk) {
-      const RenderCall c = chunk_of(call, r0, chunk);
+      const RenderCall c = chunk_of(call, r0, chunk, D);
       const bool timing = ctx->profile && r0 == 0;
       if ((s = linear ? run_rays(ctx, c, timing) : run_stages_0_1(ctx, c, 0, timing)) != ADN_OK) return s;
       if ((s = view ? run_view(ctx, c, timing) : run_stages_2_5(ctx, c, 0, nullptr, timing)) != ADN_OK) return s;
@@ -846,16 +900,16 @@ adn_status render(adn_ctx* ctx, const RenderCall& call) {
   if ((s = ensure(ctx, ctx->budget_thr, sizeof(float))) != ADN_OK) return s;
   float* d_thr = ctx->budget_thr.as<float>();
   for (int64_t r0 = 0; r0 < n_rays; r0 += chunk)
-    if ((s = run_stages_0_1(ctx, chunk_of(call, r0, chunk), r0, ctx->profile && r0 == 0)) != ADN_OK) return s;
+    if ((s = run_stages_0_1(ctx, chunk_of(call, r0, chunk, D), r0, ctx->profile && r0 == 0)) != ADN_OK) return s;
   if (ctx->profile) cudaEventRecord(ctx->ev[7], call.st);   // the selection is timed with stage 2 of the first chunk
   int launches = 0;
   ADN_CUDA(ctx, launch_budget_threshold(call.d_oracle_w ? call.d_oracle_w : ctx->raw0.as<float>(), n_rays, thr, K, budget,
                                         ctx->budget_keys.as<uint32_t>(), ctx->budget_work.p, d_thr, ctx->num_sms, call.st, &launches,
-                                        &ctx->group));
+                                        &ctx->group, D));
   ctx->stats.kernel_launches += launches;
   if (ctx->group.failed_round >= 0) return group_fail(ctx, "render");
   for (int64_t r0 = 0; r0 < n_rays; r0 += chunk)
-    if ((s = run_stages_2_5(ctx, chunk_of(call, r0, chunk), r0, d_thr, ctx->profile && r0 == 0)) != ADN_OK) return s;
+    if ((s = run_stages_2_5(ctx, chunk_of(call, r0, chunk, D), r0, d_thr, ctx->profile && r0 == 0)) != ADN_OK) return s;
   return ADN_OK;
 }
 
@@ -1001,23 +1055,24 @@ adn_status adn_create(adn_ctx** out, const adn_scene* scene, int device) {
   ctx->n_feat0 = 6 + 6 * (nfp0 + nfd0);
   ctx->sc.ndc = scene->use_ndc ? 1 : 0;
   if (scene->use_ndc && scene->ndc_w > 0 && scene->ndc_h > 0) set_ndc_projection(ctx, scene->ndc_w, scene->ndc_h, scene->ndc_focal);
-  // z LUT: LogTransform.to_world((cell + .5)/128) (depth_transformations.py:37-48), pow in double, rest in fp32
-  float lut[128];
-  const double max_v = double(scene->depth_range[1]) - double(scene->depth_range[0]);
-  for (int i = 0; i < 128; ++i) {
-    const float z = (float(i) + 0.5f) * (1.0f / 128.0f);
-    const float w = float(std::pow(max_v + 1.0, double(z)));
-    // FromClassifiedDepthAdaptiveNoDepthRange (NDC configs): the cell centre itself (nerf_raymarch_common.py:826-833)
-    lut[i] = scene->use_ndc ? z : (w - 1.0f) + scene->depth_range[0];
-  }
+  // z LUT of the default 128 depth cells (cell_depths)
+  const std::vector<float> lut = cell_depths(*scene, 128);
   // sampler 2's depth tables, one per K, so that no render uploads one
   std::vector<float> zlin;
   for (int K = 1; K <= 128; ++K) {
     const std::vector<float> t = linear_depths(*scene, K);
     zlin.insert(zlin.end(), t.begin(), t.end());
   }
-  bool ok = ensure(ctx, ctx->zlut, sizeof(lut)) == ADN_OK &&
-            cudaMemcpy(ctx->zlut.p, lut, sizeof(lut), cudaMemcpyHostToDevice) == cudaSuccess &&
+  // the tables of the other depth-cell counts (multiDepthFeatures 32, 64, 256), in cell_table's order
+  std::vector<float> zcells;
+  for (int D : {32, 64, 256}) {
+    const std::vector<float> t = cell_depths(*scene, D);
+    zcells.insert(zcells.end(), t.begin(), t.end());
+  }
+  bool ok = ensure(ctx, ctx->zlut, lut.size() * 4) == ADN_OK &&
+            cudaMemcpy(ctx->zlut.p, lut.data(), lut.size() * 4, cudaMemcpyHostToDevice) == cudaSuccess &&
+            ensure(ctx, ctx->zlut_cells, zcells.size() * 4) == ADN_OK &&
+            cudaMemcpy(ctx->zlut_cells.p, zcells.data(), zcells.size() * 4, cudaMemcpyHostToDevice) == cudaSuccess &&
             ensure(ctx, ctx->zlin, zlin.size() * 4) == ADN_OK &&
             cudaMemcpy(ctx->zlin.p, zlin.data(), zlin.size() * 4, cudaMemcpyHostToDevice) == cudaSuccess &&
             ensure(ctx, ctx->total, sizeof(long long)) == ADN_OK &&
@@ -1349,21 +1404,24 @@ adn_status adn_mlp0_forward(adn_ctx* ctx, const float* d_x0, int64_t n_rays, flo
   if (s != ADN_OK || (s = ensure(ctx, ctx->tiles0, size_t(pad128(n_rays) / 128) * n.prog.in.tile_bytes())) != ADN_OK) return s;
   ADN_CUDA(ctx, launch_pack_rows(d_x0, n_rays, nullptr, n.n_in, n.prog.in, static_cast<uint8_t*>(ctx->tiles0.p), ctx->num_sms, st));
   ctx->stats.kernel_launches++;
-  return run_mlp(ctx, 0, static_cast<uint8_t*>(ctx->tiles0.p), d_raw0, nullptr, n_rays, st);
+  return run_mlp0(ctx, static_cast<uint8_t*>(ctx->tiles0.p), d_raw0, n_rays, st);
 }
 
 adn_status adn_stage2_sample(adn_ctx* ctx, const float* d_raw0, int64_t n_rays, float thr, int K, int32_t* d_count,
                              int32_t* d_offset, int32_t* d_cell, int32_t* d_ray, float* d_z, float* d_zp, int64_t* d_total,
                              void* stream) {
-  if (!ctx || !d_total || n_rays < 0 || K < 1 || K > 128 || !(thr > 0.0f) ||
+  const int D = ctx ? depth_cells(ctx) : 128;
+  if (!ctx || !d_total || n_rays < 0 || K < 1 || K > std::min(D, 128) || !(thr > 0.0f) ||
       (n_rays > 0 && (!d_raw0 || !d_count || !d_offset || !d_ray || !d_z || !d_zp)))
-    return fail(ctx, ADN_ERR_INVALID, "stage2: bad arguments (adaptive path needs thr > 0)");
+    return fail(ctx, ADN_ERR_INVALID, "stage2: bad arguments (adaptive path needs thr > 0 and 1 <= K <= " +
+                                          std::to_string(std::min(D, 128)) + ")");
   ADN_CUDA(ctx, cudaSetDevice(ctx->device));
   CallOrder order(ctx, static_cast<cudaStream_t>(stream));
   adn_status s = order.begin("stage2");
   if (s != ADN_OK || (s = ensure(ctx, ctx->s2scratch, stage2_scratch_bytes(n_rays))) != ADN_OK) return s;
-  ADN_CUDA(ctx, launch_stage2(d_raw0, n_rays, thr, K, ctx->zlut.as<float>(), d_count, d_offset, d_cell, d_ray, d_z, d_zp,
-                              reinterpret_cast<long long*>(d_total), ctx->s2scratch.p, &ctx->s2sync, static_cast<cudaStream_t>(stream)));
+  ADN_CUDA(ctx, launch_stage2(d_raw0, n_rays, thr, K, cell_table(ctx, D), d_count, d_offset, d_cell, d_ray, d_z, d_zp,
+                              reinterpret_cast<long long*>(d_total), ctx->s2scratch.p, &ctx->s2sync, static_cast<cudaStream_t>(stream),
+                              nullptr, D));
   ctx->stats.kernel_launches++;
   return ADN_OK;
 }
@@ -1443,11 +1501,13 @@ adn_status adn_sampling_view(adn_ctx* ctx, const float* d_raw0, int64_t n_rays, 
 
 adn_status adn_budget_threshold(adn_ctx* ctx, const float* d_raw0, int64_t n_rays, float thr_min, int K, int64_t max_samples,
                                 float* d_thr, void* stream) {
-  if (!ctx || !d_thr || n_rays < 0 || (n_rays > 0 && !d_raw0) || K < 1 || K > 128 || !(thr_min > 0.0f) || max_samples < n_rays)
-    return fail(ctx, ADN_ERR_INVALID, "budget_threshold: bad arguments (need thr_min > 0, 1 <= K <= 128, max_samples >= n_rays)");
+  const int D = ctx ? depth_cells(ctx) : 128;
+  if (!ctx || !d_thr || n_rays < 0 || (n_rays > 0 && !d_raw0) || K < 1 || K > std::min(D, 128) || !(thr_min > 0.0f) || max_samples < n_rays)
+    return fail(ctx, ADN_ERR_INVALID, "budget_threshold: bad arguments (need thr_min > 0, 1 <= K <= " + std::to_string(std::min(D, 128)) +
+                                          ", max_samples >= n_rays)");
   if (n_rays * (K - 1) >= (int64_t(1) << 32))
     return fail(ctx, ADN_ERR_INVALID, "budget_threshold: at most 2^32 - 1 candidate samples (N * (K - 1))");
-  if (reinterpret_cast<uintptr_t>(d_raw0) & 15u) return fail(ctx, ADN_ERR_INVALID, "budget_threshold: d_raw0 must be 16-byte aligned");
+  if (D == 128 && (reinterpret_cast<uintptr_t>(d_raw0) & 15u)) return fail(ctx, ADN_ERR_INVALID, "budget_threshold: d_raw0 must be 16-byte aligned");
   ADN_CUDA(ctx, cudaSetDevice(ctx->device));
   CallOrder order(ctx, static_cast<cudaStream_t>(stream));
   adn_status s = order.begin("budget_threshold");
@@ -1457,7 +1517,7 @@ adn_status adn_budget_threshold(adn_ctx* ctx, const float* d_raw0, int64_t n_ray
   int launches = 0;
   ADN_CUDA(ctx, launch_budget_threshold(d_raw0, n_rays, thr_min, K, max_samples, static_cast<uint32_t*>(ctx->budget_keys.p),
                                         ctx->budget_work.p, d_thr, ctx->num_sms, static_cast<cudaStream_t>(stream), &launches,
-                                        &ctx->group));
+                                        &ctx->group, D));
   ctx->stats.kernel_launches += launches;
   return ctx->group.failed_round >= 0 ? group_fail(ctx, "budget_threshold") : ADN_OK;
 }
@@ -1494,8 +1554,8 @@ adn_status adn_stage5_composite_aux(adn_ctx* ctx, const float* d_raw1, const flo
                                     float* d_rgb, uint8_t* d_rgba8, const adn_aux_outputs* aux, void* stream) {
   const adn_aux_outputs a = aux ? *aux : adn_aux_outputs{};
   const bool reads_z = a.d_z_vals || a.d_depth_map || a.d_disp_map || a.d_depth_est;
-  if (!ctx || n_rays < 0 || K < 1 || K > 128 || (dense && K != 128))
-    return fail(ctx, ADN_ERR_INVALID, "stage5: bad arguments (dense mode needs K == 128)");
+  if (!ctx || n_rays < 0 || K < 1 || K > 128 || (dense && K != 128 && K != depth_cells(ctx)))
+    return fail(ctx, ADN_ERR_INVALID, "stage5: bad arguments (dense mode needs K == 128 or K == the sampling net's depth cells)");
   if (n_rays > 0 && (!d_raw1 || !d_zp || (!dense && (!d_offset || !d_count || (reads_z && !d_z)))))
     return fail(ctx, ADN_ERR_INVALID, "stage5: bad arguments");
   ADN_CUDA(ctx, cudaSetDevice(ctx->device));
@@ -1630,7 +1690,7 @@ adn_status adn_create_from_export_dir(adn_ctx** out, const char* dir, int device
   *out = nullptr;
   adn::ExportDir ex;
   std::string err;
-  if (!adn::load_export_dir(dir, ex, err)) {
+  if (!adn::load_export_dir(dir, ex, err) || !adn::check_depth_cells(ex, err)) {
     std::fprintf(stderr, "adanerf_b200: %s\n", err.c_str());
     return ADN_ERR_IO;
   }

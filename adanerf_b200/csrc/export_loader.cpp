@@ -348,6 +348,25 @@ bool load_export_dir(const std::string& dir_in, ExportDir& out, std::string& err
       if (i == 0 && idx == 1) width = int(t.cols);
     }
     if (i == 0 && depth == 1) width = width0;
+    if (i == 0) {
+      // multiDepthFeatures = [D, D] (src/features.py:250-252, nerf_raymarch_common.py:674-676): the depth cells the sampling
+      // net classifies; a config without the key trained the reference's default, 128.  Raw / RawSigmoid size the sampling
+      // net's output by the first entry and FromClassifiedDepthAdaptive places cells by the second, so they must agree
+      // (and with model0.onnx: check_depth_cells).
+      int cells = 128;
+      auto md = cfg.find("multiDepthFeatures");
+      if (md != cfg.end()) {
+        const auto items = list_items(md->second);
+        const bool two = items.size() == 2 && !items[0].empty() && items[0] == items[1] &&
+                         items[0].find_first_not_of("0123456789") == std::string::npos;
+        cells = two ? std::atoi(items[0].c_str()) : -1;
+        if (cells != 32 && cells != 64 && cells != 128 && cells != 256) {
+          err = "config.ini: multiDepthFeatures = " + strip(md->second) + ": need two equal entries, each 32, 64, 128 or 256";
+          return false;
+        }
+      }
+      out.depth_cells = cells;
+    }
     const std::string onnx = one_net ? "model0.onnx" : "model" + std::to_string(i) + ".onnx";
     for (const auto& [key, have] : {std::pair<const char*, int>{"layers", depth}, {"layerWidth", width}}) {
       auto it = cfg.find(key);
@@ -363,6 +382,23 @@ bool load_export_dir(const std::string& dir_in, ExportDir& out, std::string& err
     }
   }
   return true;
+}
+
+bool check_depth_cells(const ExportDir& ex, std::string& err) {
+  if (ex.sampler == 2) return true;   // a one-network export has no sampling net
+  int depth = 0, rows = 0;
+  for (const NamedTensor& t : ex.nets[0]) {
+    if (t.name.compare(0, 7, "layers.") != 0 || t.name.size() < 7 || t.name.compare(t.name.size() - 7, 7, ".weight") != 0) continue;
+    const int idx = std::atoi(t.name.c_str() + 7);
+    if (idx + 1 > depth) {
+      depth = idx + 1;
+      rows = int(t.rows);
+    }
+  }
+  if (rows == ex.depth_cells) return true;
+  err = "config.ini: multiDepthFeatures gives " + std::to_string(ex.depth_cells) + " depth cells but model0.onnx's last layer has " +
+        std::to_string(rows) + " outputs";
+  return false;
 }
 
 }  // namespace adn

@@ -135,4 +135,9 @@ bool ImageGenerator::net_shape(int net_id, int* depth, int* width, int* skip) {
   return ctx_ && adn_net_shape(ctx_, net_id, depth, width, skip) == ADN_OK;
 }
 
+int ImageGenerator::depth_cells() {
+  int n_out = 0;
+  return ctx_ && adn_net_dims(ctx_, 0, nullptr, &n_out) == ADN_OK ? n_out : 0;
+}
+
 }  // namespace adn_host

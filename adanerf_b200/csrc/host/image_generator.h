@@ -82,6 +82,8 @@ class ImageGenerator {
   bool stats(adn_stats* out);
   // The loaded network's shape (adn_net_shape): depth, width and skip layer (-1 = none).
   bool net_shape(int net_id, int* depth, int* width, int* skip);
+  // The sampling net's depth cells D (multiDepthFeatures, adn_net_dims' outputs of net 0); 0 when there is none.
+  int depth_cells();
 
  private:
   // the per-frame options every inference overload applies before it renders: rays per batch and the render-oracle view

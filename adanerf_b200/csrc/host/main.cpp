@@ -138,7 +138,9 @@ int main(int argc, char** argv) {
     const int p = id == 0 && sc.n_freq_pos0 ? sc.n_freq_pos0 : sc.n_freq_pos, q = id == 0 && sc.n_freq_dir0 ? sc.n_freq_dir0 : sc.n_freq_dir;
     char enc[32] = "?";
     if (probed) std::snprintf(enc, sizeof(enc), p < 0 && q < 0 ? "none" : "%d-%d", p < 0 ? 0 : p, q < 0 ? 0 : q);
-    std::printf("net %d: %s %d x %d, skip %d, posEnc %s\n", id, id == 0 ? "sampling" : "shading", d, w, sk, enc);
+    std::printf("net %d: %s %d x %d, skip %d, posEnc %s", id, id == 0 ? "sampling" : "shading", d, w, sk, enc);
+    if (id == 0) std::printf(", %d depth cells", gen.depth_cells());
+    std::printf("\n");
   }
   if (budget > 0 && !gen.set_sample_budget(budget)) { std::fprintf(stderr, "sample budget: %s\n", gen.last_error()); return 1; }
   if (oracle) gen.switchRenderOracle();

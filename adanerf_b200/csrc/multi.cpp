@@ -112,7 +112,7 @@ adn_status adn_multi_create_from_export_dir(adn_multi** out, const char* dir, co
   if (!out || !dir) return ADN_ERR_INVALID;
   adn::ExportDir ex;
   std::string err;
-  if (!adn::load_export_dir(dir, ex, err)) {
+  if (!adn::load_export_dir(dir, ex, err) || !adn::check_depth_cells(ex, err)) {
     std::fprintf(stderr, "adanerf_b200: %s\n", err.c_str());
     return ADN_ERR_IO;
   }

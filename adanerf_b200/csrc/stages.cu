@@ -762,6 +762,145 @@ stage2_thread_kernel(const float* __restrict__ raw0, long long n_rays, float thr
   }
 }
 
+// ---- D != 128 depth cells (multiDepthFeatures 32, 64 or 256): raw0 rows of D cells, D / 32 = C cells per lane.
+// select_cells for C cells per lane (bit l of sel[j] <-> cell C l + j), same contract: >= thr, top K by value with ties to
+// the lower cell, the arg-max cell when nothing passes.  Each pop round takes every lane's best remaining candidate (the
+// lowest j on ties), one REDUX.MAX over those heads and a ballot (ties: the lowest lane).
+template <int C>
+__device__ __forceinline__ int select_cells_c(const float (&v)[C], float thr, int K, int lane, uint32_t (&sel)[C]) {
+  uint32_t act[C];
+  int cnt = 0;
+#pragma unroll
+  for (int j = 0; j < C; ++j) {
+    act[j] = __ballot_sync(0xffffffffu, v[j] >= thr);
+    cnt += __popc(act[j]);
+  }
+  if (cnt > 0 && cnt <= K) {
+#pragma unroll
+    for (int j = 0; j < C; ++j) sel[j] = act[j];
+    return cnt;
+  }
+  const bool fallback = (cnt == 0);
+  const int need = fallback ? 1 : K;
+  uint32_t key[C];   // 0 = not a candidate (every real input has a key >= 0x007FFFFF)
+#pragma unroll
+  for (int j = 0; j < C; ++j) key[j] = (fallback || ((act[j] >> lane) & 1u)) ? order_key(v[j]) : 0u;
+  uint32_t mine = 0;
+  for (int round = 0; round < need; ++round) {
+    uint32_t head = 0u;
+    int hj = 0;
+#pragma unroll
+    for (int j = 0; j < C; ++j) {
+      hj = key[j] > head ? j : hj;
+      head = key[j] > head ? key[j] : head;
+    }
+    const uint32_t m = __reduce_max_sync(0xffffffffu, head);
+    const uint32_t who = __ballot_sync(0xffffffffu, head == m);
+    if (lane == __ffs(who) - 1) {
+      mine |= 1u << hj;
+#pragma unroll
+      for (int j = 0; j < C; ++j) key[j] = j == hj ? 0u : key[j];
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < C; ++j) sel[j] = __ballot_sync(0xffffffffu, (mine >> j) & 1u);
+  return need;
+}
+
+// Lane `lane`'s C cells of a D = 32 C row (4-byte loads: any row alignment).
+template <int C>
+__device__ __forceinline__ void ld_row_cells(const float* __restrict__ row, int lane, float (&v)[C]) {
+#pragma unroll
+  for (int j = 0; j < C; ++j) v[j] = __ldg(row + C * lane + j);
+}
+
+// Stage 2 over raw0 [n_rays, 32 C]: stage2_kernel's warp-per-ray layout, scan and look-back, with C cells per lane.
+template <int C>
+__global__ void __launch_bounds__(kS2Threads)
+stage2_cells_kernel(const float* __restrict__ raw0, long long n_rays, float thr, const float* __restrict__ d_thr, int K,
+                    const float* __restrict__ zlut, int32_t* __restrict__ count, int32_t* __restrict__ offset,
+                    int32_t* __restrict__ cell_out, int32_t* __restrict__ ray_out, float* __restrict__ z_out,
+                    float* __restrict__ zp_out, long long* __restrict__ total, unsigned long long* __restrict__ tile_state,
+                    unsigned int* __restrict__ ticket, int n_tiles, uint32_t epoch, uint32_t ticket_base) {
+  constexpr int D = 32 * C;
+  __shared__ uint32_t s_sel[kS2Rays][C];
+  __shared__ int s_cnt[kS2Rays];
+  __shared__ int s_off[kS2Rays];
+  __shared__ long long s_prefix;
+  __shared__ int s_tile;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (d_thr) thr = *d_thr;
+  if (threadIdx.x == 0) s_tile = int(atomicAdd(ticket, 1u) - ticket_base);
+  __syncthreads();
+  const int tile = s_tile;
+  const long long ray0 = (long long)tile * kS2Rays;
+
+  float rows8[8][C];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const long long r = ray0 + warp * 8 + i;
+#pragma unroll
+    for (int j = 0; j < C; ++j) rows8[i][j] = 0.0f;
+    if (r < n_rays) ld_row_cells<C>(raw0 + r * D, lane, rows8[i]);
+  }
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int rl = warp * 8 + i;
+    const long long r = ray0 + rl;
+    int cnt = 0;
+    uint32_t sel[C];
+#pragma unroll
+    for (int j = 0; j < C; ++j) sel[j] = 0u;
+    if (r < n_rays) cnt = select_cells_c<C>(rows8[i], thr, K, lane, sel);
+    if (lane == 0) {
+      s_cnt[rl] = cnt;
+#pragma unroll
+      for (int j = 0; j < C; ++j) s_sel[rl][j] = sel[j];
+    }
+  }
+  __syncthreads();
+
+  if (warp == 0) {
+    const int tile_total = s2_tile_scan(s_cnt, s_off, tile, lane, tile_state, epoch);
+    s2_lookback(&s_prefix, tile, tile_total, n_tiles, lane, tile_state, total, epoch);
+  }
+  __syncthreads();
+  const long long prefix = s_prefix;
+
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int rl = warp * 8 + i;
+    const long long r = ray0 + rl;
+    if (r >= n_rays) break;
+    const long long off = prefix + s_off[rl];
+    if (lane == 0) {
+      count[r] = s_cnt[rl];
+      offset[r] = int32_t(off);
+    }
+    const uint32_t below = (1u << lane) - 1u;
+    int rank = 0;
+    uint32_t sel[C];
+#pragma unroll
+    for (int j = 0; j < C; ++j) {
+      sel[j] = s_sel[rl][j];
+      rank += __popc(sel[j] & below);
+    }
+#pragma unroll
+    for (int j = 0; j < C; ++j) {
+      if ((sel[j] >> lane) & 1u) {
+        const int cell = C * lane + j;
+        const long long o = off + rank;
+        z_out[o] = __ldg(zlut + cell);
+        zp_out[o] = rows8[i][j];
+        if (cell_out) cell_out[o] = cell;
+        ray_out[o] = int32_t(r);
+        ++rank;
+      }
+    }
+  }
+}
+
 size_t stage2_scratch_bytes(long long n_rays) {
   const long long n_tiles = (n_rays + kS2Rays - 1) / kS2Rays;
   return size_t(n_tiles + 2) * 8;
@@ -769,8 +908,9 @@ size_t stage2_scratch_bytes(long long n_rays) {
 
 cudaError_t launch_stage2(const float* d_raw0, long long n_rays, float thr, int K, const float* d_zlut, int32_t* d_count,
                           int32_t* d_offset, int32_t* d_cell, int32_t* d_ray, float* d_z, float* d_zp, long long* d_total,
-                          void* d_scratch, Stage2Sync* sync, cudaStream_t s, const float* d_thr) {
+                          void* d_scratch, Stage2Sync* sync, cudaStream_t s, const float* d_thr, int D) {
   if (n_rays <= 0) return cudaMemsetAsync(d_total, 0, sizeof(long long), s);
+  if (D != 32 && D != 64 && D != 128 && D != 256) return cudaErrorInvalidValue;
   const int n_tiles = int((n_rays + kS2Rays - 1) / kS2Rays);
   const size_t bytes = stage2_scratch_bytes(n_rays);
   // [ticket | states]: cleared only when the buffer is new / has grown or the epoch wraps (see the state-word comment)
@@ -789,7 +929,14 @@ cudaError_t launch_stage2(const float* d_raw0, long long n_rays, float thr, int 
   sync->ticket_base += uint32_t(n_tiles);   // the launch consumes exactly n_tiles tickets (unsigned wrap-around is fine)
   // thread-per-ray kernel whenever its assumptions hold (K <= 16, 16-byte aligned rows for the cp.async fetch)
   const bool aligned = (reinterpret_cast<uintptr_t>(d_raw0) & 15u) == 0;
-  if (K <= 8 && aligned)
+#define ADN_S2_CELLS(C)                                                                                                       \
+  stage2_cells_kernel<C><<<n_tiles, kS2Threads, 0, s>>>(d_raw0, n_rays, thr, d_thr, K, d_zlut, d_count, d_offset, d_cell, d_ray, \
+                                                        d_z, d_zp, d_total, state, ticket, n_tiles, epoch, base)
+  if (D == 32) ADN_S2_CELLS(1);
+  else if (D == 64) ADN_S2_CELLS(2);
+  else if (D == 256) ADN_S2_CELLS(8);
+#undef ADN_S2_CELLS
+  else if (K <= 8 && aligned)
     stage2_thread_kernel<8><<<n_tiles, kS2Rays, kS2tSmemBytes, s>>>(d_raw0, n_rays, thr, d_thr, K, d_zlut, d_count, d_offset, d_cell,
                                                                    d_ray, d_z, d_zp, d_total, state, ticket, n_tiles, epoch, base);
   else if (K <= 16 && aligned)
@@ -932,6 +1079,65 @@ budget_keys_warp_kernel(const float* __restrict__ raw0, long long n_rays, float 
   budget_flush_hist(s_hist, hist, n_rays);
 }
 
+// budget_keys_warp_kernel over raw0 [n_rays, 32 C] (D != 128), every K: select_cells_c at thr_min, one instance of the
+// largest selected value dropped, the rest the ray's keys.
+template <int C>
+__global__ void __launch_bounds__(kS2Threads)
+budget_keys_cells_kernel(const float* __restrict__ raw0, long long n_rays, float thr_min, int K, uint32_t* __restrict__ keys,
+                         unsigned long long* __restrict__ hist) {
+  constexpr int D = 32 * C;
+  __shared__ uint32_t s_hist[kBudgetBins];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int b = threadIdx.x; b < kBudgetBins; b += kS2Threads) s_hist[b] = 0;
+  __syncthreads();
+  const int KM1 = K - 1;
+  const long long step = (long long)gridDim.x * (kS2Threads / 32);
+  for (long long r = blockIdx.x * (long long)(kS2Threads / 32) + warp; r < n_rays; r += step) {
+    float v[C];
+    ld_row_cells<C>(raw0 + r * D, lane, v);
+    uint32_t sel[C];
+    const int cnt = select_cells_c<C>(v, thr_min, K, lane, sel);
+    bool any = false;
+#pragma unroll
+    for (int j = 0; j < C; ++j) any = any || v[j] >= thr_min;
+    int n_keys = 0;
+    if (__any_sync(0xffffffffu, any)) {
+      uint32_t best = 0u;
+      int bj = 0;
+#pragma unroll
+      for (int j = 0; j < C; ++j) {
+        const uint32_t k = ((sel[j] >> lane) & 1u) ? __float_as_uint(v[j]) : 0u;
+        bj = k > best ? j : bj;
+        best = k > best ? k : best;
+      }
+      const uint32_t m = __reduce_max_sync(0xffffffffu, best);
+      const int who = __ffs(__ballot_sync(0xffffffffu, best == m)) - 1;
+#pragma unroll
+      for (int j = 0; j < C; ++j) {
+        if (lane == who && j == bj) sel[j] &= ~(1u << lane);
+        sel[j] = __shfl_sync(0xffffffffu, sel[j], who);
+      }
+      const uint32_t below = (1u << lane) - 1u;
+      int base = 0;
+#pragma unroll
+      for (int j = 0; j < C; ++j) base += __popc(sel[j] & below);
+#pragma unroll
+      for (int j = 0; j < C; ++j) {
+        if ((sel[j] >> lane) & 1u) {
+          const uint32_t k = __float_as_uint(v[j]);
+          keys[r * KM1 + base] = k;
+          atomicAdd(&s_hist[k >> 21], 1u);
+          ++base;
+        }
+      }
+      n_keys = cnt - 1;
+    }
+    for (int p = n_keys + lane; p < KM1; p += 32) keys[r * KM1 + p] = 0u;
+  }
+  __syncthreads();
+  budget_flush_hist(s_hist, hist, n_rays);
+}
+
 // Rounds 1 and 2 of the select: histogram of the next key bits over the keys that carry the current prefix.
 __global__ void __launch_bounds__(256)
 budget_hist_kernel(const uint32_t* __restrict__ keys, long long n_keys, const BudgetState* __restrict__ st, int round,
@@ -1020,7 +1226,8 @@ budget_select_kernel(const unsigned long long* __restrict__ hist_all, BudgetStat
 
 cudaError_t launch_budget_threshold(const float* d_raw0, long long n_rays, float thr_min, int K, long long max_samples,
                                     uint32_t* d_keys, void* d_work, float* d_thr, int num_sms, cudaStream_t s, int* launches,
-                                    BudgetGroup* group) {
+                                    BudgetGroup* group, int D) {
+  if (D != 32 && D != 64 && D != 128 && D != 256) return cudaErrorInvalidValue;
   unsigned long long* hist = static_cast<unsigned long long*>(d_work);
   BudgetState* st = reinterpret_cast<BudgetState*>(hist + budget_round_offset(3));
   const bool grouped = group && group->fn;
@@ -1040,7 +1247,14 @@ cudaError_t launch_budget_threshold(const float* d_raw0, long long n_rays, float
   const bool select_all = n_keys > 0 || grouped;
   int n = 0;
   if (select_all) {
-    if (K <= 16) {
+    const unsigned warp_grid = unsigned(std::max(1ll, std::min<long long>((n_rays + kS2Threads / 32 - 1) / (kS2Threads / 32), 8ll * num_sms)));
+    if (D == 32) {
+      budget_keys_cells_kernel<1><<<warp_grid, kS2Threads, 0, s>>>(d_raw0, n_rays, thr_min, K, d_keys, hist);
+    } else if (D == 64) {
+      budget_keys_cells_kernel<2><<<warp_grid, kS2Threads, 0, s>>>(d_raw0, n_rays, thr_min, K, d_keys, hist);
+    } else if (D == 256) {
+      budget_keys_cells_kernel<8><<<warp_grid, kS2Threads, 0, s>>>(d_raw0, n_rays, thr_min, K, d_keys, hist);
+    } else if (K <= 16) {
       const long long n_tiles = (n_rays + kS2Rays - 1) / kS2Rays;
       budget_keys_thread_kernel<<<unsigned(std::max(1ll, std::min<long long>(n_tiles, 5ll * num_sms))), kS2Rays, 0, s>>>(
           d_raw0, n_rays, thr_min, K, d_keys, hist);

@@ -64,12 +64,13 @@ struct Stage2Sync {
   uint32_t epoch = 0, ticket_base = 0;
 };
 // d_thr: when non-null the kernel reads the threshold from this device float (a sample-budget threshold) instead of `thr`.
+// D: the depth cells of a raw0 row (multiDepthFeatures: 32, 64, 128 or 256), raw0 [n_rays, D] and d_zlut [D]; 1 <= K <= min(D, 128).
 cudaError_t launch_stage2(const float* d_raw0, long long n_rays, float thr, int K, const float* d_zlut, int32_t* d_count,
                           int32_t* d_offset, int32_t* d_cell, int32_t* d_ray, float* d_z, float* d_zp, long long* d_total,
-                          void* d_scratch, Stage2Sync* sync, cudaStream_t s, const float* d_thr = nullptr);
+                          void* d_scratch, Stage2Sync* sync, cudaStream_t s, const float* d_thr = nullptr, int D = 128);
 
-// Sample budget: writes to *d_thr the smallest threshold t >= thr_min (> 0) at which stage 2 over raw0 [n_rays, 128] with K
-// samples per ray yields at most max_samples (>= n_rays) samples in all.  d_raw0 must be 16-byte aligned.
+// Sample budget: writes to *d_thr the smallest threshold t >= thr_min (> 0) at which stage 2 over raw0 [n_rays, D] with K
+// samples per ray yields at most max_samples (>= n_rays) samples in all.  At D = 128 d_raw0 must be 16-byte aligned.
 // d_keys: [n_rays * (K - 1)] uint32 scratch; d_work: budget_work_bytes() of scratch.  Stream ordered, no host synchronisation; adds its kernel count to *launches.
 //
 // group (may be null, or have a null fn): the call is one member of a budget group.  fn is called on the host once per select
@@ -87,7 +88,7 @@ struct BudgetGroup {
 size_t budget_work_bytes();
 cudaError_t launch_budget_threshold(const float* d_raw0, long long n_rays, float thr_min, int K, long long max_samples,
                                     uint32_t* d_keys, void* d_work, float* d_thr, int num_sms, cudaStream_t s, int* launches,
-                                    BudgetGroup* group = nullptr);
+                                    BudgetGroup* group = nullptr, int D = 128);
 // Dense (thr == 0): count = K, offset = ray*K, total = N*K; no index arrays are materialised.
 cudaError_t launch_stage2_dense(long long n_rays, int K, int32_t* d_count, int32_t* d_offset, long long* d_total,
                                 cudaStream_t s);
@@ -134,7 +135,7 @@ struct Stage5Aux {
   bool any() const { return weights || alpha || z_vals || depth_map || acc_map || disp_map || depth_est; }
 };
 
-// Stage 5.  zp: adaptive -> packed [M]; dense (dense_zp_stride > 0) -> raw0 [N, stride].
+// Stage 5.  zp: adaptive -> packed [M]; dense -> raw0 [N, K] (K = D, one sample per depth cell).
 // d_ray_d non-null: the density composite of the fixed-K sampler (nerf_raw2outputs, src/nerf_raymarch_common.py:19-68)
 // over K samples per ray at offset r K: alpha = 1 - exp(-relu(a) dist), dist = (z[k+1] - z[k], last 1e10) * |ray_d [N,3]|;
 // d_zp, d_offset, d_count and dense are not read, and z_vals is z unchanged.

@@ -223,6 +223,7 @@ def write_export_dir(path, scene, sd0, sd1, thr, K, sampler="FromClassifiedDepth
     import os
     os.makedirs(path, exist_ok=True)
     (d0, w0, _), (d1, w1, skip) = net_shapes(sd0, sd1)
+    cells = int(sd0[f"layers.{d0 - 1}.weight"].shape[0])   # multiDepthFeatures: the sampling net's output width
     as_np = lambda sd: {k: (v.detach().cpu().numpy() if hasattr(v, "detach") else np.asarray(v)) for k, v in sd.items()}
     write_onnx_initializers(os.path.join(path, "model0.onnx"), as_np(sd0))
     write_onnx_initializers(os.path.join(path, "model1.onnx"), as_np(sd1))
@@ -242,13 +243,13 @@ def write_export_dir(path, scene, sd0, sd1, thr, K, sampler="FromClassifiedDepth
                     "outFeatures = [RawSigmoid, RGBARayMarch]\nrayMarchSampler = [none, FromClassifiedDepthAdaptiveNoDepthRange]\n"
                     "rayMarchNormalization = [InverseSqrtDistCentered, None]\nuseNDC = True\n"
                     f"numRaymarchSamples = [{K}, {K}]\ndepthTransform = linear\nzNear = [0.001, 0.001]\nzFar = [1.0, 1.0]\n"
-                    f"adaptiveSamplingThreshold = {thr}\nmultiDepthFeatures = [128, 128]\naccumulationMult = alpha\n")
+                    f"adaptiveSamplingThreshold = {thr}\nmultiDepthFeatures = [{cells}, {cells}]\naccumulationMult = alpha\n")
         else:
             f.write("inFeatures = [SpherePosDir, RayMarchFromPoses]\n"
                     f"outFeatures = [RawSigmoid, RGBARayMarch]\nrayMarchSampler = [none, {sampler}]\n"
                     "rayMarchNormalization = [InverseSqrtDistCentered, InverseSqrtDistCentered]\n"
                     f"numRaymarchSamples = [{K}, {K}]\ndepthTransform = log\nzNear = [0.001, 0.001]\nzFar = [1.0, 1.0]\n"
-                    f"adaptiveSamplingThreshold = {thr}\nmultiDepthFeatures = [128, 128]\naccumulationMult = alpha\n")
+                    f"adaptiveSamplingThreshold = {thr}\nmultiDepthFeatures = [{cells}, {cells}]\naccumulationMult = alpha\n")
             if sampler == "FromClassifiedDepth":
                 f.write(f"losses = [{sampling_loss}, MSE]\n")
         f.write(f"activation = [relu, nerf]\nlayers = [{d0}, {d1}]\nlayerWidth = [{w0}, {w1}]\nskips = [, {_skips_entry(d1, skip)}]\n")

@@ -175,6 +175,14 @@ class Renderer:
         self._check(self.lib.adn_net_dims(self.handle, int(net_id), C.byref(n_in), C.byref(n_out)))
         return n_in.value, n_out.value
 
+    def depth_cells(self):
+        """D, the depth cells the sampling net classifies (multiDepthFeatures: 32, 64, 128 or 256): its output width, the
+        row width of raw0 / oracle_weights.  128 while no sampling net is set."""
+        try:
+            return self.net_dims(0)[1]
+        except AdnError:
+            return 128
+
     def net_shape(self, net_id):
         """(depth, width, skip) the library inferred from the weights of network net_id; skip = -1 when it has none."""
         d, w, s = C.c_int(), C.c_int(), C.c_int()
@@ -228,7 +236,7 @@ class Renderer:
 
     def render_rays(self, pose, rot, dirs, thr, K, want_nsamples=True, want_oracle_weights=False, want_aux=False, out=None,
                     aux_out=None):
-        """dirs [N,3] (cuda tensor) -> dict(rgb [N,3], n_samples [N] int32, oracle_weights [N,128]).
+        """dirs [N,3] (cuda tensor) -> dict(rgb [N,3], n_samples [N] int32, oracle_weights [N,D]; D = depth_cells()).
         want_aux: True or an iterable of AUX_KEYS -> additionally weights / alpha / z_vals [N,K] and depth_map /
         acc_map / disp_map / depth_est [N] (adaptive_raw2outputs' other outputs, src/nerf_raymarch_common.py:137-144;
         depth_est = "NeRFOutputDepth", src/features.py:574-577).  aux_out: dict of contiguous float32 tensors on the
@@ -251,7 +259,7 @@ class Renderer:
             raise ValueError(f"{who}: out must be a contiguous float32 [N,3] tensor on the renderer's device")
         rgb = out if out is not None else torch.empty((n, 3), dtype=torch.float32, device=self._dev())
         ns = torch.empty((n,), dtype=torch.int32, device=self._dev()) if want_nsamples else None
-        ow = torch.empty((n, 128), dtype=torch.float32, device=self._dev()) if want_oracle_weights else None
+        ow = torch.empty((n, self.depth_cells()), dtype=torch.float32, device=self._dev()) if want_oracle_weights else None
         out = dict(rgb=rgb, n_samples=ns, oracle_weights=ow)
         aux = None
         if want_aux:
@@ -455,7 +463,10 @@ class Renderer:
         return out
 
     def stage2(self, raw0, thr, K):
+        """Stage 2 alone (adn_stage2_sample): raw0 [N,D] (D = depth_cells()) -> the packed selection."""
         x = self._f32(raw0)
+        if x.dim() != 2 or x.shape[1] != self.depth_cells():
+            raise ValueError(f"stage2: raw0 must be [N, {self.depth_cells()}] (the sampling net's depth cells), got {tuple(x.shape)}")
         n = x.shape[0]
         dev = self._dev()
         count = torch.empty((n,), dtype=torch.int32, device=dev)
@@ -537,9 +548,11 @@ class Renderer:
         return z
 
     def budget_threshold(self, raw0, thr_min, K, max_samples, out=None):
-        """raw0 [N,128] -> [1] float32 device tensor: the smallest threshold >= thr_min at which stage 2 with K samples per
+        """raw0 [N,D] (D = depth_cells()) -> [1] float32 device tensor: the smallest threshold >= thr_min at which stage 2 with K samples per
         ray yields at most max_samples samples (the selection a "sample_budget" render makes).  Stream ordered, no sync."""
         x = self._f32(raw0)
+        if x.dim() != 2 or x.shape[1] != self.depth_cells():
+            raise ValueError(f"budget_threshold: raw0 must be [N, {self.depth_cells()}] (the sampling net's depth cells), got {tuple(x.shape)}")
         t = out if out is not None else torch.empty((1,), dtype=torch.float32, device=self._dev())
         self._check(self.lib.adn_budget_threshold(self.handle, x.data_ptr(), x.shape[0], float(thr_min), int(K), int(max_samples),
                                                   t.data_ptr(), self._stream()))
@@ -582,8 +595,8 @@ class Renderer:
 
     def stage5(self, raw1, zp, z, offset, count, K, want_aux=True, aux=None, dense=False, rgba8=False, out=None):
         """Stage 5 alone (adn_stage5_composite_aux) -> dict(rgb [N,3], rgba8 [N,4] uint8, and each requested aux output).
-        want_aux: weights and depth_map (aux=None only).  aux: True or an iterable of AUX_KEYS.  dense: zp is raw0 [N,128]
-        and z / offset / count may be None (K must be 128).  out: dict of tensors to write into instead of new ones (keys
+        want_aux: weights and depth_map (aux=None only).  aux: True or an iterable of AUX_KEYS.  dense: zp is raw0 [N,K]
+        and z / offset / count may be None (K must be 128 or depth_cells()).  out: dict of tensors to write into instead of new ones (keys
         "rgb", "rgba8" and AUX_KEYS; each one given is also requested) -- slots the kernel does not write keep their
         contents."""
         dev = self._dev()

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-/* d_dirs [V N,3] camera-space directions, n_per_view = N; d_rgb [V N,3], d_nsamples [V N], d_oracle_weights [V N,128] and
+/* d_dirs [V N,3] camera-space directions, n_per_view = N; d_rgb [V N,3], d_nsamples [V N], d_oracle_weights [V N,D] and
  * aux ([V N,K] / [V N]; aux may be NULL) as adn_render_rays_aux. */
 adn_status adn_render_views_rays(adn_ctx* ctx, int n_views, const float* poses, const float* rots, const float* d_dirs,
                                  int64_t n_per_view, float thr, int K, float* d_rgb, int32_t* d_nsamples,
